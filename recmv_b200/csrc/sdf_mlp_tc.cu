@@ -8,13 +8,14 @@
 //  * tensor cores: wgmma.mma_async m64n128k16 (fp16 inputs, fp32 accumulators in registers).  Two consumer warpgroups
 //    each own half of a layer's 512 outputs (two 128-column accumulators, 128 registers per thread).  fp32 parity mode
 //    (passes = 3): operands are split a = hi + lo in fp16 and every product is 3 MMAs (hi*hi + lo*hi + hi*lo).
-//  * weights: fp16 hi/lo panels streamed by TMA (128-byte swizzle) from L2 through a 5-slot x 16 KB ring of
-//    [128 outputs x 64 inputs] boxes, signalled with mbarrier complete_tx; a warpgroup releases a slot once the MMAs
-//    that read it have completed.
+//  * weights: fp16 hi/lo panels streamed by TMA from L2, one ring per warpgroup of 5 slots x 8 KB, each slot one
+//    [128 outputs x 32 inputs] half of a [128 x 64] weight box (64-byte swizzle), signalled with mbarrier complete_tx; a
+//    warpgroup releases a slot as soon as the wgmma commit group that last reads it has retired.
 //  * activations: 64 x 512 fp16 hi + lo (128 KB) in shared memory in the K-major SW128 layout, rewritten IN PLACE by
 //    the epilogue of the warpgroups once both have finished the layer's MMAs (two named barriers per layer).
-//  * warp roles (11 warps): 0-7 the two MMA / epilogue warpgroups; 8 TMA producer; 9-10 prologue for the NEXT tile
-//    (point fetch / inverse LBS / PE, or the input rows of the translator / colour networks).
+//  * warp roles (12 warps): 0-7 the two MMA / epilogue warpgroups; 8, 9 TMA producers (ring of warpgroup 0, 1);
+//    10-11 prologue for the NEXT tile (point fetch / inverse LBS / PE, or the input rows of the translator / colour
+//    networks).
 //  * the same engine runs three networks (Net<0> SDF, Net<1> translator + LBS, Net<2> colour) and a forward-mode
 //    (value + tangents, 4 rows per point) variant of the first two.
 // Every mbarrier wait is bounded: a protocol bug surfaces as a status code, not a hung GPU.
@@ -28,29 +29,32 @@ using namespace tc;
 namespace {
 
 constexpr int kMmaWarps = 8;                      // two warpgroups
-constexpr int kProducerWarp = kMmaWarps;          // warp 8
-constexpr int kPrologueWarps = 2;                 // warps 9, 10: one thread per tile row
-constexpr int kThreads = 32 * (kMmaWarps + 1 + kPrologueWarps);
+constexpr int kProducerWarp = kMmaWarps;          // warps 8, 9: TMA producer of the weight ring of warpgroup 0, 1
+constexpr int kPrologueWarp = kProducerWarp + 2;  // warps 10, 11: one thread per tile row
+constexpr int kPrologueWarps = 2;
+constexpr int kThreads = 32 * (kPrologueWarp + kPrologueWarps);   // 12 warps = three whole warpgroups
 constexpr int kRowsPerCta = 64;
 #ifndef RECMV_TC_TWO_SWEEPS
 #define RECMV_TC_TWO_SWEEPS 1   // last layer, parity mode: correction MMAs first, hi*hi MMAs in a second sweep
 #endif
 constexpr bool kTwoSweeps = RECMV_TC_TWO_SWEEPS != 0;
-constexpr int kSlots = 5;
-constexpr uint32_t kSlotBytes = 16384;            // [128 outputs][64 inputs] fp16
+// One weight ring per warpgroup.  A slot holds a [128 outputs x 32 inputs] half of a weight box (64-byte swizzle), so a
+// box = two consecutive slots; 5 slots let a warpgroup keep two half-boxes in flight beyond the three its MMAs may hold.
+constexpr int kSlots = 5;                         // per ring
+constexpr uint32_t kSlotBytes = 8192;             // [128 outputs][32 inputs] fp16
 // shared memory map (offsets from a 1024-aligned base)
 constexpr uint32_t kOffAHi = 0;
 constexpr uint32_t kOffALo = 65536;
 constexpr uint32_t kOffPeHi = 131072;
 constexpr uint32_t kOffPeLo = 139264;
-constexpr uint32_t kOffW = 147456;
-constexpr uint32_t kOffBar = kOffW + kSlots * kSlotBytes;  // 229376
+constexpr uint32_t kOffW = 147456;                         // ring g at kOffW + g * kSlots * kSlotBytes
+constexpr uint32_t kOffBar = kOffW + 2 * kSlots * kSlotBytes;  // 229376
 // barrier indices (8 bytes each)
-constexpr int kBarFull = 0;      // [5] weight slot filled (1 arming arrival + tx bytes)
-constexpr int kBarEmpty = 5;     // [5] slot consumed (one arrival by the warpgroup that used it)
-constexpr int kBarPeReady = 10;  //     tile input written by the prologue warps (one arrival per warp)
-constexpr int kBarPeFree = 11;   //     the MMAs of layer kInFreeLayer are done with the tile input (one arrival per warpgroup)
-constexpr int kNumBars = 12;
+constexpr int kBarFull = 0;      // [2][5] weight slot filled (1 arming arrival + tx bytes)
+constexpr int kBarEmpty = 10;    // [2][5] slot consumed (one arrival by the ring's warpgroup)
+constexpr int kBarPeReady = 20;  //       tile input written by the prologue warps (one arrival per warp)
+constexpr int kBarPeFree = 21;   //       the MMAs of layer kInFreeLayer are done with the tile input (one arrival per warpgroup)
+constexpr int kNumBars = 22;
 constexpr int kBarConsumers = 1; // named barrier of the 256 MMA threads
 constexpr uint32_t kOffMisc = kOffBar + kNumBars * 8;  // abort flag, valid flags
 constexpr uint32_t kSmemBytes = kOffMisc + 16 + 128 + 1024 /*alignment slack*/;
@@ -163,38 +167,54 @@ template <> struct Net<2> {
   __device__ static int ntiles(int l) { return l == 4 ? 1 : 4; }
 };
 
-// The MMAs of one weight slot (one K block x one 128-wide output tile x one weight plane) into accumulator `acc`.
-//   passes 1:                  a_hi . w_hi
-//   passes 3, one sweep:       plane 0: a_hi . w_hi + a_lo . w_hi;  plane 1: a_hi . w_lo
-//   passes 3, two sweeps:      sweep 0 plane 0: a_lo . w_hi;  plane 1: a_hi . w_lo;  sweep 1: a_hi . w_hi
-// (last layer, parity mode: the tensor core accumulates with truncation, so every MMA added to a LARGE accumulator costs
-// ~1 ulp of it; the correction products are 2^-11 of the result and issued first, while the accumulator is still tiny.)
-__device__ __forceinline__ void slot_mmas(float (&acc)[64], uint64_t a_hi, uint64_t a_lo, uint64_t b, int passes,
-                                          bool two_sweeps, int sweep, int plane, bool first) {
+// The MMAs of one weight box (one 64-wide K block x one 128-wide output tile x one weight plane) into accumulator `acc`.
+// The box arrives as two ring slots, b0 = inputs 0..31 and b1 = inputs 32..63 (K steps 0, 1 and 2, 3), and its MMAs
+// form two commit groups: the first is the last to read b0, the second reads b1 only, so b0 is released one group
+// before b1.  Straight-line code with a fixed accumulator: wgmma.fence ... commit holds no branch, which lets ptxas keep
+// the MMAs in flight instead of serialising them.  Per accumulator element the order of the products is
+//   box_mmas:        a . w            K steps 0..3        (tc1; parity mode: the w_lo box and every two-sweep box)
+//   box_mmas_hi_lo:  a_hi . w_hi      K steps 0..3, then a_lo . w_hi K steps 0..3      (parity mode, the w_hi box)
+// Parity mode, last layer (two sweeps): sweep 0 plane 0: a_lo . w_hi;  plane 1: a_hi . w_lo;  sweep 1: a_hi . w_hi (the
+// tensor core accumulates with truncation, so every MMA added to a LARGE accumulator costs ~1 ulp of it; the correction
+// products are 2^-11 of the result and issued first, while the accumulator is still tiny.)
+// scale0 = 0: the first MMA overwrites the accumulator.
+__device__ __forceinline__ void box_mmas(float (&acc)[64], uint64_t a, uint64_t b0, uint64_t b1, uint32_t scale0) {
   wg_fence();
-  if (two_sweeps) {
-    const uint64_t a = (sweep == 0 && plane == 0) ? a_lo : a_hi;
-#pragma unroll
-    for (int k = 0; k < 4; ++k) wgmma_n128<0, 0>(acc, a + 2 * k, b + 2 * k, (first && k == 0) ? 0u : 1u);
-  } else {
-#pragma unroll
-    for (int k = 0; k < 4; ++k) wgmma_n128<0, 0>(acc, a_hi + 2 * k, b + 2 * k, (first && k == 0) ? 0u : 1u);
-    if (passes == 3 && plane == 0) {
-#pragma unroll
-      for (int k = 0; k < 4; ++k) wgmma_n128<0, 0>(acc, a_lo + 2 * k, b + 2 * k, 1u);
-    }
-  }
+  wgmma_n128<0, 0>(acc, a, b0, scale0);
+  wgmma_n128<0, 0>(acc, a + 2, b0 + 2, 1u);
+  wg_commit();
+  wgmma_n128<0, 0>(acc, a + 4, b1, 1u);
+  wgmma_n128<0, 0>(acc, a + 6, b1 + 2, 1u);
+  wg_commit();
+}
+__device__ __forceinline__ void box_mmas_hi_lo(float (&acc)[64], uint64_t a_hi, uint64_t a_lo, uint64_t b0, uint64_t b1,
+                                               uint32_t scale0) {
+  wg_fence();
+  wgmma_n128<0, 0>(acc, a_hi, b0, scale0);
+  wgmma_n128<0, 0>(acc, a_hi + 2, b0 + 2, 1u);
+  wgmma_n128<0, 0>(acc, a_hi + 4, b1, 1u);
+  wgmma_n128<0, 0>(acc, a_hi + 6, b1 + 2, 1u);
+  wgmma_n128<0, 0>(acc, a_lo, b0, 1u);
+  wgmma_n128<0, 0>(acc, a_lo + 2, b0 + 2, 1u);
+  wg_commit();
+  wgmma_n128<0, 0>(acc, a_lo + 4, b1, 1u);
+  wgmma_n128<0, 0>(acc, a_lo + 6, b1 + 2, 1u);
   wg_commit();
 }
 
+// output tiles of a layer with T tiles that warpgroup g owns (tiles 2 g, 2 g + 1): 0, 1 or 2
+__device__ __forceinline__ int own_tiles(int T, int g) { return min(max(T - 2 * g, 0), 2); }
+
 }  // namespace
 
-template <bool kJvp, int kNet>
+// kPasses: 3 = parity mode (hi * hi + lo * hi + hi * lo), 1 = hi * hi only (TcParams::passes must agree)
+template <bool kJvp, int kNet, int kPasses>
 __global__ void __launch_bounds__(kThreads, 1)
-sdf_tc_kernel(const __grid_constant__ CUtensorMap tmap128, const TcParams prm) {
+sdf_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams prm) {
   using NetT = Net<kNet>;
   constexpr int kNumLayers = NetT::kLayers;   // shadows the SDF constant of common.cuh
   static_assert(!kJvp || kNet == 0 || kNet == 1, "the forward-mode variant exists for the SDF network and the deformer");
+  static_assert(kPasses == 1 || kPasses == 3, "precision mode");
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* gbase = smem_raw + (base - smem_u32(smem_raw));
@@ -210,40 +230,47 @@ sdf_tc_kernel(const __grid_constant__ CUtensorMap tmap128, const TcParams prm) {
   const long long num_tiles = (Ptot + kPtsPerTile - 1) / kPtsPerTile;
   const long long n_iter = (long long)blockIdx.x < num_tiles ? (num_tiles - 1 - blockIdx.x) / gridDim.x + 1 : 0;
   auto tile_of = [&](long long it) { return (long long)blockIdx.x + it * gridDim.x; };
-  const int passes = prm.passes;
   auto BAR = [&](int i) { return bar0 + 8u * (uint32_t)i; };
-  auto SLOT = [&](int s) { return base + kOffW + (uint32_t)s * kSlotBytes; };
+  // slot s of the weight ring of warpgroup g, its full / empty barriers
+  auto SLOT = [&](int g, int s) { return base + kOffW + (uint32_t)(g * kSlots + s) * kSlotBytes; };
+  auto FULL = [&](int g, int s) { return BAR(kBarFull + g * kSlots + s); };
+  auto EMPTY = [&](int g, int s) { return BAR(kBarEmpty + g * kSlots + s); };
 
   if (threadIdx.x == 0) {
     *abort_flag = 0;
-    for (int s = 0; s < kSlots; ++s) { mbar_init(BAR(kBarFull + s), 1); mbar_init(BAR(kBarEmpty + s), 1); }
+    for (int s = 0; s < 2 * kSlots; ++s) { mbar_init(BAR(kBarFull + s), 1); mbar_init(BAR(kBarEmpty + s), 1); }
     mbar_init(BAR(kBarPeReady), kPrologueWarps);
     mbar_init(BAR(kBarPeFree), 2);
     fence_mbar_init();
   }
-  if (warp == kProducerWarp && lane == 0) prefetch_tmap(&tmap128);
+  if (warp >= kProducerWarp && warp < kPrologueWarp && lane == 0) prefetch_tmap(&tmap);
   __syncthreads();
 
-  if (warp == kProducerWarp) {
-    // ============== TMA producer: the weight boxes of every layer, in the order the warpgroups consume them ==============
+  if (warp >= kProducerWarp && warp < kPrologueWarp) {
+    // ====== TMA producers: warp 8 + g streams the weight boxes of warpgroup g, in the order that warpgroup consumes them ======
+    const int g = warp - kProducerWarp;
     if (lane == 0) {
-      long long u = 0;   // slot use counter
+      int slot = 0;
+      uint32_t phase = 0;   // parity of the ring's current pass
       for (long long it = 0; it < n_iter; ++it) {
         for (int l = 0; l < kNumLayers; ++l) {
-          const int nkb = NetT::nkb(l), T = NetT::ntiles(l);
+          const int nkb = NetT::nkb(l), nt_own = own_tiles(NetT::ntiles(l), g);
           // last layer, parity mode: sweep 0 streams (w_hi, w_lo) for the correction MMAs, sweep 1 streams w_hi again
-          const int nsweep = (kTwoSweeps && passes == 3 && l == kNumLayers - 1) ? 2 : 1;
+          const int nsweep = (kTwoSweeps && kPasses == 3 && l == kNumLayers - 1) ? 2 : 1;
           for (int sweep = 0; sweep < nsweep; ++sweep) {
-            const int nplanes = (passes == 3 && sweep == 0) ? 2 : 1;
+            const int nplanes = (kPasses == 3 && sweep == 0) ? 2 : 1;
             for (int i = 0; i < nkb; ++i) {
               const int kbi = NetT::kb_at(l, i);
               const int panel = NetT::pbase(l) + (kbi == 8 ? nkb - 1 : kbi);   // the PE block is the layer's last panel
-              for (int nt = 0; nt < T; ++nt) {
-                for (int plane = 0; plane < nplanes; ++plane, ++u) {
-                  const int slot = (int)(u % kSlots);
-                  mbar_wait(BAR(kBarEmpty + slot), (uint32_t)(((u / kSlots) & 1) ^ 1), abort_flag, prm.status, 100 + slot);
-                  mbar_expect_tx_local(BAR(kBarFull + slot), kSlotBytes);
-                  tma_load_2d(SLOT(slot), &tmap128, BAR(kBarFull + slot), 0, (plane * NetT::kPanels + panel) * 512 + nt * 128);
+              for (int t = 0; t < nt_own; ++t) {
+                for (int plane = 0; plane < nplanes; ++plane) {
+                  for (int half = 0; half < 2; ++half) {
+                    mbar_wait(EMPTY(g, slot), phase ^ 1u, abort_flag, prm.status, 100 + g * kSlots + slot);
+                    mbar_expect_tx_local(FULL(g, slot), kSlotBytes);
+                    tma_load_2d(SLOT(g, slot), &tmap, FULL(g, slot), 32 * half,
+                                (plane * NetT::kPanels + panel) * 512 + (2 * g + t) * 128);
+                    if (++slot == kSlots) { slot = 0; phase ^= 1u; }
+                  }
                 }
               }
             }
@@ -258,54 +285,86 @@ sdf_tc_kernel(const __grid_constant__ CUtensorMap tmap128, const TcParams prm) {
     const int c = lane & 3;                        // column pair of the fragment
     const int comp = kJvp ? ((lane >> 2) & 3) : 0; // JVP: 0 = value row, 1..3 = tangent rows (same for both fragment rows)
     const bool is_value = comp == 0;
-    float acc0[64], acc1[64];
+    float acc[2][64];   // output tiles 2 g and 2 g + 1
 #pragma unroll
-    for (int i = 0; i < 64; ++i) { acc0[i] = 0.f; acc1[i] = 0.f; }
-    long long u = 0;   // slot use counter (producer order)
+    for (int i = 0; i < 64; ++i) { acc[0][i] = 0.f; acc[1][i] = 0.f; }
+    // this warpgroup's ring: next slot to consume, parity of its pass, and the slot its in-flight MMAs still read
+    int slot = 0, held = -1, s0 = 0, s1 = 0;
+    uint32_t phase = 0;
+    // wait for the next box (two slots) and return its B descriptors
+    auto acquire = [&](uint64_t& b0, uint64_t& b1) {
+      s0 = slot;
+      mbar_wait(FULL(g, slot), phase, abort_flag, prm.status, 230 + g * kSlots + slot);
+      if (++slot == kSlots) { slot = 0; phase ^= 1u; }
+      s1 = slot;
+      mbar_wait(FULL(g, slot), phase, abort_flag, prm.status, 230 + g * kSlots + slot);
+      if (++slot == kSlots) { slot = 0; phase ^= 1u; }
+      b0 = smem_desc_sw64(SLOT(g, s0));
+      b1 = smem_desc_sw64(SLOT(g, s1));
+    };
+    // once the box's first commit group has retired: release its first half and the previous box's second half (whose
+    // group retired before it); the second half stays held until the next box's first group has retired
+    auto retire = [&]() {
+      wg_wait<1>();
+      if (signaller) {
+        if (held >= 0) mbar_arrive_local(EMPTY(g, held));
+        mbar_arrive_local(EMPTY(g, s0));
+      }
+      held = s1;
+    };
     for (long long it = 0; it < n_iter; ++it) {
       const long long tile = tile_of(it);
       for (int l = 0; l < kNumLayers; ++l) {
         if (l == 0) mbar_wait(BAR(kBarPeReady), (uint32_t)(it & 1), abort_flag, prm.status, 220);
-        const int nkb = NetT::nkb(l), T = NetT::ntiles(l);
+        const int nkb = NetT::nkb(l), T = NetT::ntiles(l), nt_own = own_tiles(T, g);
         const bool hidden = l < kNumLayers - 1;
-        const bool two_sweeps = kTwoSweeps && passes == 3 && l == kNumLayers - 1;
-        int pending = -1;        // slot whose MMAs may still be running (released one step later)
-        long long pending_u = 0;
+        const bool two_sweeps = kTwoSweeps && kPasses == 3 && l == kNumLayers - 1;
+        // the layer's first MMA overwrites the accumulators; zeroing them here tells the compiler that the previous
+        // layer's values are dead once its epilogue has read them
+#pragma unroll
+        for (int i = 0; i < 64; ++i) { acc[0][i] = 0.f; acc[1][i] = 0.f; }
         for (int sweep = 0; sweep < (two_sweeps ? 2 : 1); ++sweep) {
-          const int nplanes = (passes == 3 && sweep == 0) ? 2 : 1;
           for (int i = 0; i < nkb; ++i) {
             const int kbi = NetT::kb_at(l, i);
             const bool is_pe = kbi == 8;
             const uint64_t a_hi = smem_desc_sw128(is_pe ? base + kOffPeHi : base + kOffAHi + kbi * 8192);
             const uint64_t a_lo = smem_desc_sw128(is_pe ? base + kOffPeLo : base + kOffALo + kbi * 8192);
-            for (int nt = 0; nt < T; ++nt) {
-              for (int plane = 0; plane < nplanes; ++plane, ++u) {
-                if ((nt >> 1) != g) continue;   // the other warpgroup's box
-                const int slot = (int)(u % kSlots);
-                // the producer refills use u only after use u - kSlots was released: if that is the slot this warpgroup
-                // still holds, retire it first (the two warpgroups consume interleaved blocks of the ring)
-                if (pending >= 0 && u - pending_u >= kSlots) {
-                  wg_wait<0>();
-                  if (signaller) mbar_arrive_local(BAR(kBarEmpty + pending));
-                  pending = -1;
-                }
-                mbar_wait(BAR(kBarFull + slot), (uint32_t)((u / kSlots) & 1), abort_flag, prm.status, 230 + slot);
-                const uint64_t b = smem_desc_sw128(SLOT(slot));
-                const bool first = sweep == 0 && i == 0 && plane == 0;
-                if (nt & 1) slot_mmas(acc1, a_hi, a_lo, b, passes, two_sweeps, sweep, plane, first);
-                else slot_mmas(acc0, a_hi, a_lo, b, passes, two_sweeps, sweep, plane, first);
-                wg_wait<1>();
-                if (pending >= 0 && signaller) mbar_arrive_local(BAR(kBarEmpty + pending));
-                pending = slot;
-                pending_u = u;
+            const uint32_t scale0 = (sweep == 0 && i == 0) ? 0u : 1u;   // the layer's first MMA overwrites
+#pragma unroll
+            for (int t = 0; t < 2; ++t) {
+              if (t >= nt_own) continue;   // warpgroup-uniform: a tile this warpgroup does not own in this layer
+              uint64_t b0, b1;
+              if (kPasses == 1) {
+                acquire(b0, b1);
+                box_mmas(acc[t], a_hi, b0, b1, scale0);
+                retire();
+              } else if (!two_sweeps) {
+                acquire(b0, b1);                                   // w_hi
+                box_mmas_hi_lo(acc[t], a_hi, a_lo, b0, b1, scale0);
+                retire();
+                acquire(b0, b1);                                   // w_lo
+                box_mmas(acc[t], a_hi, b0, b1, 1u);
+                retire();
+              } else if (sweep == 0) {
+                acquire(b0, b1);                                   // w_hi: a_lo . w_hi
+                box_mmas(acc[t], a_lo, b0, b1, scale0);
+                retire();
+                acquire(b0, b1);                                   // w_lo: a_hi . w_lo
+                box_mmas(acc[t], a_hi, b0, b1, 1u);
+                retire();
+              } else {
+                acquire(b0, b1);                                   // w_hi: a_hi . w_hi
+                box_mmas(acc[t], a_hi, b0, b1, 1u);
+                retire();
               }
             }
           }
         }
         wg_wait<0>();
-        wg_fence_regs(acc0);
-        wg_fence_regs(acc1);
-        if (pending >= 0 && signaller) mbar_arrive_local(BAR(kBarEmpty + pending));
+        wg_fence_regs(acc[0]);
+        wg_fence_regs(acc[1]);
+        if (held >= 0 && signaller) mbar_arrive_local(EMPTY(g, held));
+        held = -1;
         if (l == NetT::kInFreeLayer && signaller) mbar_arrive_local(BAR(kBarPeFree));   // prologue may refill its block
 
         const float* bias = prm.bias + l * 512;
@@ -319,14 +378,16 @@ sdf_tc_kernel(const __grid_constant__ CUtensorMap tmap128, const TcParams prm) {
 #pragma unroll
           for (int t = 0; t < 2; ++t) {
             const int f_base = (2 * g + t) * 128 + 2 * c;
+            // column pair j outer, fragment row h inner: each bias pair is used as soon as it is loaded (the other order
+            // keeps a tile's 16 bias pairs live next to the 128 accumulator registers)
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              const int row = 16 * wq + (lane >> 2) + 8 * h;
+            for (int j = 0; j < 16; ++j) {
+              const int f = f_base + 8 * j;
 #pragma unroll
-              for (int j = 0; j < 16; ++j) {
-                const int f = f_base + 8 * j;
-                const float r0 = t ? acc1[4 * j + 2 * h] : acc0[4 * j + 2 * h];
-                const float r1 = t ? acc1[4 * j + 2 * h + 1] : acc0[4 * j + 2 * h + 1];
+              for (int h = 0; h < 2; ++h) {
+                const int row = 16 * wq + (lane >> 2) + 8 * h;
+                const float r0 = acc[t][4 * j + 2 * h];
+                const float r1 = acc[t][4 * j + 2 * h + 1];
                 if (prm.dbg_out && prm.dbg_layer == l && tile == 0) {
                   prm.dbg_out[row * 512 + f] = r0 * kAccUnscale;
                   prm.dbg_out[row * 512 + f + 1] = r1 * kAccUnscale;
@@ -352,7 +413,7 @@ sdf_tc_kernel(const __grid_constant__ CUtensorMap tmap128, const TcParams prm) {
                 split2(v0, v1, hi, lo);
                 const uint32_t off = (uint32_t)(f >> 6) * 8192u + sw128_elem(row, f & 63);
                 st_shared_b32(base + kOffAHi + off, hi);
-                if (passes == 3) st_shared_b32(base + kOffALo + off, lo);
+                if (kPasses == 3) st_shared_b32(base + kOffALo + off, lo);
               }
             }
           }
@@ -375,7 +436,7 @@ sdf_tc_kernel(const __grid_constant__ CUtensorMap tmap128, const TcParams prm) {
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
                   const int f = (2 * g + t) * 128 + 8 * j + 2 * c + e;
-                  const float r = t ? acc1[4 * j + 2 * h + e] : acc0[4 * j + 2 * h + e];
+                  const float r = acc[t][4 * j + 2 * h + e];
                   if (prm.dbg_out && prm.dbg_layer == l && tile == 0) prm.dbg_out[row * 512 + f] = r * kAccUnscale;
                   // column 0 = sdf, columns 1..256 = features
                   if (kJvp && !is_value) {
@@ -395,13 +456,13 @@ sdf_tc_kernel(const __grid_constant__ CUtensorMap tmap128, const TcParams prm) {
               for (int e = 0; e < 2; ++e) {
                 const int f0 = 2 * c + e, f1 = 8 + 2 * c + e;
                 (void)f1;
-                if (f0 < 3) prm.out_rgb[3 * p + f0] = tanhf(fmaf(acc0[2 * h + e], acc_unscale, __ldg(bias + f0)));
+                if (f0 < 3) prm.out_rgb[3 * p + f0] = tanhf(fmaf(acc[0][2 * h + e], acc_unscale, __ldg(bias + f0)));
               }
             }
           } else if (g == 0) {
             // deformer: columns 0..2 = offset; out = p + offset, then LBS forward.  Columns 0, 1 live in lane 4 r, column 2
             // in lane 4 r + 1 of the fragment row: gather them (warp-uniform shuffles)
-            const float own0 = acc0[2 * h] * acc_unscale, own1 = acc0[2 * h + 1] * acc_unscale;
+            const float own0 = acc[0][2 * h] * acc_unscale, own1 = acc[0][2 * h + 1] * acc_unscale;
             const float v[3] = {__shfl_sync(0xffffffffu, own0, lane & ~3), __shfl_sync(0xffffffffu, own1, lane & ~3),
                                 __shfl_sync(0xffffffffu, own0, (lane & ~3) + 1)};
             if (kJvp) {
@@ -460,7 +521,7 @@ sdf_tc_kernel(const __grid_constant__ CUtensorMap tmap128, const TcParams prm) {
     }
   } else {
     // ================================ prologue for the next tile ========================
-    const int row = (warp - kProducerWarp - 1) * 32 + lane;
+    const int row = (warp - kPrologueWarp) * 32 + lane;
     for (long long it = 0; it < n_iter; ++it) {
       const long long tile = tile_of(it);
       const long long p = kJvp ? tile * kPtsPerTile + (row >> 2) : tile * kPtsPerTile + row;
@@ -507,7 +568,7 @@ sdf_tc_kernel(const __grid_constant__ CUtensorMap tmap128, const TcParams prm) {
           split8(v, hi, lo);
           const uint32_t off = (uint32_t)(chunk >> 3) * 8192u + sw128_offset(row, chunk & 7);
           st_shared_v4(base + kOffAHi + off, hi);
-          if (passes == 3) st_shared_v4(base + kOffALo + off, lo);
+          if (kPasses == 3) st_shared_v4(base + kOffALo + off, lo);
         }
       } else if (kNet == 1) {
         // deformer input row: [PE(p) (39) | cond[frame] (128) | 0 (25)] = three 64-wide K blocks written into the
@@ -541,7 +602,7 @@ sdf_tc_kernel(const __grid_constant__ CUtensorMap tmap128, const TcParams prm) {
           split8(head + 8 * chunk, hi, lo);
           const uint32_t off = sw128_offset(row, chunk);
           st_shared_v4(base + kOffAHi + off, hi);
-          if (passes == 3) st_shared_v4(base + kOffALo + off, lo);
+          if (kPasses == 3) st_shared_v4(base + kOffALo + off, lo);
         }
 #pragma unroll 1
         for (int chunk = 5; chunk < 24; ++chunk) {         // columns 40..191: cond[1..127] then zeros
@@ -556,7 +617,7 @@ sdf_tc_kernel(const __grid_constant__ CUtensorMap tmap128, const TcParams prm) {
           split8(v, hi, lo);
           const uint32_t off = (uint32_t)(chunk >> 3) * 8192u + sw128_offset(row, chunk & 7);
           st_shared_v4(base + kOffAHi + off, hi);
-          if (passes == 3) st_shared_v4(base + kOffALo + off, lo);
+          if (kPasses == 3) st_shared_v4(base + kOffALo + off, lo);
         }
       } else {
         float pe[40];
@@ -630,18 +691,34 @@ struct TmapCacheEntry {
 };
 using TmapCache = TmapCacheEntry;
 
+// the dynamic shared memory opt-in of both precision modes of one network variant
+template <bool kJvp, int kNet> cudaError_t tc_allow_smem() {
+  cudaError_t e = cudaFuncSetAttribute(sdf_tc_kernel<kJvp, kNet, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(sdf_tc_kernel<kJvp, kNet, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
+  return e;
+}
+
 // opt-in to the 226 KB of dynamic shared memory once per device for every instantiation
 int tc_prepare_launch(int dev) {
   static bool done[16] = {false};
   if (done[dev & 15]) return 0;
-  cudaError_t e = cudaFuncSetAttribute(sdf_tc_kernel<false, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(sdf_tc_kernel<true, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(sdf_tc_kernel<false, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(sdf_tc_kernel<true, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(sdf_tc_kernel<false, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
+  cudaError_t e = tc_allow_smem<false, 0>();
+  if (e == cudaSuccess) e = tc_allow_smem<true, 0>();
+  if (e == cudaSuccess) e = tc_allow_smem<false, 1>();
+  if (e == cudaSuccess) e = tc_allow_smem<true, 1>();
+  if (e == cudaSuccess) e = tc_allow_smem<false, 2>();
   if (e != cudaSuccess) return (int)e;
   done[dev & 15] = true;
   return 0;
+}
+
+// launches the instantiation of prm.passes (1 or 3, checked by the callers)
+template <bool kJvp, int kNet>
+void tc_launch(int grid, cudaStream_t st, const CUtensorMap& tmap, const TcParams& prm) {
+  if (prm.passes == 3)
+    sdf_tc_kernel<kJvp, kNet, 3><<<grid, kThreads, kSmemBytes, st>>>(tmap, prm);
+  else
+    sdf_tc_kernel<kJvp, kNet, 1><<<grid, kThreads, kSmemBytes, st>>>(tmap, prm);
 }
 
 }  // namespace
@@ -684,9 +761,9 @@ static int launch_tc(const PointSource& src, const void* packed, const PeWeights
   prm.dbg_layer = dbg_layer; prm.dbg_out = dbg_out; prm.out_grad = out_grad;
   const int grid = tc_grid(P, out_grad ? kRowsPerCta / 4 : kRowsPerCta);
   if (out_grad)
-    sdf_tc_kernel<true, 0><<<grid, kThreads, kSmemBytes, st>>>(tc_.m128, prm);
+    tc_launch<true, 0>(grid, st, tc_.m128, prm);
   else
-    sdf_tc_kernel<false, 0><<<grid, kThreads, kSmemBytes, st>>>(tc_.m128, prm);
+    tc_launch<false, 0>(grid, st, tc_.m128, prm);
   int s = launch_status();
   if (s) return s;
   if (status_host) {  // diagnostics path: wait for the launch, then report (and clear) the status record
@@ -840,9 +917,9 @@ static int deformer_launch(const float* ps, const float* conds, const int64_t* b
   prm.out_translated = out_translated; prm.out_offset = out_offset; prm.out_posed = out_posed; prm.out_jac = out_jac;
   const int grid = tc_grid(P, out_jac ? kRowsPerCta / 4 : kRowsPerCta);   // forward mode: 4 rows per point
   if (out_jac)
-    sdf_tc_kernel<true, 1><<<grid, kThreads, kSmemBytes, st>>>(tc_.m128, prm);
+    tc_launch<true, 1>(grid, st, tc_.m128, prm);
   else
-    sdf_tc_kernel<false, 1><<<grid, kThreads, kSmemBytes, st>>>(tc_.m128, prm);
+    tc_launch<false, 1>(grid, st, tc_.m128, prm);
   return launch_status();
 }
 
@@ -922,7 +999,7 @@ extern "C" int recmv_rendernet_fwd(const float* points, const float* normals, co
   prm.P = P; prm.passes = mode == RECMV_MLP_TC_F16X3 ? 3 : 1; prm.status = sd; prm.dbg_layer = -1;
   set_acc_scales(prm);
   prm.normals = normals; prm.view_dirs = view_dirs; prm.feats = feats; prm.out_rgb = out_rgb;
-  sdf_tc_kernel<false, 2><<<tc_grid(P, kRowsPerCta), kThreads, kSmemBytes, st>>>(tc_.m128, prm);
+  tc_launch<false, 2>(tc_grid(P, kRowsPerCta), st, tc_.m128, prm);
   return launch_status();
 }
 

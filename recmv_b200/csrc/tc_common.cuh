@@ -144,6 +144,11 @@ __device__ __forceinline__ void wgmma_n16(float (&d)[8], uint64_t desc_a, uint64
 __device__ __forceinline__ uint64_t smem_desc_sw128(uint32_t smem_addr) {
   return (uint64_t)((smem_addr >> 4) & 0x3FFF) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
 }
+// K-major, 64-byte swizzle: rows of 64 B (32 fp16 along K), 8-row groups 512 B apart (SBO), atoms 512-B aligned;
+// [62,64) = 2 (64 B).  One K = 16 step inside the 32-wide atom advances the start address by 32 B.
+__device__ __forceinline__ uint64_t smem_desc_sw64(uint32_t smem_addr) {
+  return (uint64_t)((smem_addr >> 4) & 0x3FFF) | ((uint64_t)1 << 16) | ((uint64_t)(512 >> 4) << 32) | ((uint64_t)2 << 62);
+}
 // MN-major, 128-byte swizzle: canonical layout ((8,8,m),(8,k)):((1,8,LBO),(64,SBO)) in fp16 elements -- a [8 k-rows]
 // [64 mn] atom of 1024 B, atoms stacked along k every SBO = 1024 B and along mn every LBO (8192 B here: two TMA boxes of
 // {64 columns, 64 rows}).  One K = 16 step advances the start address by 16 rows = 2048 B.
@@ -224,7 +229,8 @@ __device__ __forceinline__ void st_shared_b32(uint32_t addr, uint32_t v) {
 }
 
 // ---- host: tensor map over the fp16 weight panels -------------------------------------------------------
-// 2-D tensor [rows, 64] fp16 (128-byte rows), box [64 x box_rows], 128-byte swizzle.
+// 2-D tensor [rows, 64] fp16 (128-byte rows), box [32 x box_rows] (half a row: inputs 0..31 or 32..63 of a panel),
+// 64-byte swizzle -- the layout smem_desc_sw64 describes.
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -240,10 +246,10 @@ inline int make_panel_tmap(CUtensorMap* out, const void* base, uint64_t rows, ui
   }
   cuuint64_t dims[2] = {64, rows};
   cuuint64_t strides[1] = {128};
-  cuuint32_t box[2] = {64, box_rows};
+  cuuint32_t box[2] = {32, box_rows};
   cuuint32_t estr[2] = {1, 1};
   CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS ? 0 : (int)cudaErrorInvalidValue;
 }
