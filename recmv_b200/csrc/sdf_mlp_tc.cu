@@ -92,6 +92,7 @@ struct TcParams {
   const float* view_dirs;        // [P,3]
   const float* feats;            // [P,256]
   float* out_rgb;                // [P,3]
+  int last_tiles;                // SDF network: 128-wide output tiles of the last layer (3: sdf + features, 1: sdf only)
 };
 
 // softplus(beta=100, threshold=20) * kActScale straight from the raw accumulator, in base 2:
@@ -138,8 +139,9 @@ __device__ __forceinline__ void positional_encode_tangent(float cx, float cy, fl
   }
 }
 
-// Network descriptions driving the same pipeline.  ntiles(l): 128-wide output tiles of layer l (warpgroup g owns tiles
-// 2 g and 2 g + 1); kb_at(l, i): the i-th K block (64 inputs) of layer l's input, 8 = the positional-encoding block.
+// Network descriptions driving the same pipeline.  ntiles(l, last): 128-wide output tiles of layer l (warpgroup g owns
+// tiles 2 g and 2 g + 1; `last` = TcParams::last_tiles); kb_at(l, i): the i-th K block (64 inputs) of layer l's input,
+// 8 = the positional-encoding block.
 template <int kNet> struct Net;
 // SDF network (model/network.py:135-141): PE block -> 512 x3 -> 473 -> [skip: +PE block] 512 x4 -> 257
 template <> struct Net<0> {
@@ -147,7 +149,7 @@ template <> struct Net<0> {
   __device__ static int nkb(int l) { return num_panels(l); }
   __device__ static int pbase(int l) { return panel_base(l); }
   __device__ static int kb_at(int l, int i) { return l == 0 ? 8 : (l == 4 ? (i == 0 ? 8 : i - 1) : i); }
-  __device__ static int ntiles(int l) { return l == 8 ? 3 : 4; }
+  __device__ static int ntiles(int l, int last) { return l == 8 ? last : 4; }
 };
 // MLPTranslator (model/Deformer.py:141-206): [PE(39) | cond(128) | 0 x25] = 3 K blocks -> 512 x4 (ReLU) -> 3
 template <> struct Net<1> {
@@ -155,7 +157,7 @@ template <> struct Net<1> {
   __device__ static int nkb(int l) { return l == 0 ? 3 : 8; }
   __device__ static int pbase(int l) { return l == 0 ? 0 : 3 + 8 * (l - 1); }
   __device__ static int kb_at(int, int i) { return i; }   // the input block lives in the activation buffer
-  __device__ static int ntiles(int l) { return l == 4 ? 1 : 4; }
+  __device__ static int ntiles(int l, int) { return l == 4 ? 1 : 4; }
 };
 // RenderingNetwork_view_norm, mode 'idr' (model/RenderNet.py:59-96): [p 3 | PE4(v) 27 | n 3 | feat 256 | 0 x31] = 5 K
 // blocks -> 512 x4 (ReLU) -> 3 -> tanh
@@ -164,7 +166,7 @@ template <> struct Net<2> {
   __device__ static int nkb(int l) { return l == 0 ? 5 : 8; }
   __device__ static int pbase(int l) { return l == 0 ? 0 : 5 + 8 * (l - 1); }
   __device__ static int kb_at(int, int i) { return i; }
-  __device__ static int ntiles(int l) { return l == 4 ? 1 : 4; }
+  __device__ static int ntiles(int l, int) { return l == 4 ? 1 : 4; }
 };
 
 // The MMAs of one weight box (one 64-wide K block x one 128-wide output tile x one weight plane) into accumulator `acc`.
@@ -254,7 +256,7 @@ sdf_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams prm) {
       uint32_t phase = 0;   // parity of the ring's current pass
       for (long long it = 0; it < n_iter; ++it) {
         for (int l = 0; l < kNumLayers; ++l) {
-          const int nkb = NetT::nkb(l), nt_own = own_tiles(NetT::ntiles(l), g);
+          const int nkb = NetT::nkb(l), nt_own = own_tiles(NetT::ntiles(l, prm.last_tiles), g);
           // last layer, parity mode: sweep 0 streams (w_hi, w_lo) for the correction MMAs, sweep 1 streams w_hi again
           const int nsweep = (kTwoSweeps && kPasses == 3 && l == kNumLayers - 1) ? 2 : 1;
           for (int sweep = 0; sweep < nsweep; ++sweep) {
@@ -316,7 +318,7 @@ sdf_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams prm) {
       const long long tile = tile_of(it);
       for (int l = 0; l < kNumLayers; ++l) {
         if (l == 0) mbar_wait(BAR(kBarPeReady), (uint32_t)(it & 1), abort_flag, prm.status, 220);
-        const int nkb = NetT::nkb(l), T = NetT::ntiles(l), nt_own = own_tiles(T, g);
+        const int nkb = NetT::nkb(l), T = NetT::ntiles(l, prm.last_tiles), nt_own = own_tiles(T, g);
         const bool hidden = l < kNumLayers - 1;
         const bool two_sweeps = kTwoSweeps && kPasses == 3 && l == kNumLayers - 1;
         // the layer's first MMA overwrites the accumulators; zeroing them here tells the compiler that the previous
@@ -759,6 +761,8 @@ static int launch_tc(const PointSource& src, const void* packed, const PeWeights
   prm.out_sdf = out_sdf; prm.out_feat = out_feat; prm.P = P; prm.P_dev = P_dev; prm.passes = passes; prm.status = sd;
   set_acc_scales(prm);
   prm.dbg_layer = dbg_layer; prm.dbg_out = dbg_out; prm.out_grad = out_grad;
+  // the last layer's output tiles 1 and 2 hold features only: computed when someone reads them
+  prm.last_tiles = (out_feat || (dbg_out && dbg_layer == kNumLayers - 1)) ? 3 : 1;
   const int grid = tc_grid(P, out_grad ? kRowsPerCta / 4 : kRowsPerCta);
   if (out_grad)
     tc_launch<true, 0>(grid, st, tc_.m128, prm);
