@@ -15,7 +15,7 @@ SIZES = [1, 64, 77, 5000]   # one tile, exactly one tile, a ragged tile count, m
 
 @pytest.fixture(scope="module")
 def packed():
-    net =testing.build_sdf(getTmpSdf, seed=0, perturb_seed=101).to(DEV)
+    net = testing.build_sdf(getTmpSdf, seed=0, perturb_seed=101).to(DEV)
     return net.packed_weights()
 
 
