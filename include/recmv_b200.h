@@ -223,7 +223,7 @@ RECMV_API int recmv_mlp_layer_planes(const void* a_hi, const void* a_lo, int64_t
                            int64_t ldy, float* Y2, int64_t ldy2, void* y_hi, void* y_lo, int64_t ldyp, int planes_with_dyn,
                            recmv_stream_t stream);
 
-/* Weight gradient from the same planes, no transposed copies (tcgen05 reads the row-major planes as MN-major operands):
+/* Weight gradient from the same planes, no transposed copies (wgmma reads the row-major planes as MN-major operands):
  *   dW [out_dim][in_dim] = scale * G^T X,  g planes [P][ldg_p] = 64 * dyn * g (columns < out_dim), x planes [P][ldx_p] = 64 * x.
  * The sample range is split over the SMs, partial tiles are summed in a fixed order (deterministic).  db [out_dim] (optional)
  * = sum_p g[p][:] = the bias gradient, from one more product of the G tiles with a tile of ones in the same launch.  workspace:

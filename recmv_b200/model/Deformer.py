@@ -164,7 +164,7 @@ class MLPTranslator(nn.Module):
             return tr.view(ps.shape[0], ps.shape[1], 3)
         if (self.fusable and self.train_fused and ps.is_cuda and self.mlp_mode != ops.MLP_FP32_SIMT
                 and conds.dim() == 2):
-            # training path: tcgen05 layer GEMMs forward + backward (ops.TranslatorTrainFunction)
+            # training path: tensor-core layer GEMMs forward + backward (ops.TranslatorTrainFunction)
             self.last_path = "fused-train"
             flat = ps.reshape(-1, 3).contiguous().float()
             inds = batch_inds if batch_inds is not None else torch.arange(

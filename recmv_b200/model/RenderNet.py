@@ -70,7 +70,7 @@ class RenderingNetwork_view_norm(nn.Module):
                                          ratio_to_weights(self.multires_v, ratio), self.mlp_mode)
         if (self.fusable and self.train_fused and points.is_cuda and points.dim() == 2
                 and self.mlp_mode != ops.MLP_FP32_SIMT):
-            # training path: tcgen05 layer GEMMs forward + backward (ops.RenderNetTrainFunction); tanh and the
+            # training path: tensor-core layer GEMMs forward + backward (ops.RenderNetTrainFunction); tanh and the
             # weight-norm re-parametrisation stay (tiny) torch graphs
             self.last_path = "fused-train"
             Ws, bs = [], []

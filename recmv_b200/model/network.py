@@ -105,7 +105,7 @@ class ImplicitNetwork(nn.Module):
             raise RuntimeError("recmv_b200.ImplicitNetwork runs on CUDA tensors only (no CPU path)")
         mode = ops.DEFAULT_MLP_MODE if self.mlp_mode is None else self.mlp_mode
         if self._fusable and self.train_fused and mode != ops.MLP_FP32_SIMT and input.dim() == 2:
-            # training path: tcgen05 layer GEMMs forward (outputs kept for the backward) + tcgen05 backward
+            # training path: tensor-core layer GEMMs forward (outputs kept for the backward) + tensor-core backward
             # (ops.SdfMlpTrainFunction); weight-norm's W = g v / |v| stays a (tiny) torch graph so (g, v) receive
             # their gradients from dW
             self.last_path = "fused-train"

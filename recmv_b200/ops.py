@@ -458,7 +458,7 @@ def sdf_value_and_grad(x, packed, pe_w=None, mode=None, want_feat=False):
 
 
 # --------------------------------------------------------------------------------------------------
-# Training path: fused forward that saves the layer inputs + tcgen05 backward GEMMs (csrc/gemm3.cu)
+# Training path: layer GEMMs that save their outputs for the backward (csrc/gemm3_tma.cu, first generation csrc/gemm3.cu)
 # --------------------------------------------------------------------------------------------------
 ACT_NONE, ACT_SOFTPLUS100, ACT_RELU = 0, 1, 2
 # "planes": forward / backward-data layer GEMMs fed by TMA from fp16 hi / lo operand planes (csrc/gemm3_tma.cu);
@@ -712,7 +712,8 @@ def _sdf_composite(x, Ws, bs, pe_w):
 
 class SdfMlpTrainFunction(torch.autograd.Function):
     """ImplicitNetwork.forward with gradients (model/network.py:89-119 inside train.py:317-330), all GEMMs on the tensor cores
-    in the engine's fp32-grade arithmetic (csrc/gemm3.cu: fp16 hi/lo split, 3 MMAs per product, fp32 accumulation).
+    in the engine's fp32-grade arithmetic (fp16 hi/lo split, 3 MMAs per product, fp32 accumulation): TMA-fed GEMMs on
+    operand planes (csrc/gemm3_tma.cu), or the first-generation csrc/gemm3.cu with RECMV_TRAIN_GEMM=producers.
 
     forward : PE kernel + 9 layer launches  Y = softplus(X W^T + b)  whose outputs stay in HBM as the next layer's input
               AND as what the backward needs (16 KB per point -- what autograd keeps for the reference's graph); the skip
@@ -934,7 +935,7 @@ def _plain_composite(X0, Ws, bs):
 
 class TranslatorTrainFunction(torch.autograd.Function):
     """MLPTranslator offset MLP with gradients (model/Deformer.py:171-206): input row [PE6(p) 39 | cond[frame] 128] ->
-    512 x4 ReLU -> 3, forward / backward-data / weight gradient on the tensor cores (csrc/gemm3.cu); returns the OFFSET (the caller
+    512 x4 ReLU -> 3, forward / backward-data / weight gradient on the tensor cores (csrc/gemm3_tma.cu); returns the OFFSET (the caller
     adds p).  create_graph=True falls back to a torch graph inside backward, like SdfMlpTrainFunction."""
     last_backward = None
 

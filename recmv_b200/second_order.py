@@ -16,9 +16,10 @@ runs on the same backward-data GEMMs as the first-order path, and is itself an a
     downward : an ordinary backward-data pass that picks zb_l up at every layer                       (8 layer GEMMs)
     weights  : dW_l = h_{l+1}^T tu_l + zb_l^T a_l  (two weight-gradient launches over all layers),  db_l = sum zb_l
 
-with h_{l+1} the first-order cotangent at z_l.  Everything heavy is a 3xfp16 tcgen05 GEMM of csrc/gemm3.cu; the per-layer
-element-wise products are torch ops on [P,512] tensors, the positional encoding's own VJP is a torch graph (so its second
-derivative comes from autograd).  A request that ALSO wants parameter gradients with a graph (loss.backward(create_graph=
+with h_{l+1} the first-order cotangent at z_l.  Everything heavy is a 3xfp16 wgmma GEMM: the SDF network's passes run on the
+operand-plane kernels of csrc/gemm3_tma.cu, each followed by one element-wise launch that also writes the next GEMM's
+planes; the translator and colour networks' reverse chain still runs on csrc/gemm3.cu with torch element-wise ops.  The
+positional encoding's own VJP is a torch graph (so its second derivative comes from autograd).  A request that ALSO wants parameter gradients with a graph (loss.backward(create_graph=
 True)) still takes the torch-composite fallback."""
 import torch
 

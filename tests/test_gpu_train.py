@@ -1,5 +1,5 @@
-"""GPU parity of the TRAINING path of the SDF network: the fused forward that saves the layer inputs and the tensor-core
-backward GEMMs (csrc/gemm3.cu) behind `loss.backward()`, against
+"""GPU parity of the TRAINING path of the SDF network: the forward that saves the layer inputs and the tensor-core
+backward GEMMs (csrc/gemm3_tma.cu; the first-generation csrc/gemm3.cu entries at ragged shapes) behind `loss.backward()`, against
   * the gradients torch autograd produces through the REFERENCE's own ImplicitNetwork (fp32 = the reference's numbers,
     fp64 = ground truth), tests/golden/sdf_bwd_*.npz from tests/golden/make_golden_r2.py;
   * fp64 matmuls for the two GEMM entry points at ragged shapes.
