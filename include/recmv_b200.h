@@ -83,6 +83,31 @@ RECMV_API int recmv_gridsample3d_bwd2(const void* gg_input, const void* gg_grid,
 RECMV_API int recmv_voxel_to_channels_last(const float* src, float* dst, int C, int D, int H, int W,
                                  recmv_stream_t stream);
 
+/* ---- skinning-voxel construction: compute_lbswField / smooth_weights ------------------------
+ * replaces model/Deformer.py:533-591 and utils/LBSWsmpl.py:2-51.  Setup work (once per body), not per step.
+ * knn_blend: voxel centre (x,y,z) of cell (i_W,i_H,i_D) is c/res + (1/res)/2 (align_corners = 0) or c/(res-1)
+ *   (align_corners != 0, every extent >= 2), times (bmax - bmin) plus bmin, all in fp32 as the reference rounds.
+ *   verts [V,3] f32 (V <= 14336, staged in shared memory), vert_ws [V,C] f32 with C == 24, bmin / bmax host [3].
+ *   The k nearest vertices (1 <= k <= 32, k <= V) by fp32 distance sqrt(fma(dz,dz,fma(dy,dy,dx*dx))); on
+ *   exactly equal distances the LOWER vertex index wins (torch.topk leaves that case undefined).  Each distance is
+ *   clamped to [1e-4, 1] and inverted, the inverses are normalised, and the 24 weights are blended in neighbour
+ *   order (nearest first).  out_cl [D,H,W,24] f32, voxel (z H + y) W + x; out_idx [D*H*W, k] int32 (nearest
+ *   first) or NULL.  No atomics: bit-identical from run to run.
+ * smooth: `times` Jacobi passes of the 6-neighbour stencil on channels-last buffers: interior voxels get
+ *   mean = (z+ + z- + y+ + y- + x+ + x-) / 6 (summed in that order, true division), w' = (w - mean) * 0.7 + mean;
+ *   boundary voxels (and every voxel of a grid with an extent below 3) keep their values; then every voxel is
+ *   divided by its sequential channel sum.  No FMA contraction.  times == 0 leaves the values as they are
+ *   (the reference's loop does not run).  Afterwards, if zero_below > 0, values below it become 0 with no
+ *   renormalisation (LBSWsmpl.py:10).  buf_a holds the input [D,H,W,24] and is overwritten; buf_b is scratch of
+ *   the same size (may be NULL when times <= 1).  Outputs: out_ncdhw [24,D,H,W] (the reference's `ws`) and
+ *   out_cl [D,H,W,24], bit-identical to recmv_voxel_to_channels_last(out_ncdhw).  buf_a, buf_b, out_cl must be
+ *   distinct and 16-byte aligned.                                                                             */
+RECMV_API int recmv_lbsw_knn_blend(const float* verts, const float* vert_ws, int V, int C, const float bmin[3] /*host*/,
+                                   const float bmax[3] /*host*/, int W, int H, int D, int align_corners, int k,
+                                   float* out_cl, int32_t* out_idx, recmv_stream_t stream);
+RECMV_API int recmv_lbsw_smooth(float* buf_a, float* buf_b, int D, int H, int W, int times, float zero_below,
+                                float* out_ncdhw, float* out_cl, recmv_stream_t stream);
+
 /* ---- A12: MCGpu.mc_gpu --------------------------------------------------------------------
  * replaces MCGpu/MCGpu.cpp:20-56 + CudaKernels.cu:316-521.  sdf [NX,NY,NZ] f32, z fastest.
  * Deterministic: vertices and faces come out in the order a sequential sweep of the reference

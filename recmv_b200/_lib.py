@@ -50,6 +50,9 @@ SIGNATURES = {
                                         c_int64, c_int, c_int, c_void_p]),
     "recmv_voxel_to_channels_last": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int,
                                              c_void_p]),
+    "recmv_lbsw_knn_blend": (c_int, [c_void_p, c_void_p, c_int, c_int, POINTER(c_float), POINTER(c_float), c_int, c_int,
+                                     c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "recmv_lbsw_smooth": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p]),
     "recmv_mc_scratch_bytes": (c_int, [c_int, c_int, c_int, POINTER(c_size_t)]),
     "recmv_mc_count": (c_int, [c_void_p, c_int, c_int, c_int, c_float, c_void_p, POINTER(c_int64),
                                POINTER(c_int64), c_void_p]),

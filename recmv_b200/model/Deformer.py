@@ -416,3 +416,67 @@ class LBSkinner(nn.Module):
         xc, ok = ops.lbs_inverse(x_obs.reshape(-1, 3), A, trans, self.ws_channels_last(), center, extend,
                                  batch_inds, ppf)
         return xc.view(shp), ok
+
+
+# -- skinning-voxel construction (model/Deformer.py:533-623): setup work, run once per body ----------------------------
+def _host3(v):
+    return [float(x) for x in torch.as_tensor(v).float().view(-1).tolist()]
+
+
+def _lbsw_field(bmins, bmaxs, resolutions, smpl_verts, smpl_ws, align_corners, mean_neighbor, smooth_times, zero_below):
+    """(ws [1,24,D,H,W], its channels-last copy [D,H,W,24]): the kNN blend kernel, then the smoothing kernel."""
+    if not smpl_verts.is_cuda:
+        raise RuntimeError("compute_lbswField runs on CUDA tensors only (no CPU path)")
+    verts = smpl_verts.reshape(-1, 3).float().contiguous()
+    vert_ws = smpl_ws.reshape(verts.shape[0], -1).float().contiguous()
+    ws_cl = ops.lbsw_knn_blend(verts, vert_ws, _host3(bmins), _host3(bmaxs), resolutions, mean_neighbor, align_corners)
+    return ops.lbsw_smooth(ws_cl, smooth_times, zero_below)
+
+
+def smooth_weights(weights, times=3):
+    """model/Deformer.py:533-544 on a [1,24,D,H,W] CUDA voxel (returns a new tensor; `weights` is left as it is)."""
+    if not weights.is_cuda:
+        raise RuntimeError("smooth_weights runs on CUDA tensors only (no CPU path)")
+    return ops.lbsw_smooth(ops.voxel_to_channels_last(weights.float().contiguous()), times)[0]
+
+
+def compute_lbswField(bmins, bmaxs, resolutions, smpl_verts, smpl_ws, align_corners=False, mean_neighbor=5,
+                      smooth_times=30):
+    """model/Deformer.py:546-591 -> ws [1,24,D,H,W] on the device of smpl_verts (CUDA only).  Two kernels instead of
+    38 chunks of a [50000, V, 3] difference tensor; the k-th-distance ties that torch.topk leaves undefined go to the
+    lower vertex index."""
+    return _lbsw_field(bmins, bmaxs, resolutions, smpl_verts, smpl_ws, align_corners, mean_neighbor, smooth_times, 0.0)[0]
+
+
+def skinner_from_body(verts, vert_ws, Js, parents, pose, resolution, extra_trans=None):
+    """The part of initialLBSkinner after SMPL (model/Deformer.py:603-623), line by line: the field is built over the
+    vertices' tight [min, max] box, the skinner normalises with its centre and 1.1 x its largest extent.
+    verts [V,3] (or [1,V,3]), vert_ws [V,24], Js [24,3], parents [24], pose (24 x 3 axis-angle).
+    Returns (LBSkinner, verts [V,3], None); the skinner's channels-last cache is already filled."""
+    verts = verts.reshape(-1, 3)
+    bbox_data_min = verts.min(0).values
+    bbox_data_max = verts.max(0).values
+    bbox_data_extend = (bbox_data_max - bbox_data_min).max()
+    bbox_grid_extend = bbox_data_extend * 1.1
+    grid_center = (bbox_data_min + bbox_data_max) / 2
+    ws, ws_cl = _lbsw_field(bbox_data_min.tolist(), bbox_data_max, resolution, verts, vert_ws.reshape(verts.shape[0], 24),
+                            False, 30, 30, 0.0)
+    sk = LBSkinner(ws, bbox_data_min, bbox_data_max, Js, parents, init_pose=pose, align_corners=False,
+                   extra_trans=extra_trans, bbox_extend=bbox_grid_extend, bbox_center=grid_center)
+    sk._ws_cl, sk._ws_key = ws_cl, (sk.ws.data_ptr(), sk.ws._version)
+    return sk, verts, None
+
+
+def initialLBSkinner(gender, shape, pose, resolution, bmins=None, bmaxs=None, extra_trans=None):
+    """model/Deformer.py:594-623.  SMPL itself is not part of this package: `smpl_pytorch` is imported here, as the
+    reference does at module level."""
+    from smpl_pytorch.SMPL import getSMPL
+    smpl = getSMPL(gender).to(shape.device)
+    Js, _ = smpl.skeleton(shape.view(1, -1), True)
+    verts, _, _ = smpl(shape.view(1, -1), pose.view(1, 24, 3), True)
+    if bmins is not None and bmaxs is not None:
+        # the reference defines its box only in the adaptive branch, so given boxes fail at Deformer.py:612
+        raise UnboundLocalError("local variable 'bbox_data_min' referenced before assignment")
+    sk, v, _ = skinner_from_body(verts.view(6890, 3), smpl.weight.view(6890, 24), Js, smpl.parents, pose, resolution,
+                                 extra_trans)
+    return sk, v, torch.tensor(smpl.faces, dtype=torch.long, device=verts.device)

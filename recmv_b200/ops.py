@@ -243,6 +243,43 @@ def voxel_to_channels_last(ws):
 
 
 # --------------------------------------------------------------------------------------------------
+# skinning-voxel construction (model/Deformer.py:533-591, utils/LBSWsmpl.py)
+# --------------------------------------------------------------------------------------------------
+def lbsw_knn_blend(verts, vert_ws, bmin, bmax, resolution, k, align_corners=False, want_idx=False):
+    """k-nearest-vertex blend of the skinning weights at every voxel centre (recmv_lbsw_knn_blend).
+    verts [V,3], vert_ws [V,24] fp32 CUDA; bmin / bmax: 3 host floats; resolution (W,H,D).
+    Returns ws_cl [D,H,W,24] (and idx [D*H*W,k] int32, nearest first, when want_idx)."""
+    _check_input(verts, "verts")
+    _check_input(vert_ws, "vert_ws")
+    W, H, D = (int(r) for r in resolution)
+    V, C = vert_ws.shape
+    out = torch.empty((D, H, W, C), dtype=torch.float32, device=verts.device)
+    idx = torch.empty((D * H * W, k), dtype=torch.int32, device=verts.device) if want_idx else None
+    lo, hi = (c_float * 3)(*[float(v) for v in bmin]), (c_float * 3)(*[float(v) for v in bmax])
+    with torch.cuda.device(verts.device):
+        check(_lib.load().recmv_lbsw_knn_blend(_ptr(verts), _ptr(vert_ws), V, C, lo, hi, W, H, D, int(bool(align_corners)),
+                                               int(k), _ptr(out), _ptr(idx), _stream(verts)), "recmv_lbsw_knn_blend")
+    return (out, idx) if want_idx else out
+
+
+def lbsw_smooth(ws_cl, times, zero_below=0.0):
+    """`times` passes of the reference's smooth_weights on a channels-last [D,H,W,24] voxel (recmv_lbsw_smooth), then
+    values below zero_below (if > 0) set to 0.  `ws_cl` is consumed (used as the first ping-pong buffer).
+    Returns (ws [1,24,D,H,W], ws_cl [D,H,W,24]) -- the second is what LBSkinner samples."""
+    _check_input(ws_cl, "ws_cl")
+    D, H, W, C = ws_cl.shape
+    if C != 24 or ws_cl.dtype != torch.float32:
+        raise RuntimeError("lbsw_smooth expects a float32 [D,H,W,24] voxel")
+    spare = torch.empty_like(ws_cl) if times >= 2 else None
+    out = torch.empty((1, C, D, H, W), dtype=torch.float32, device=ws_cl.device)
+    out_cl = torch.empty_like(ws_cl)
+    with torch.cuda.device(ws_cl.device):
+        check(_lib.load().recmv_lbsw_smooth(_ptr(ws_cl), _ptr(spare), D, H, W, int(times), float(zero_below), _ptr(out),
+                                            _ptr(out_cl), _stream(ws_cl)), "recmv_lbsw_smooth")
+    return out, out_cl
+
+
+# --------------------------------------------------------------------------------------------------
 # MCGpu
 # --------------------------------------------------------------------------------------------------
 _mc_state = {}   # per device: grow-only scratch + output buffers (like the MCGpu singleton, MCGpu/CudaKernels.cu:524-604)

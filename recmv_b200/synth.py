@@ -47,6 +47,37 @@ def skinning_voxel(shape=(65, 225, 129), seed=7, device="cpu", smooth=1):
     return (ws / ws.sum(1, keepdim=True)).contiguous()
 
 
+def body_points(num=6890, seed=5):
+    """(verts [num,3], weights [num,24]) fp32 on CPU: a stand-in for the SMPL vertices and skinning weights that
+    model/Deformer.py:594-623 diffuses into the voxel.  Points lie on capsules around the bones of skeleton() (radius
+    per bone, bones chosen in proportion to their length); each point's weights go to the parent joints of its three
+    nearest bones, falling off with the distance to them, so they are sparse like SMPL's.  Computed in float64 from a
+    seeded CPU generator, then rounded: bit-reproducible."""
+    g = generator(seed, "cpu")
+    Js = skeleton()[0].double()
+    par = torch.tensor(PARENTS[1:])
+    a, b = Js[par], Js[1:]                                    # 23 bones: parent joint -> child joint
+    length = (b - a).norm(dim=1)
+    radius = torch.full((23,), 0.045, dtype=torch.float64)
+    radius[[2, 5, 8, 11, 12, 14]] = 0.11                    # spine and neck bones: a thicker torso
+    radius[[0, 1, 3, 4]] = 0.07                             # thighs
+    bone = torch.multinomial((length + 0.05).float(), num, replacement=True, generator=g)
+    t = torch.rand(num, generator=g, dtype=torch.float64)
+    u = torch.randn((num, 3), generator=g, dtype=torch.float64)
+    u = u / u.norm(dim=1, keepdim=True)
+    verts = a[bone] + t[:, None] * (b - a)[bone] + radius[bone][:, None] * u
+    # distance of every point to every bone segment -> weights of the parent joints of the three nearest bones
+    ab = (b - a)[None]
+    s = ((verts[:, None] - a[None]) * ab).sum(-1) / (ab * ab).sum(-1)
+    d = (verts[:, None] - (a[None] + s.clamp(0, 1)[..., None] * ab)).norm(dim=-1) - radius[None]
+    dn, bn = d.topk(3, dim=1, largest=False)
+    wn = torch.exp(-(dn - dn[:, :1]) / 0.02)
+    wn = wn / wn.sum(1, keepdim=True)
+    ws = torch.zeros((num, 24), dtype=torch.float64)
+    ws.index_put_((torch.arange(num)[:, None].expand(-1, 3), par[bn]), wn, accumulate=True)
+    return verts.float().contiguous(), ws.float().contiguous()
+
+
 def poses_trans(num_frames, seed=11, device="cpu"):
     g = generator(seed, device)
     poses = torch.randn((num_frames, 24, 3), generator=g, device=device) * 0.2

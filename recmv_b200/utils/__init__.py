@@ -97,6 +97,22 @@ def implicit_surface_grad_coeffs(sdf, deformer, ps, rays, grad_l_p, defconds, ba
     return coef, vec, rg, ok, d
 
 
+def smooth_weights(weights, times=3):
+    """utils/LBSWsmpl.py:2-11: model.Deformer.smooth_weights followed by weights < 5e-3 -> 0 (CUDA only)."""
+    if not weights.is_cuda:
+        raise RuntimeError("smooth_weights runs on CUDA tensors only (no CPU path)")
+    return _ops.lbsw_smooth(_ops.voxel_to_channels_last(weights.float().contiguous()), times, 5e-3)[0]
+
+
+def compute_lbswField(bmins, bmaxs, resolutions, smpl_verts, smpl_ws, align_corners=False, mean_neighbor=5,
+                      smooth_times=30):
+    """utils/LBSWsmpl.py:13-51 (exported as utils.compute_lbswField): the model/Deformer.py construction with the final
+    5e-3 threshold.  CUDA only."""
+    from ..model.Deformer import _lbsw_field
+    return _lbsw_field(bmins, bmaxs, resolutions, smpl_verts, smpl_ws, align_corners, mean_neighbor, smooth_times,
+                       5e-3)[0]
+
+
 def GMRobustError(x, c, square=False):
     """Geman-McClure robust error (utils/utils.py:48-52)."""
     if square:
