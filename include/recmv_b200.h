@@ -161,6 +161,31 @@ RECMV_API int recmv_lbs_inverse(const float* x_obs, const float* A, const float*
 RECMV_API int recmv_bone_matrices(const float* poses, const float* Js, const int* parents, const float* init_pose,
                         float* G, float* A, int num_frames, recmv_stream_t stream);
 
+/* VJP of recmv_bone_matrices (the autograd path of LBSkinner.bone_matrices / posedSkeleton when poses require grad).
+ * G [F,24,4,4] is what recmv_bone_matrices wrote for these poses.  dG [F,24,4,4] (cotangent of G, e.g. of the posed
+ * skeleton) and dA [F,24,4,4] (cotangent of A) may each be NULL; row 3 of either is ignored.  init_pose as in the
+ * forward.  Writes dposes [F,24,3].  One thread per frame, no atomics: deterministic.                              */
+RECMV_API int recmv_bone_matrices_backward(const float* poses, const float* Js, const int* parents,
+                                           const float* init_pose, const float* G, const float* dG, const float* dA,
+                                           float* dposes, int num_frames, recmv_stream_t stream);
+
+/* Backward of recmv_lbs_fwd for the training step (pose / translation / point gradients).  Same inputs as the
+ * forward (trans is accepted for symmetry and may be NULL: no gradient depends on it) plus grad_out [P,3].  Outputs,
+ * each may be NULL:
+ *   dps    [P,3]       = J^T g (J = d out / d ps, weights resampled at ps) when tps is NULL, else T[:3,:3]^T g
+ *   dtps   [P,3]       the weight term, only when tps is given (ignored otherwise)
+ *   dA     [F,24,4,4]  dA_f[j][r][c] = sum over the points of frame f of w_j g_r [ps;1]_c; row 3 is zero
+ *   dtrans [F,3]       sum over the points of frame f of g
+ * Frames as in the forward (batch_inds, unsorted allowed, or points_per_frame; clamped to [0, F)).  dA / dtrans are
+ * reduced over fixed chunks of 256 points and then over the chunks in order, so they are bit-identical from run to run
+ * and on any GPU.  workspace: recmv_lbs_backward_workspace_bytes(P, F) bytes, 16-byte aligned, needed when dA or
+ * dtrans is requested (it may be NULL when P == 0); it carries nothing between calls.                              */
+RECMV_API int recmv_lbs_backward_workspace_bytes(int64_t P, int num_frames, size_t* bytes /*host*/);
+RECMV_API int recmv_lbs_backward(const float* ps, const float* tps, const float* A, const float* trans,
+                                 const int64_t* batch_inds, int64_t points_per_frame, int num_frames,
+                                 const recmv_voxel_t* vox /*host*/, const float* grad_out, float* dps, float* dtps,
+                                 float* dA, float* dtrans, void* workspace, int64_t P, recmv_stream_t stream);
+
 /* ---- A1+A2: Embedder + ImplicitNetwork.forward -------------------------------------------------
  * replaces model/Embedder.py:43-50 + model/network.py:89-119 (+ utils/utils.py:40-46 weights).
  * Network shape is the reference's getTmpSdf: PE(6) 39 -> 512 x3 -> 473 (+39 skip)/sqrt2 -> 512 x4

@@ -65,6 +65,10 @@ SIGNATURES = {
     "recmv_lbs_inverse": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int,
                                   POINTER(Voxel), c_void_p, c_void_p, c_int64, c_void_p]),
     "recmv_bone_matrices": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
+    "recmv_bone_matrices_backward": (c_int, [c_void_p] * 8 + [c_int, c_void_p]),
+    "recmv_lbs_backward_workspace_bytes": (c_int, [c_int64, c_int, POINTER(c_size_t)]),
+    "recmv_lbs_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, POINTER(Voxel),
+                                   c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p]),
     "recmv_sdf_packed_bytes": (c_size_t, []),
     "recmv_sdf_pack_weights": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),
     "recmv_sdf_mlp_fwd": (c_int, [c_void_p, c_void_p, POINTER(c_float), c_void_p, c_void_p, c_int64,

@@ -186,12 +186,15 @@ __device__ __forceinline__ bool inverse_lbs_point(const Voxel& v, const float* _
 // sampler's backward, GridSamplerMineKernel.cu:42-59,330-520: factor size/2 * 2/extend per axis, zero on an axis
 // whose coordinate was clamped).  Evaluated corner by corner -- T_c = sum_b ws[corner][b] A_b, Y_c = T_c [q;1] --
 // so nothing of size 24 x 3 is ever live in registers.
-__device__ __forceinline__ void lbs_forward_jac(const Voxel& v, const float* __restrict__ Af,
-                                                const float* __restrict__ tf, float qx, float qy, float qz,
-                                                float out[3], float J[9]) {
-  float gx = (qx - v.cx) / v.ext * 2.f;
-  float gy = (qy - v.cy) / v.ext * 2.f;
-  float gz = (qz - v.cz) / v.ext * 2.f;
+//
+// lbs_blend_jac is the shared core: the weights are sampled at s and the blended transform is applied to a (the
+// `[tps, ps]` form of LBSkinner.repose samples at tps and moves ps).  It returns T (rows 0..2 of sum_b w_b A_b) and
+// only the weight term Jw_ij = sum_b (A_b [a;1])_i * d w_b / d s_j; lbs_forward_jac is the case s = a.
+__device__ __forceinline__ void lbs_blend_jac(const Voxel& v, const float* __restrict__ Af, float sx, float sy,
+                                              float sz, float qx, float qy, float qz, float T[12], float J[9]) {
+  float gx = (sx - v.cx) / v.ext * 2.f;
+  float gy = (sy - v.cy) / v.ext * 2.f;
+  float gz = (sz - v.cz) / v.ext * 2.f;
   float mx, my, mz;
   float ix = clip_grad<float>(unnormalize(gx, v.W), v.W, &mx);
   float iy = clip_grad<float>(unnormalize(gy, v.H), v.H, &my);
@@ -206,7 +209,6 @@ __device__ __forceinline__ void lbs_forward_jac(const Voxel& v, const float* __r
   const float wy[2] = {(float)(y0 + 1) - iy, iy - (float)y0};
   const float wz[2] = {(float)(z0 + 1) - iz, iz - (float)z0};
   const int xs[2] = {x0, x1}, ys[2] = {y0, y1}, zs[2] = {z0, z1};
-  float T[12];
 #pragma unroll
   for (int e = 0; e < 12; ++e) T[e] = 0.f;
 #pragma unroll
@@ -242,6 +244,13 @@ __device__ __forceinline__ void lbs_forward_jac(const Voxel& v, const float* __r
       J[3 * i + 2] = fmaf(Y[i], dcz, J[3 * i + 2]);
     }
   }
+}
+
+__device__ __forceinline__ void lbs_forward_jac(const Voxel& v, const float* __restrict__ Af,
+                                                const float* __restrict__ tf, float qx, float qy, float qz,
+                                                float out[3], float J[9]) {
+  float T[12];
+  lbs_blend_jac(v, Af, qx, qy, qz, qx, qy, qz, T, J);
 #pragma unroll
   for (int i = 0; i < 3; ++i) {
     out[i] = (T[4 * i] * qx + T[4 * i + 1] * qy + T[4 * i + 2] * qz + T[4 * i + 3]) + __ldg(tf + i);

@@ -7,8 +7,12 @@ LBSkinner.forward:
   * bone matrices A = G . init_pose are built on the host side in torch (24 joints, tiny);
   * no autograd needed -> ONE fused launch (voxel sample + blend + apply, recmv_lbs_fwd) over the
     channels-last cache of `ws` (rebuilt when `ws` changes, e.g. load_state_dict);
-  * autograd needed -> the CUDA GridSamplerMine3dFunction (twice differentiable) + batched blend,
-    without the reference's per-frame python loop and its `.item()` sync (Deformer.py:438-444).
+  * poses or translations that require grad (training) -> ops.LbsTrainFunction: the same forward kernel, and one
+    backward kernel for the point / pose / translation gradients, on a chain built and differentiated by kernels
+    (ops.BoneMatricesFunction);
+  * otherwise with autograd (only the points, or train_fused = False, or a create_graph backward) -> the CUDA
+    GridSamplerMine3dFunction (twice differentiable) + batched blend, without the reference's per-frame python loop and
+    its `.item()` sync (Deformer.py:438-444).
 """
 import numpy as np
 import torch
@@ -239,7 +243,13 @@ class LBSkinner(nn.Module):
         self._ws_key = None
         self._bbox_key, self._bbox_host = None, None
         self._parents_i32 = None
+        self.train_fused = True   # poses / trans that require grad: kernel chain + ops.LbsTrainFunction (False: torch graph)
         self.last_path = None
+
+    @property
+    def last_backward(self):
+        """Which backward branch of ops.LbsTrainFunction ran last: "fused" or "autograd-composite (create_graph)"."""
+        return ops.LbsTrainFunction.last_backward
 
     def bbox_size(self):
         margin = torch.tensor([0.15, 0.15, 0.20]).to(self.b_min)
@@ -293,10 +303,18 @@ class LBSkinner(nn.Module):
             self._parents_i32 = torch.as_tensor(self.parents).to(torch.int32).to(device).contiguous()
         return self._parents_i32
 
+    def _chain_graph(self, poses):
+        """True when the poses need a graph and it is the device chain's (ops.BoneMatricesFunction)."""
+        return poses.is_cuda and self.train_fused and torch.is_grad_enabled() and poses.requires_grad
+
     def bone_matrices(self, poses):
-        """A [N,24,4,4] = G . init_pose (Deformer.py:372-405).  One kernel when no graph is needed."""
+        """A [N,24,4,4] = G . init_pose (Deformer.py:372-405).  One kernel when no graph is needed; with a graph, the same
+        kernel forward and its VJP kernel backward (train_fused), or the torch chain."""
         if poses.is_cuda and not (torch.is_grad_enabled() and poses.requires_grad):
             return ops.bone_matrices(poses.reshape(-1, 24, 3), self.Js, self._parents_dev(poses.device), self.init_pose)[1]
+        if self._chain_graph(poses):
+            return ops.BoneMatricesFunction.apply(poses.reshape(-1, 24, 3).float(), self.Js, self._parents_dev(poses.device),
+                                                  self.init_pose)[1]
         results, Js = self._chain(poses)
         batch_size = poses.shape[0]
         if self.init_pose is None:
@@ -310,6 +328,10 @@ class LBSkinner(nn.Module):
         assert (poses.shape[0] == trans.shape[0])
         if poses.is_cuda and not (torch.is_grad_enabled() and poses.requires_grad):
             G, _ = ops.bone_matrices(poses.reshape(-1, 24, 3), self.Js, self._parents_dev(poses.device), None, want_A=False)
+            return G[:, :, :3, 3]
+        if self._chain_graph(poses):
+            G, _ = ops.BoneMatricesFunction.apply(poses.reshape(-1, 24, 3).float(), self.Js, self._parents_dev(poses.device),
+                                                  None)
             return G[:, :, :3, 3]
         results, _ = self._chain(poses)
         return results[:, :, :3, 3]
@@ -388,7 +410,23 @@ class LBSkinner(nn.Module):
             out = ops.lbs_forward(ps.reshape(-1, 3), A, trans, self.ws_channels_last(), center, extend,
                                   batch_inds, 0, None if tps is ps else tps.reshape(-1, 3))
             return out
+        if self.train_fused and torch.is_grad_enabled() and (poses.requires_grad or trans.requires_grad):
+            # training step: forward kernel, backward kernel for the pose / translation / point gradients
+            self.last_path = "fused-train"
+            p32 = ps.float().contiguous()
+            t32 = None if tps is ps else tps.float().contiguous()
+            bi = None if batch_inds is None else batch_inds.contiguous().long()
+            if bi is None:
+                assert (batch_size == ps.shape[0])
+            return ops.LbsTrainFunction.apply(p32, t32, A.float(), trans.float().contiguous(), bi,
+                                              (self.ws_channels_last(), center, extend),
+                                              lambda p, t, a, tr: self._composite(p, p if t is None else t, a, tr, bi))
         self.last_path = "autograd-composite"
+        return self._composite(ps, tps, A, trans, batch_inds)
+
+    def _composite(self, ps, tps, A, trans, batch_inds):
+        """The skinning as a torch graph on the CUDA sampler (twice differentiable)."""
+        batch_size = A.shape[0]
         nps = self.inv_transform_v(tps, self.bbox_extend, self.bbox_center).view(-1, 3)
         # the frozen voxel in its cached channels-last layout (one corner = 24 contiguous floats = 3 sectors instead of the
         # reference layout's 24)

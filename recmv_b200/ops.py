@@ -428,6 +428,117 @@ def bone_matrices(poses, Js, parents_i32, init_pose=None, want_A=True):
     return G, A
 
 
+def bone_matrices_backward(poses, Js, parents_i32, init_pose, G, dG=None, dA=None):
+    """dposes [F,24,3] = VJP of bone_matrices at `poses` (G: its output); dG / dA: cotangents of G / A or None."""
+    poses = poses.detach().contiguous().float()
+    _check_input(poses, "poses")
+    F_ = poses.shape[0]
+    dev = poses.device
+    dposes = torch.empty((F_, 24, 3), dtype=torch.float32, device=dev)
+    dG = dG.contiguous().float() if dG is not None else None
+    dA = dA.contiguous().float() if dA is not None else None
+    ip = init_pose.contiguous().float() if init_pose is not None else None
+    with torch.cuda.device(dev):
+        check(_lib.load().recmv_bone_matrices_backward(_ptr(poses), _ptr(Js.contiguous().float()), _ptr(parents_i32),
+                                                       _ptr(ip), _ptr(G.contiguous()), _ptr(dG), _ptr(dA), _ptr(dposes),
+                                                       F_, _stream(poses)), "recmv_bone_matrices_backward")
+    return dposes
+
+
+class BoneMatricesFunction(torch.autograd.Function):
+    """(G, A) of the kinematic chain (recmv_bone_matrices) with its VJP on the device (recmv_bone_matrices_backward): the
+    autograd path of LBSkinner.bone_matrices / posedSkeleton when the poses are trained.  poses [F,24,3] fp32.
+    First order only: nothing in the training step differentiates the skeleton twice."""
+
+    @staticmethod
+    def forward(ctx, poses, Js, parents_i32, init_pose):
+        G, A = bone_matrices(poses, Js, parents_i32, init_pose)
+        ctx.save_for_backward(poses, G)
+        ctx.Js, ctx.parents, ctx.init_pose = Js, parents_i32, init_pose
+        return G, A
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, dG, dA):
+        poses, G = ctx.saved_tensors
+        if not ctx.needs_input_grad[0]:
+            return None, None, None, None
+        return bone_matrices_backward(poses, ctx.Js, ctx.parents, ctx.init_pose, G, dG, dA), None, None, None
+
+
+def lbs_backward(ps, A, grad_out, ws_cl, center, extend, batch_inds=None, points_per_frame=0, tps=None,
+                 want_ps=True, want_tps=True, want_A=True, want_trans=True):
+    """(dps, dtps, dA, dtrans) of lbs_forward for the cotangent grad_out [P,3] (recmv_lbs_backward); an output that is not
+    wanted (or dtps without tps) is None."""
+    ps = ps.contiguous().float()
+    A = A.contiguous().float()
+    g = grad_out.contiguous().float()
+    P = ps.numel() // 3
+    F_ = int(A.shape[0])
+    dev = ps.device
+    if tps is not None:
+        tps = tps.contiguous().float()
+    if batch_inds is not None:
+        batch_inds = batch_inds.contiguous().long()
+    dps = torch.empty((P, 3), dtype=torch.float32, device=dev) if want_ps else None
+    dtps = torch.empty((P, 3), dtype=torch.float32, device=dev) if want_tps and tps is not None else None
+    dA = torch.empty((F_, 24, 4, 4), dtype=torch.float32, device=dev) if want_A else None
+    dtrans = torch.empty((F_, 3), dtype=torch.float32, device=dev) if want_trans else None
+    lib = _lib.load()
+    nbytes = c_size_t(0)
+    check(lib.recmv_lbs_backward_workspace_bytes(P, F_, byref(nbytes)), "recmv_lbs_backward_workspace_bytes")
+    work = torch.empty((max(int(nbytes.value), 16),), dtype=torch.uint8, device=dev) if (want_A or want_trans) else None
+    vox = make_voxel(ws_cl, center, extend)
+    with torch.cuda.device(dev):
+        check(lib.recmv_lbs_backward(_ptr(ps), _ptr(tps), _ptr(A), None, _ptr(batch_inds), int(points_per_frame), F_,
+                                     byref(vox), _ptr(g), _ptr(dps), _ptr(dtps), _ptr(dA), _ptr(dtrans), _ptr(work), P,
+                                     _stream(ps)), "recmv_lbs_backward")
+    return dps, dtps, dA, dtrans
+
+
+class LbsTrainFunction(torch.autograd.Function):
+    """LBSkinner.forward with gradients for the poses / translations (and the points): forward recmv_lbs_fwd, backward
+    recmv_lbs_backward (weights resampled, not kept in the graph).  ps [...,3] contiguous fp32 ([N,V,3] with frame = row,
+    or [P,3] with batch_inds); tps None or the sampling points of the `[tps, ps]` form; A [F,24,4,4]; trans [F,3].
+    `skin` = (ws_cl, center, extend).  A backward under create_graph (the train-phase Jacobians of utils) evaluates
+    `composite(ps, tps, A, trans)` -- the torch-sampler graph of LBSkinner -- on the saved inputs and differentiates it
+    with create_graph=True; `last_backward` says which branch ran."""
+    last_backward = None
+
+    @staticmethod
+    def forward(ctx, ps, tps, A, trans, batch_inds, skin, composite):
+        ws_cl, center, extend = skin
+        ppf = 0 if batch_inds is not None else ps.shape[1]
+        out = lbs_forward(ps.reshape(-1, 3), A, trans, ws_cl, center, extend, batch_inds, ppf,
+                          None if tps is None else tps.reshape(-1, 3))
+        ctx.save_for_backward(ps, tps, A, trans, batch_inds)
+        ctx.skin, ctx.composite, ctx.ppf = skin, composite, ppf
+        return out.view(ps.shape)
+
+    @staticmethod
+    def backward(ctx, g):
+        ps, tps, A, trans, batch_inds = ctx.saved_tensors
+        need = ctx.needs_input_grad
+        if torch.is_grad_enabled():
+            LbsTrainFunction.last_backward = "autograd-composite (create_graph)"
+            args = [ps, tps, A, trans]
+            ins = [t if (t is None or t.requires_grad) else t.detach() for t in args]
+            with torch.enable_grad():
+                out = ctx.composite(*ins)
+                diff = [t for t in ins if t is not None and t.requires_grad]
+                gr = iter(torch.autograd.grad([out], diff, [g], create_graph=True, allow_unused=True))
+            res = [next(gr) if (t is not None and t.requires_grad) else None for t in ins]
+            return (*[r if n else None for r, n in zip(res, need[:4])], None, None, None)
+        LbsTrainFunction.last_backward = "fused"
+        ws_cl, center, extend = ctx.skin
+        dps, dtps, dA, dtrans = lbs_backward(ps.reshape(-1, 3), A, g.reshape(-1, 3), ws_cl, center, extend, batch_inds,
+                                             ctx.ppf, None if tps is None else tps.reshape(-1, 3), want_ps=need[0],
+                                             want_tps=need[1], want_A=need[2], want_trans=need[3])
+        dps = dps.view(ps.shape) if dps is not None else None
+        dtps = dtps.view(tps.shape) if dtps is not None else None
+        return dps, dtps, dA, dtrans, None, None, None
+
+
 # --------------------------------------------------------------------------------------------------
 # SDF MLP
 # --------------------------------------------------------------------------------------------------
