@@ -38,6 +38,23 @@ constexpr int kRowsPerCta = 64;
 #define RECMV_TC_TWO_SWEEPS 1   // last layer, parity mode: correction MMAs first, hi*hi MMAs in a second sweep
 #endif
 constexpr bool kTwoSweeps = RECMV_TC_TWO_SWEEPS != 0;
+#ifndef RECMV_TC_STALL_PROF
+#define RECMV_TC_STALL_PROF 0   // diagnostics build only (tools/tc_stall_profile.py): per-CTA clock64() stall counters
+#endif
+constexpr bool kStallProf = RECMV_TC_STALL_PROF != 0;
+// Stall counters of the diagnostics build, in SM cycles summed over CTAs.  Consumer counters are taken by thread 0 of
+// each MMA warpgroup, producer counters by the producer lane; what a warpgroup does outside them is issuing MMAs.
+enum StallCounter {
+  kStFull,           // consumer: waits on a FULL barrier (weights not there yet)
+  kStWgWait,         // consumer: wgmma.wait_group (tensor pipe still busy with this warpgroup's groups)
+  kStEpilogue,       // consumer: softplus / store epilogue of every layer
+  kStNamedBar,       // consumer: the two named barriers per hidden layer
+  kStPeReady,        // consumer: wait for the prologue's tile input
+  kStConsumerTotal,  // consumer: the whole tile loop
+  kStEmpty,          // producer: waits on an EMPTY barrier (ring full)
+  kStProducerTotal,  // producer: the whole tile loop
+  kStCounters
+};
 // One weight ring per warpgroup.  A slot holds a [128 outputs x 32 inputs] half of a weight box (64-byte swizzle), so a
 // box = two consecutive slots; 5 slots let a warpgroup keep two half-boxes in flight beyond the three its MMAs may hold.
 constexpr int kSlots = 5;                         // per ring
@@ -57,7 +74,11 @@ constexpr int kBarPeFree = 21;   //       the MMAs of layer kInFreeLayer are don
 constexpr int kNumBars = 22;
 constexpr int kBarConsumers = 1; // named barrier of the 256 MMA threads
 constexpr uint32_t kOffMisc = kOffBar + kNumBars * 8;  // abort flag, valid flags
-constexpr uint32_t kSmemBytes = kOffMisc + 16 + 128 + 1024 /*alignment slack*/;
+constexpr uint32_t kOffProf = kOffMisc + 16 + 128;     // diagnostics build: [4 roles][kStCounters] u64
+constexpr uint32_t kSmemBytes = kOffProf + (kStallProf ? 4 * kStCounters * 8 : 0) + 1024 /*alignment slack*/;
+#if RECMV_TC_STALL_PROF
+__device__ unsigned long long g_tc_stall[kStCounters];   // read and cleared by recmv_tc_stall_profile
+#endif
 
 struct TcParams {
   PointSource src;
@@ -237,6 +258,25 @@ sdf_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams prm) {
   auto SLOT = [&](int g, int s) { return base + kOffW + (uint32_t)(g * kSlots + s) * kSlotBytes; };
   auto FULL = [&](int g, int s) { return BAR(kBarFull + g * kSlots + s); };
   auto EMPTY = [&](int g, int s) { return BAR(kBarEmpty + g * kSlots + s); };
+  // diagnostics build: the stall counters of role r (0, 1: MMA warpgroup g; 2, 3: producer of ring g), kept by one
+  // thread each in shared memory and added to g_tc_stall when its loop ends
+  auto stall_begin = [&](bool mine, int r) -> unsigned long long* {
+    unsigned long long* c = reinterpret_cast<unsigned long long*>(gbase + kOffProf) + r * kStCounters;
+    if (kStallProf && mine)
+      for (int k = 0; k < kStCounters; ++k) c[k] = 0;
+    return c;
+  };
+  auto stall_now = [&]() -> long long { return kStallProf ? clock64() : 0; };
+  auto stall_add = [&](unsigned long long* c, bool mine, int k, long long t0) {
+    if (kStallProf && mine) c[k] += (unsigned long long)(clock64() - t0);
+  };
+  auto stall_end = [&](unsigned long long* c, bool mine) {
+#if RECMV_TC_STALL_PROF
+    if (mine)
+      for (int k = 0; k < kStCounters; ++k) atomicAdd(&g_tc_stall[k], c[k]);
+#endif
+    (void)c; (void)mine;
+  };
 
   if (threadIdx.x == 0) {
     *abort_flag = 0;
@@ -252,6 +292,8 @@ sdf_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams prm) {
     // ====== TMA producers: warp 8 + g streams the weight boxes of warpgroup g, in the order that warpgroup consumes them ======
     const int g = warp - kProducerWarp;
     if (lane == 0) {
+      unsigned long long* stall = stall_begin(true, 2 + g);
+      const long long t_loop = stall_now();
       int slot = 0;
       uint32_t phase = 0;   // parity of the ring's current pass
       for (long long it = 0; it < n_iter; ++it) {
@@ -267,7 +309,9 @@ sdf_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams prm) {
               for (int t = 0; t < nt_own; ++t) {
                 for (int plane = 0; plane < nplanes; ++plane) {
                   for (int half = 0; half < 2; ++half) {
+                    const long long t0 = stall_now();
                     mbar_wait(EMPTY(g, slot), phase ^ 1u, abort_flag, prm.status, 100 + g * kSlots + slot);
+                    stall_add(stall, true, kStEmpty, t0);
                     mbar_expect_tx_local(FULL(g, slot), kSlotBytes);
                     tma_load_2d(SLOT(g, slot), &tmap, FULL(g, slot), 32 * half,
                                 (plane * NetT::kPanels + panel) * 512 + (2 * g + t) * 128);
@@ -279,6 +323,8 @@ sdf_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams prm) {
           }
         }
       }
+      stall_add(stall, true, kStProducerTotal, t_loop);
+      stall_end(stall, true);
     }
   } else if (warp < kMmaWarps) {
     // ================================ MMA warpgroups + epilogue =========================================
@@ -294,30 +340,40 @@ sdf_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams prm) {
     int slot = 0, held = -1, s0 = 0, s1 = 0;
     uint32_t phase = 0;
     // wait for the next box (two slots) and return its B descriptors
+    unsigned long long* stall = stall_begin(signaller, g);
     auto acquire = [&](uint64_t& b0, uint64_t& b1) {
+      const long long t0 = stall_now();
       s0 = slot;
       mbar_wait(FULL(g, slot), phase, abort_flag, prm.status, 230 + g * kSlots + slot);
       if (++slot == kSlots) { slot = 0; phase ^= 1u; }
       s1 = slot;
       mbar_wait(FULL(g, slot), phase, abort_flag, prm.status, 230 + g * kSlots + slot);
       if (++slot == kSlots) { slot = 0; phase ^= 1u; }
+      stall_add(stall, signaller, kStFull, t0);
       b0 = smem_desc_sw64(SLOT(g, s0));
       b1 = smem_desc_sw64(SLOT(g, s1));
     };
     // once the box's first commit group has retired: release its first half and the previous box's second half (whose
     // group retired before it); the second half stays held until the next box's first group has retired
     auto retire = [&]() {
+      const long long t0 = stall_now();
       wg_wait<1>();
+      stall_add(stall, signaller, kStWgWait, t0);
       if (signaller) {
         if (held >= 0) mbar_arrive_local(EMPTY(g, held));
         mbar_arrive_local(EMPTY(g, s0));
       }
       held = s1;
     };
+    const long long t_loop = stall_now();
     for (long long it = 0; it < n_iter; ++it) {
       const long long tile = tile_of(it);
       for (int l = 0; l < kNumLayers; ++l) {
-        if (l == 0) mbar_wait(BAR(kBarPeReady), (uint32_t)(it & 1), abort_flag, prm.status, 220);
+        if (l == 0) {
+          const long long t0 = stall_now();
+          mbar_wait(BAR(kBarPeReady), (uint32_t)(it & 1), abort_flag, prm.status, 220);
+          stall_add(stall, signaller, kStPeReady, t0);
+        }
         const int nkb = NetT::nkb(l), T = NetT::ntiles(l, prm.last_tiles), nt_own = own_tiles(T, g);
         const bool hidden = l < kNumLayers - 1;
         const bool two_sweeps = kTwoSweeps && kPasses == 3 && l == kNumLayers - 1;
@@ -362,9 +418,11 @@ sdf_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams prm) {
             }
           }
         }
+        long long t_ep = stall_now();
         wg_wait<0>();
         wg_fence_regs(acc[0]);
         wg_fence_regs(acc[1]);
+        stall_add(stall, signaller, kStWgWait, t_ep);
         if (held >= 0 && signaller) mbar_arrive_local(EMPTY(g, held));
         held = -1;
         if (l == NetT::kInFreeLayer && signaller) mbar_arrive_local(BAR(kBarPeFree));   // prologue may refill its block
@@ -375,8 +433,16 @@ sdf_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams prm) {
         const float acc_unscale = kAccUnscale * (1.f + prm.acc_gain_kb * (float)nkb);
         const float acc_u1 = acc_unscale * kSoftplusLog2Scale;
         if (hidden) {
+          t_ep = stall_now();
           named_sync(kBarConsumers, 256);   // both warpgroups are done reading the layer input: overwrite it in place
+          stall_add(stall, signaller, kStNamedBar, t_ep);
+          t_ep = stall_now();
           const float* bsel = (!kJvp && kNet == 0) ? bias + kNumLayers * 512 : bias;   // SDF: the b * 100 log2 e plane
+          // The loop body holds no per-element branch: an operand beyond fp16's range is reported once per layer (same tag),
+          // the diagnostics dump branches once per column group, and the activation stores are plain C++ stores (no asm
+          // memory clobber), so ptxas can overlap the bias loads and MUFU chains of neighbouring elements.  The epilogue
+          // runs with two warps per scheduler and is latency-bound.
+          bool out_of_range = false;
 #pragma unroll
           for (int t = 0; t < 2; ++t) {
             const int f_base = (2 * g + t) * 128 + 2 * c;
@@ -385,15 +451,16 @@ sdf_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams prm) {
 #pragma unroll
             for (int j = 0; j < 16; ++j) {
               const int f = f_base + 8 * j;
+              if (prm.dbg_out && prm.dbg_layer == l && tile == 0) {
+#pragma unroll
+                for (int i = 0; i < 4; ++i)
+                  prm.dbg_out[(16 * wq + (lane >> 2) + 8 * (i >> 1)) * 512 + f + (i & 1)] = acc[t][4 * j + i] * kAccUnscale;
+              }
 #pragma unroll
               for (int h = 0; h < 2; ++h) {
                 const int row = 16 * wq + (lane >> 2) + 8 * h;
                 const float r0 = acc[t][4 * j + 2 * h];
                 const float r1 = acc[t][4 * j + 2 * h + 1];
-                if (prm.dbg_out && prm.dbg_layer == l && tile == 0) {
-                  prm.dbg_out[row * 512 + f] = r0 * kAccUnscale;
-                  prm.dbg_out[row * 512 + f + 1] = r1 * kAccUnscale;
-                }
                 const float2 bb = __ldg(reinterpret_cast<const float2*>(bsel + f));
                 float v0, v1;
                 if (!kJvp && kNet == 0) {
@@ -410,20 +477,25 @@ sdf_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams prm) {
                   v0 = (kNet == 0 ? act_jvp(z0, zv0, is_value) : (zv0 > 0.f ? z0 : 0.f)) * kActScale;
                   v1 = (kNet == 0 ? act_jvp(z1, zv1, is_value) : (zv1 > 0.f ? z1 : 0.f)) * kActScale;
                 }
-                range_check2(v0, v1, prm.status, 1000 + l);
+                out_of_range |= !(fmaxf(fabsf(v0), fabsf(v1)) < 65504.f);
                 uint32_t hi, lo;
                 split2(v0, v1, hi, lo);
                 const uint32_t off = (uint32_t)(f >> 6) * 8192u + sw128_elem(row, f & 63);
-                st_shared_b32(base + kOffAHi + off, hi);
-                if (kPasses == 3) st_shared_b32(base + kOffALo + off, lo);
+                *reinterpret_cast<uint32_t*>(gbase + kOffAHi + off) = hi;
+                if (kPasses == 3) *reinterpret_cast<uint32_t*>(gbase + kOffALo + off) = lo;
               }
             }
           }
+          if (out_of_range) report_range(prm.status, 1000 + l);
           fence_proxy_async();
+          stall_add(stall, signaller, kStEpilogue, t_ep);
+          t_ep = stall_now();
           named_sync(kBarConsumers, 256);   // the next layer's input is complete
+          stall_add(stall, signaller, kStNamedBar, t_ep);
           continue;
         }
         // ---- last layer ----
+        t_ep = stall_now();
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           const int row = 16 * wq + (lane >> 2) + 8 * h;
@@ -519,8 +591,11 @@ sdf_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams prm) {
             }
           }
         }
+        stall_add(stall, signaller, kStEpilogue, t_ep);
       }
     }
+    stall_add(stall, signaller, kStConsumerTotal, t_loop);
+    stall_end(stall, signaller);
   } else {
     // ================================ prologue for the next tile ========================
     const int row = (warp - kPrologueWarp) * 32 + lane;
@@ -1046,3 +1121,19 @@ extern "C" int recmv_sdf_mlp_tc_debug(const float* x, const void* packed, const 
   return launch_tc(src, packed, pw, out_sdf, out_feat, nullptr, P, passes, dbg_layer, dbg_out, status_host,
                    (cudaStream_t)stream);
 }
+
+#if RECMV_TC_STALL_PROF
+// Diagnostics build only (see include/recmv_b200_diag.h): the stall counters summed over every launch since the last
+// reset, in the order of StallCounter.  Synchronises the device.
+extern "C" int recmv_tc_stall_profile(unsigned long long* counters, int n, int reset) {
+  if (!counters) return RECMV_E_NULL;
+  if (n < kStCounters) return RECMV_E_SHAPE;
+  cudaError_t e = cudaDeviceSynchronize();
+  if (e == cudaSuccess) e = cudaMemcpyFromSymbol(counters, g_tc_stall, sizeof(unsigned long long) * kStCounters);
+  if (e == cudaSuccess && reset) {
+    const unsigned long long zero[kStCounters] = {};
+    e = cudaMemcpyToSymbol(g_tc_stall, zero, sizeof(zero));
+  }
+  return e == cudaSuccess ? RECMV_OK : (int)e;
+}
+#endif
