@@ -186,6 +186,26 @@ RECMV_API int recmv_lbs_backward(const float* ps, const float* tps, const float*
                                  const recmv_voxel_t* vox /*host*/, const float* grad_out, float* dps, float* dtps,
                                  float* dA, float* dtrans, void* workspace, int64_t P, recmv_stream_t stream);
 
+/* VJP of the point outputs of recmv_lbs_backward (the train-phase Jacobians of utils.compute_Jacobian, differentiated
+ * again by the loss).  V(ps, tps, A, g) = (dps, dtps) of recmv_lbs_backward: dps = (T3 + Jw)^T g when tps is NULL
+ * (s = ps), else dps = T3^T g and dtps = Jw^T g, with T3 = sum_b w_b(s) A_b[:3,:3] and Jw = sum_b (A_b [ps;1]) (x)
+ * grad w_b(s).  Cotangents: cot_ps u [P,3] of dps and cot_tps v [P,3] of dtps (tps form only; v' = u when tps is
+ * NULL).  At least one is needed; a missing one is zero.  Outputs, each may be NULL, and dropping one changes no bit
+ * of another:
+ *   d_grad_out [P,3]       = T3 u + Jw v'
+ *   dps        [P,3]       = sum_b (grad w_b . v') A_b3^T g, plus dtps's term when tps is NULL
+ *   dtps       [P,3]       = sum_b (g^T A_b3 u) grad w_b + sum_b (g . A_b [ps;1]) H_b v'   (H_b: Hessian of w_b; a
+ *                            clamped axis contributes zero, as to the first derivative)
+ *   dA         [F,24,4,4]  dA_f[b] rows 0..2 = sum over the points of frame f of g (w_b [u;0] + (grad w_b . v') [ps;1])^T;
+ *                          row 3 is zero
+ * Frames, the workspace (recmv_lbs_backward_workspace_bytes, needed for dA) and the deterministic chunked reduce are
+ * those of recmv_lbs_backward.  cot_tps or dtps without tps is rejected.                                           */
+RECMV_API int recmv_lbs_vjp_backward(const float* ps, const float* tps, const float* A, const int64_t* batch_inds,
+                                     int64_t points_per_frame, int num_frames, const recmv_voxel_t* vox /*host*/,
+                                     const float* grad_out, const float* cot_ps, const float* cot_tps,
+                                     float* d_grad_out, float* dps, float* dtps, float* dA, void* workspace, int64_t P,
+                                     recmv_stream_t stream);
+
 /* ---- A1+A2: Embedder + ImplicitNetwork.forward -------------------------------------------------
  * replaces model/Embedder.py:43-50 + model/network.py:89-119 (+ utils/utils.py:40-46 weights).
  * Network shape is the reference's getTmpSdf: PE(6) 39 -> 512 x3 -> 473 (+39 skip)/sqrt2 -> 512 x4

@@ -187,11 +187,15 @@ __device__ __forceinline__ bool inverse_lbs_point(const Voxel& v, const float* _
 // whose coordinate was clamped).  Evaluated corner by corner -- T_c = sum_b ws[corner][b] A_b, Y_c = T_c [q;1] --
 // so nothing of size 24 x 3 is ever live in registers.
 //
-// lbs_blend_jac is the shared core: the weights are sampled at s and the blended transform is applied to a (the
-// `[tps, ps]` form of LBSkinner.repose samples at tps and moves ps).  It returns T (rows 0..2 of sum_b w_b A_b) and
-// only the weight term Jw_ij = sum_b (A_b [a;1])_i * d w_b / d s_j; lbs_forward_jac is the case s = a.
-__device__ __forceinline__ void lbs_blend_jac(const Voxel& v, const float* __restrict__ Af, float sx, float sy,
-                                              float sz, float qx, float qy, float qz, float T[12], float J[9]) {
+// The trilinear cell around the sampling point s with the sampler's clamp rule: corner indices, per-axis weights
+// (corner weight = wx[dx] wy[dy] wz[dz]) and d i / d s per axis, zero on an axis whose coordinate was clamped.
+struct SkinCell {
+  int xs[2], ys[2], zs[2];
+  float wx[2], wy[2], wz[2];
+  float mx, my, mz;
+};
+
+__device__ __forceinline__ void skin_cell(const Voxel& v, float sx, float sy, float sz, SkinCell& k) {
   float gx = (sx - v.cx) / v.ext * 2.f;
   float gy = (sy - v.cy) / v.ext * 2.f;
   float gz = (sz - v.cz) / v.ext * 2.f;
@@ -202,13 +206,26 @@ __device__ __forceinline__ void lbs_blend_jac(const Voxel& v, const float* __res
   if (!(ix == ix)) { ix = 0.f; mx = 0.f; }
   if (!(iy == iy)) { iy = 0.f; my = 0.f; }
   if (!(iz == iz)) { iz = 0.f; mz = 0.f; }
-  mx *= (float)v.W / v.ext; my *= (float)v.H / v.ext; mz *= (float)v.D / v.ext;   // d i / d q
+  k.mx = mx * ((float)v.W / v.ext); k.my = my * ((float)v.H / v.ext); k.mz = mz * ((float)v.D / v.ext);   // d i / d s
   int x0 = (int)floorf(ix), y0 = (int)floorf(iy), z0 = (int)floorf(iz);
-  int x1 = min(x0 + 1, v.W - 1), y1 = min(y0 + 1, v.H - 1), z1 = min(z0 + 1, v.D - 1);
-  const float wx[2] = {(float)(x0 + 1) - ix, ix - (float)x0};
-  const float wy[2] = {(float)(y0 + 1) - iy, iy - (float)y0};
-  const float wz[2] = {(float)(z0 + 1) - iz, iz - (float)z0};
-  const int xs[2] = {x0, x1}, ys[2] = {y0, y1}, zs[2] = {z0, z1};
+  k.xs[0] = x0; k.xs[1] = min(x0 + 1, v.W - 1);
+  k.ys[0] = y0; k.ys[1] = min(y0 + 1, v.H - 1);
+  k.zs[0] = z0; k.zs[1] = min(z0 + 1, v.D - 1);
+  k.wx[0] = (float)(x0 + 1) - ix; k.wx[1] = ix - (float)x0;
+  k.wy[0] = (float)(y0 + 1) - iy; k.wy[1] = iy - (float)y0;
+  k.wz[0] = (float)(z0 + 1) - iz; k.wz[1] = iz - (float)z0;
+}
+
+// lbs_blend_jac is the shared core: the weights are sampled at s and the blended transform is applied to a (the
+// `[tps, ps]` form of LBSkinner.repose samples at tps and moves ps).  It returns T (rows 0..2 of sum_b w_b A_b) and
+// only the weight term Jw_ij = sum_b (A_b [a;1])_i * d w_b / d s_j; lbs_forward_jac is the case s = a.
+__device__ __forceinline__ void lbs_blend_jac(const Voxel& v, const float* __restrict__ Af, float sx, float sy,
+                                              float sz, float qx, float qy, float qz, float T[12], float J[9]) {
+  SkinCell k;
+  skin_cell(v, sx, sy, sz, k);
+  const float mx = k.mx, my = k.my, mz = k.mz;
+  const float* wx = k.wx; const float* wy = k.wy; const float* wz = k.wz;
+  const int* xs = k.xs; const int* ys = k.ys; const int* zs = k.zs;
 #pragma unroll
   for (int e = 0; e < 12; ++e) T[e] = 0.f;
 #pragma unroll

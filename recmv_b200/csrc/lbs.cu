@@ -306,6 +306,64 @@ __host__ inline size_t lbs_bwd_layout(int64_t P, int nf, size_t* off_frame, size
   return *off_n + (size_t)chunks * sizeof(int);
 }
 
+// Slots of one chunk, called by all kBwdChunk threads (t < n owns point t of frame f): the first point of each frame
+// in the chunk opens a slot, numbered in order of appearance; every point learns its slot, every slot its frame.
+__device__ __forceinline__ void lbs_chunk_slots(int t, int n, int f, int* s_frame, int* s_slot, unsigned char* s_opens,
+                                                int* s_warp_first, const LbsBwdWorkspace& ws, int64_t chunk,
+                                                int slots) {
+  s_frame[t] = t < n ? f : -1;
+  __syncthreads();
+  int first = t;
+  if (t < n) {
+    for (int j = 0; j < t; ++j)
+      if (s_frame[j] == f) { first = j; break; }
+  }
+  const bool opens = t < n && first == t;
+  s_opens[t] = opens ? 1 : 0;
+  const unsigned ball = __ballot_sync(0xffffffffu, opens);
+  if ((t & 31) == 0) s_warp_first[t >> 5] = __popc(ball);
+  __syncthreads();
+  if (t == 0) {
+    int run = 0;
+    for (int k = 0; k < kBwdChunk / 32; ++k) { const int c = s_warp_first[k]; s_warp_first[k] = run; run += c; }
+    ws.nslots[chunk] = run;
+  }
+  __syncthreads();
+  if (opens) {
+    const int my_slot = s_warp_first[t >> 5] + __popc(ball & ((1u << (t & 31)) - 1u));
+    s_slot[t] = my_slot;
+    ws.slot_frame[chunk * slots + my_slot] = f;
+  }
+  __syncthreads();
+  if (t < n && !opens) s_slot[t] = s_slot[first];
+  __syncthreads();
+}
+
+// Flush of one chunk's records `rec` (entries 0..nentries-1): thread e owns entry e of every record and walks the
+// points in order, term(e) giving the per-point step acc -> acc'.  A run that starts at the point opening its slot
+// stores, later runs of the same frame add.
+template <typename EntryTerm>
+__device__ __forceinline__ void lbs_chunk_flush(int t, int n, int nentries, const int* s_slot,
+                                                const unsigned char* s_opens, float* rec, EntryTerm term) {
+  for (int e = t; e < nentries; e += kBwdChunk) {
+    const auto step = term(e);
+    float acc = 0.f;
+    int start = 0;
+    for (int i = 0; i < n; ++i) {
+      if (s_slot[i] != s_slot[start]) {
+        float* d = rec + (size_t)s_slot[start] * kRecStride + e;
+        *d = s_opens[start] ? acc : *d + acc;
+        acc = 0.f; start = i;
+      }
+      acc = step(i, acc);
+    }
+    if (n > 0) {
+      float* d = rec + (size_t)s_slot[start] * kRecStride + e;
+      *d = s_opens[start] ? acc : *d + acc;
+    }
+  }
+}
+
 __global__ void __launch_bounds__(kBwdChunk) lbs_bwd_chunk_kernel(
     const float* __restrict__ ps, const float* __restrict__ tps, const float* __restrict__ A,
     const int64_t* __restrict__ batch_inds, int64_t ppf, int nf, Voxel vox,
@@ -366,56 +424,158 @@ __global__ void __launch_bounds__(kBwdChunk) lbs_bwd_chunk_kernel(
     ga[0] = g0; ga[1] = g1; ga[2] = g2; ga[3] = ax; ga[4] = ay; ga[5] = az; ga[6] = 1.f;
   }
   if (!reduce) return;
-  s_frame[t] = t < n ? f : -1;
-  __syncthreads();
-  // slots: the first point of each frame in the chunk opens a slot, numbered in order of appearance
-  int first = t;
-  if (t < n) {
-    for (int j = 0; j < t; ++j)
-      if (s_frame[j] == f) { first = j; break; }
-  }
-  const bool opens = t < n && first == t;
-  s_opens[t] = opens ? 1 : 0;
-  const unsigned ball = __ballot_sync(0xffffffffu, opens);
-  if ((t & 31) == 0) s_warp_first[t >> 5] = __popc(ball);
-  __syncthreads();
-  if (t == 0) {
-    int run = 0;
-    for (int k = 0; k < kBwdChunk / 32; ++k) { const int c = s_warp_first[k]; s_warp_first[k] = run; run += c; }
-    ws.nslots[chunk] = run;
-  }
-  __syncthreads();
-  if (opens) {
-    const int my_slot = s_warp_first[t >> 5] + __popc(ball & ((1u << (t & 31)) - 1u));
-    s_slot[t] = my_slot;
-    ws.slot_frame[chunk * slots + my_slot] = f;
-  }
-  __syncthreads();
-  if (t < n && !opens) s_slot[t] = s_slot[first];
-  __syncthreads();
-  // thread e owns entry e of every record of this chunk; a run that starts at the point opening its slot stores,
-  // later runs of the same frame add
-  float* rec = ws.rec + (size_t)chunk * slots * kRecStride;
-  for (int e = t; e < kRecEntries; e += kBwdChunk) {
+  lbs_chunk_slots(t, n, f, s_frame, s_slot, s_opens, s_warp_first, ws, chunk, slots);
+  lbs_chunk_flush(t, n, kRecEntries, s_slot, s_opens, ws.rec + (size_t)chunk * slots * kRecStride, [&](int e) {
     const bool is_dA = e < 288;
     const int j = is_dA ? e / 12 : 0, r = is_dA ? (e >> 2) % 3 : e - 288, c = is_dA ? (e & 3) : 3;
-    float acc = 0.f;
-    int start = 0;
-    for (int i = 0; i < n; ++i) {
-      if (s_slot[i] != s_slot[start]) {
-        float* d = rec + (size_t)s_slot[start] * kRecStride + e;
-        *d = s_opens[start] ? acc : *d + acc;
-        acc = 0.f; start = i;
-      }
+    return [=](int i, float acc) {
       const float* ga = s_ga + i * 8;
-      if (is_dA) acc = fmaf(s_w[i * 25 + j], ga[r] * ga[3 + c], acc);
-      else acc += ga[r];
+      return is_dA ? fmaf(s_w[i * 25 + j], ga[r] * ga[3 + c], acc) : acc + ga[r];
+    };
+  });
+}
+
+// Second-order skinning backward: the VJP of (dps, dtps) = V(ps, tps, A, g) of lbs_bwd_chunk_kernel.  With cotangents
+// u (of dps) and v (of dtps; v' = u when s = a) it differentiates phi = g^T T3 u + g^T Jw v':
+//   d g = T3 u + Jw v'
+//   d a = sum_b (grad w_b . v') A_b3^T g
+//   d s = sum_b (g^T A_b3 u) grad w_b + sum_b (g . A_b a') H_b v'       (H_b: Hessian of the trilinear weight)
+//   dA_b (rows 0..2) = g (w_b u' + (grad w_b . v') a')^T
+// corner by corner like lbs_blend_jac: with T_c = sum_b ws[c][b] A_b, every sum over b becomes a sum over the eight
+// corners of the corner weight (or its gradient, or its Hessian, whose only nonzero entries are the mixed partials)
+// times a product with T_c.  w_b and gw_b = grad w_b . v' are accumulated in this thread's shared-memory row for the dA
+// records, which go through the same slots and reduce as lbs_bwd_chunk_kernel.
+constexpr int kVjpRow = 25;                                       // w / gw rows padded to 25 floats
+constexpr int kVjpStage = 12;                                     // g 0 | u 0 | a 1
+constexpr size_t kVjpSmem = (size_t)kBwdChunk * (2 * kVjpRow + kVjpStage) * sizeof(float);
+
+__global__ void __launch_bounds__(kBwdChunk) lbs_vjp_bwd_chunk_kernel(
+    const float* __restrict__ ps, const float* __restrict__ tps, const float* __restrict__ A,
+    const int64_t* __restrict__ batch_inds, int64_t ppf, int nf, Voxel vox, const float* __restrict__ grad_out,
+    const float* __restrict__ cot_ps, const float* __restrict__ cot_tps, float* __restrict__ d_grad_out,
+    float* __restrict__ dps, float* __restrict__ dtps, LbsBwdWorkspace ws, int slots, int reduce, int64_t P) {
+  extern __shared__ float4 s_dyn4[];
+  float* s_w = reinterpret_cast<float*>(s_dyn4);
+  float* s_gw = s_w + kBwdChunk * kVjpRow;
+  float* s_st = s_gw + kBwdChunk * kVjpRow;
+  __shared__ int s_frame[kBwdChunk];
+  __shared__ int s_slot[kBwdChunk];
+  __shared__ unsigned char s_opens[kBwdChunk];
+  __shared__ int s_warp_first[kBwdChunk / 32];
+  const int t = threadIdx.x;
+  const int64_t chunk = blockIdx.x;
+  const int64_t p = chunk * kBwdChunk + t;
+  const int n = (int)min((int64_t)kBwdChunk, P - chunk * kBwdChunk);
+  int f = 0;
+  if (t < n) {
+    const float ax = ps[3 * p], ay = ps[3 * p + 1], az = ps[3 * p + 2];
+    float sx = ax, sy = ay, sz = az;
+    if (tps) { sx = tps[3 * p]; sy = tps[3 * p + 1]; sz = tps[3 * p + 2]; }
+    float g[3] = {0.f, 0.f, 0.f}, u[3] = {0.f, 0.f, 0.f}, v[3];
+    if (grad_out) { g[0] = grad_out[3 * p]; g[1] = grad_out[3 * p + 1]; g[2] = grad_out[3 * p + 2]; }
+    if (cot_ps) { u[0] = cot_ps[3 * p]; u[1] = cot_ps[3 * p + 1]; u[2] = cot_ps[3 * p + 2]; }
+    if (!tps) {
+      v[0] = u[0]; v[1] = u[1]; v[2] = u[2];
+    } else if (cot_tps) {
+      v[0] = cot_tps[3 * p]; v[1] = cot_tps[3 * p + 1]; v[2] = cot_tps[3 * p + 2];
+    } else {
+      v[0] = 0.f; v[1] = 0.f; v[2] = 0.f;
     }
-    if (n > 0) {
-      float* d = rec + (size_t)s_slot[start] * kRecStride + e;
-      *d = s_opens[start] ? acc : *d + acc;
+    f = frame_of(batch_inds, p, ppf, nf);
+    const float* Af = A + (size_t)f * 24 * 16;
+    float* sw = s_w + t * kVjpRow;
+    float* sgw = s_gw + t * kVjpRow;
+    if (reduce) {
+#pragma unroll
+      for (int b = 0; b < 24; ++b) { sw[b] = 0.f; sgw[b] = 0.f; }
     }
+    SkinCell k;
+    skin_cell(vox, sx, sy, sz, k);
+    float dg[3] = {0.f, 0.f, 0.f}, da[3] = {0.f, 0.f, 0.f}, ds[3] = {0.f, 0.f, 0.f};
+    float Y0[3] = {0.f, 0.f, 0.f}, q0[3] = {0.f, 0.f, 0.f}, gY0 = 0.f, gTu0 = 0.f;
+#pragma unroll 1
+    for (int c = 0; c < 8; ++c) {
+      const int dx = c & 1, dy = (c >> 1) & 1, dz = c >> 2;
+      const float wx = dx ? k.wx[1] : k.wx[0], wy = dy ? k.wy[1] : k.wy[0], wz = dz ? k.wz[1] : k.wz[0];
+      const float ex = (dx ? 1.f : -1.f) * k.mx, ey = (dy ? 1.f : -1.f) * k.my, ez = (dz ? 1.f : -1.f) * k.mz;
+      const float cw = wx * wy * wz;
+      const float dcx = ex * wy * wz, dcy = ey * wx * wz, dcz = ez * wx * wy;   // grad of the corner weight
+      const float hxy = ex * ey * wz, hxz = ex * ez * wy, hyz = ey * ez * wx;    // its mixed second partials
+      const float dv = dcx * v[0] + dcy * v[1] + dcz * v[2];
+      const int zi = dz ? k.zs[1] : k.zs[0], yi = dy ? k.ys[1] : k.ys[0], xi = dx ? k.xs[1] : k.xs[0];
+      const float* wsp = vox.ws + (((size_t)zi * vox.H + yi) * vox.W + xi) * 24;
+      float Tc[12];
+#pragma unroll
+      for (int e = 0; e < 12; ++e) Tc[e] = 0.f;
+#pragma unroll 4
+      for (int b = 0; b < 24; ++b) {
+        const float wb = __ldg(wsp + b);
+        const float4* a4 = reinterpret_cast<const float4*>(Af + b * 16);
+        const float4 r0 = __ldg(a4), r1 = __ldg(a4 + 1), r2 = __ldg(a4 + 2);
+        Tc[0] = fmaf(wb, r0.x, Tc[0]); Tc[1] = fmaf(wb, r0.y, Tc[1]); Tc[2] = fmaf(wb, r0.z, Tc[2]); Tc[3] = fmaf(wb, r0.w, Tc[3]);
+        Tc[4] = fmaf(wb, r1.x, Tc[4]); Tc[5] = fmaf(wb, r1.y, Tc[5]); Tc[6] = fmaf(wb, r1.z, Tc[6]); Tc[7] = fmaf(wb, r1.w, Tc[7]);
+        Tc[8] = fmaf(wb, r2.x, Tc[8]); Tc[9] = fmaf(wb, r2.y, Tc[9]); Tc[10] = fmaf(wb, r2.z, Tc[10]); Tc[11] = fmaf(wb, r2.w, Tc[11]);
+        if (reduce) { sw[b] = fmaf(wb, cw, sw[b]); sgw[b] = fmaf(wb, dv, sgw[b]); }
+      }
+      float Y[3], Tu[3], q[3];
+#pragma unroll
+      for (int i = 0; i < 3; ++i) {
+        Y[i] = Tc[4 * i] * ax + Tc[4 * i + 1] * ay + Tc[4 * i + 2] * az + Tc[4 * i + 3];
+        Tu[i] = Tc[4 * i] * u[0] + Tc[4 * i + 1] * u[1] + Tc[4 * i + 2] * u[2];
+        q[i] = g[0] * Tc[i] + g[1] * Tc[4 + i] + g[2] * Tc[8 + i];   // (T_c3^T g)_i
+      }
+      float gY = g[0] * Y[0] + g[1] * Y[1] + g[2] * Y[2];
+      float gTu = q[0] * u[0] + q[1] * u[1] + q[2] * u[2];
+      // the gradients and Hessians of the eight corner weights each sum to zero, so corner 0's values are taken off
+      // every corner's before they are weighted: the sums then add up small differences instead of cancelling terms
+      // of the size of T_c [a;1]
+      if (c == 0) {
+#pragma unroll
+        for (int i = 0; i < 3; ++i) { Y0[i] = Y[i]; q0[i] = q[i]; }
+        gY0 = gY; gTu0 = gTu;
+      }
+      gY -= gY0; gTu -= gTu0;
+      const float Hv[3] = {hxy * v[1] + hxz * v[2], hxy * v[0] + hyz * v[2], hxz * v[0] + hyz * v[1]};
+      const float dc[3] = {dcx, dcy, dcz};
+#pragma unroll
+      for (int i = 0; i < 3; ++i) {
+        dg[i] = fmaf(cw, Tu[i], fmaf(dv, Y[i] - Y0[i], dg[i]));
+        da[i] = fmaf(dv, q[i] - q0[i], da[i]);
+        ds[i] = fmaf(gTu, dc[i], fmaf(gY, Hv[i], ds[i]));
+      }
+    }
+    if (d_grad_out) {
+#pragma unroll
+      for (int i = 0; i < 3; ++i) d_grad_out[3 * p + i] = dg[i];
+    }
+    if (tps) {
+      if (dps) {
+#pragma unroll
+        for (int i = 0; i < 3; ++i) dps[3 * p + i] = da[i];
+      }
+      if (dtps) {
+#pragma unroll
+        for (int i = 0; i < 3; ++i) dtps[3 * p + i] = ds[i];
+      }
+    } else if (dps) {
+#pragma unroll
+      for (int i = 0; i < 3; ++i) dps[3 * p + i] = da[i] + ds[i];
+    }
+    float* st = s_st + t * kVjpStage;
+    st[0] = g[0]; st[1] = g[1]; st[2] = g[2]; st[3] = 0.f;
+    st[4] = u[0]; st[5] = u[1]; st[6] = u[2]; st[7] = 0.f;
+    st[8] = ax; st[9] = ay; st[10] = az; st[11] = 1.f;
   }
+  if (!reduce) return;
+  lbs_chunk_slots(t, n, f, s_frame, s_slot, s_opens, s_warp_first, ws, chunk, slots);
+  // dA entries only: the record's dtrans entries are left as they are and the reduce is run without dtrans
+  lbs_chunk_flush(t, n, 288, s_slot, s_opens, ws.rec + (size_t)chunk * slots * kRecStride, [&](int e) {
+    const int j = e / 12, r = (e >> 2) % 3, c = e & 3;
+    return [=](int i, float acc) {
+      const float* st = s_st + i * kVjpStage;
+      return fmaf(st[r], fmaf(s_w[i * kVjpRow + j], st[4 + c], s_gw[i * kVjpRow + j] * st[8 + c]), acc);
+    };
+  });
 }
 
 __global__ void __launch_bounds__(1024) lbs_bwd_reduce_kernel(LbsBwdWorkspace ws, int slots, int64_t chunks,
@@ -551,6 +711,57 @@ extern "C" int recmv_lbs_backward(const float* ps, const float* tps, const float
   if (reduce) {
     lbs_bwd_reduce_kernel<<<dim3((unsigned)num_frames, (kRecEntries + 31) / 32), dim3(32, 32), 0, st>>>(
         ws, slots, chunks, dA, dtrans);
+    s = launch_status();
+  }
+  return s;
+}
+
+extern "C" int recmv_lbs_vjp_backward(const float* ps, const float* tps, const float* A, const int64_t* batch_inds,
+                                      int64_t points_per_frame, int num_frames, const recmv_voxel_t* vox,
+                                      const float* grad_out, const float* cot_ps, const float* cot_tps,
+                                      float* d_grad_out, float* dps, float* dtps, float* dA, void* workspace, int64_t P,
+                                      recmv_stream_t stream) {
+  int s = lbs_check(vox, num_frames, P);
+  if (s) return s;
+  if (!tps && (cot_tps || dtps)) return RECMV_E_NULL;
+  const int reduce = dA ? 1 : 0;
+  const int64_t chunks = (P + kBwdChunk - 1) / kBwdChunk;
+  if (chunks > 0x7fffffff) return RECMV_E_RANGE;
+  const bool per_point = d_grad_out || dps || dtps || reduce;
+  if (P > 0 && per_point) {
+    if (!ps || !A) return RECMV_E_NULL;
+    if ((dps || dtps || reduce) && !grad_out) return RECMV_E_NULL;   // every output but d_grad_out is linear in g
+    if (!cot_ps && !cot_tps) return RECMV_E_NULL;
+  }
+  if (reduce && P > 0 && !workspace) return RECMV_E_NULL;
+  if (((uintptr_t)workspace & 15) != 0) return RECMV_E_SHAPE;
+  size_t off_frame, off_n;
+  lbs_bwd_layout(P, num_frames, &off_frame, &off_n);
+  LbsBwdWorkspace ws;
+  ws.rec = (float*)workspace;
+  ws.slot_frame = (int*)((char*)workspace + off_frame);
+  ws.nslots = (int*)((char*)workspace + off_n);
+  const int slots = (int)lbs_bwd_slots(num_frames);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (P > 0 && per_point) {
+    static int smem_set[16] = {0};   // per device
+    int dev = 0;
+    cudaGetDevice(&dev);
+    if (!smem_set[dev & 15]) {
+      cudaError_t e = cudaFuncSetAttribute(lbs_vjp_bwd_chunk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                           (int)kVjpSmem);
+      if (e != cudaSuccess) { cudaGetLastError(); return (int)e; }
+      smem_set[dev & 15] = 1;
+    }
+    lbs_vjp_bwd_chunk_kernel<<<(unsigned)chunks, kBwdChunk, kVjpSmem, st>>>(
+        ps, tps, A, batch_inds, points_per_frame, num_frames, to_voxel(vox), grad_out, cot_ps, cot_tps, d_grad_out,
+        dps, dtps, ws, slots, reduce, P);
+    s = launch_status();
+    if (s) return s;
+  }
+  if (reduce) {
+    lbs_bwd_reduce_kernel<<<dim3((unsigned)num_frames, (kRecEntries + 31) / 32), dim3(32, 32), 0, st>>>(
+        ws, slots, chunks, dA, nullptr);
     s = launch_status();
   }
   return s;

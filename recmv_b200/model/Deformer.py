@@ -10,6 +10,9 @@ LBSkinner.forward:
   * poses or translations that require grad (training) -> ops.LbsTrainFunction: the same forward kernel, and one
     backward kernel for the point / pose / translation gradients, on a chain built and differentiated by kernels
     (ops.BoneMatricesFunction);
+    A create_graph backward for the point gradients only (utils.compute_Jacobian) with `second_order_fused` gives
+    differentiable point gradients on the device (ops.LbsVjpFunction); any other create_graph backward differentiates
+    the composite below;
   * otherwise with autograd (only the points, or train_fused = False, or a create_graph backward) -> the CUDA
     GridSamplerMine3dFunction (twice differentiable) + batched blend, without the reference's per-frame python loop and
     its `.item()` sync (Deformer.py:438-444).
@@ -244,11 +247,15 @@ class LBSkinner(nn.Module):
         self._bbox_key, self._bbox_host = None, None
         self._parents_i32 = None
         self.train_fused = True   # poses / trans that require grad: kernel chain + ops.LbsTrainFunction (False: torch graph)
+        # the train-phase Jacobians (create_graph, input gradients only) through ops.LbsVjpFunction instead of the
+        # composite's torch graph
+        self.second_order_fused = False
         self.last_path = None
 
     @property
     def last_backward(self):
-        """Which backward branch of ops.LbsTrainFunction ran last: "fused" or "autograd-composite (create_graph)"."""
+        """Which backward branch of ops.LbsTrainFunction ran last: "fused", "fused (create_graph, input gradient)" or
+        "autograd-composite (create_graph)"."""
         return ops.LbsTrainFunction.last_backward
 
     def bbox_size(self):
@@ -420,7 +427,8 @@ class LBSkinner(nn.Module):
                 assert (batch_size == ps.shape[0])
             return ops.LbsTrainFunction.apply(p32, t32, A.float(), trans.float().contiguous(), bi,
                                               (self.ws_channels_last(), center, extend),
-                                              lambda p, t, a, tr: self._composite(p, p if t is None else t, a, tr, bi))
+                                              lambda p, t, a, tr: self._composite(p, p if t is None else t, a, tr, bi),
+                                              self.second_order_fused)
         self.last_path = "autograd-composite"
         return self._composite(ps, tps, A, trans, batch_inds)
 

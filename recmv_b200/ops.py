@@ -496,29 +496,109 @@ def lbs_backward(ps, A, grad_out, ws_cl, center, extend, batch_inds=None, points
     return dps, dtps, dA, dtrans
 
 
+def lbs_vjp_backward(ps, A, grad_out, ws_cl, center, extend, batch_inds=None, points_per_frame=0, tps=None,
+                     cot_ps=None, cot_tps=None, want_grad_out=True, want_ps=True, want_tps=True, want_A=True):
+    """(d_grad_out, dps, dtps, dA) of the point outputs (dps, dtps) of lbs_backward, for their cotangents cot_ps /
+    cot_tps [P,3] (recmv_lbs_vjp_backward; a missing cotangent is zero, cot_tps needs tps).  An output that is not
+    wanted (or dtps without tps) is None."""
+    ps = ps.contiguous().float()
+    A = A.contiguous().float()
+    g = grad_out.contiguous().float()
+    P = ps.numel() // 3
+    F_ = int(A.shape[0])
+    dev = ps.device
+    if tps is not None:
+        tps = tps.contiguous().float()
+    else:
+        cot_tps = None
+    if batch_inds is not None:
+        batch_inds = batch_inds.contiguous().long()
+    if cot_ps is None and cot_tps is None:
+        cot_ps = torch.zeros_like(ps)
+    cot_ps = cot_ps.contiguous().float() if cot_ps is not None else None
+    cot_tps = cot_tps.contiguous().float() if cot_tps is not None else None
+    dg = torch.empty((P, 3), dtype=torch.float32, device=dev) if want_grad_out else None
+    dps = torch.empty((P, 3), dtype=torch.float32, device=dev) if want_ps else None
+    dtps = torch.empty((P, 3), dtype=torch.float32, device=dev) if want_tps and tps is not None else None
+    dA = torch.empty((F_, 24, 4, 4), dtype=torch.float32, device=dev) if want_A else None
+    lib = _lib.load()
+    work = None
+    if want_A:
+        nbytes = c_size_t(0)
+        check(lib.recmv_lbs_backward_workspace_bytes(P, F_, byref(nbytes)), "recmv_lbs_backward_workspace_bytes")
+        work = torch.empty((max(int(nbytes.value), 16),), dtype=torch.uint8, device=dev)
+    vox = make_voxel(ws_cl, center, extend)
+    with torch.cuda.device(dev):
+        check(lib.recmv_lbs_vjp_backward(_ptr(ps), _ptr(tps), _ptr(A), _ptr(batch_inds), int(points_per_frame), F_,
+                                         byref(vox), _ptr(g), _ptr(cot_ps), _ptr(cot_tps), _ptr(dg), _ptr(dps),
+                                         _ptr(dtps), _ptr(dA), _ptr(work), P, _stream(ps)), "recmv_lbs_vjp_backward")
+    return dg, dps, dtps, dA
+
+
+class LbsVjpFunction(torch.autograd.Function):
+    """(dps, dtps) = the point gradients of lbs_backward for the cotangent g, as a differentiable op: forward
+    recmv_lbs_backward with only dps / dtps, backward recmv_lbs_vjp_backward (d g, d ps, d tps, d A).  ps / tps / g
+    [P,3] fp32, A [F,24,4,4]; dtps is None when tps is None.  This is the create_graph backward of LbsTrainFunction for
+    input gradients (the train-phase Jacobians); its own backward is first order."""
+
+    @staticmethod
+    def forward(ctx, ps, tps, A, g, batch_inds, ppf, skin):
+        ws_cl, center, extend = skin
+        dps, dtps, _, _ = lbs_backward(ps, A, g, ws_cl, center, extend, batch_inds, ppf, tps, want_ps=True,
+                                       want_tps=True, want_A=False, want_trans=False)
+        ctx.save_for_backward(ps, tps, A, g, batch_inds)
+        ctx.skin, ctx.ppf = skin, ppf
+        return dps, dtps
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, u, v):
+        ps, tps, A, g, batch_inds = ctx.saved_tensors
+        need = ctx.needs_input_grad
+        want_tps = need[1] and tps is not None
+        if not (need[0] or want_tps or need[2] or need[3]):
+            return None, None, None, None, None, None, None
+        ws_cl, center, extend = ctx.skin
+        dg, dps, dtps, dA = lbs_vjp_backward(ps, A, g, ws_cl, center, extend, batch_inds, ctx.ppf, tps, u,
+                                             v if tps is not None else None, want_grad_out=need[3], want_ps=need[0],
+                                             want_tps=want_tps, want_A=need[2])
+        return dps, dtps, dA, dg, None, None, None
+
+
 class LbsTrainFunction(torch.autograd.Function):
     """LBSkinner.forward with gradients for the poses / translations (and the points): forward recmv_lbs_fwd, backward
     recmv_lbs_backward (weights resampled, not kept in the graph).  ps [...,3] contiguous fp32 ([N,V,3] with frame = row,
     or [P,3] with batch_inds); tps None or the sampling points of the `[tps, ps]` form; A [F,24,4,4]; trans [F,3].
-    `skin` = (ws_cl, center, extend).  A backward under create_graph (the train-phase Jacobians of utils) evaluates
-    `composite(ps, tps, A, trans)` -- the torch-sampler graph of LBSkinner -- on the saved inputs and differentiates it
-    with create_graph=True; `last_backward` says which branch ran."""
+    `skin` = (ws_cl, center, extend).  A backward under create_graph (the train-phase Jacobians of utils) that asks for
+    input gradients only (`input_grad_only()`), with `second_order_fused`, returns LbsVjpFunction's differentiable point
+    gradients; any other backward under create_graph evaluates `composite(ps, tps, A, trans)` -- the torch-sampler graph
+    of LBSkinner -- on the saved inputs and differentiates it with create_graph=True.  `last_backward` says which branch
+    ran."""
     last_backward = None
 
     @staticmethod
-    def forward(ctx, ps, tps, A, trans, batch_inds, skin, composite):
+    def forward(ctx, ps, tps, A, trans, batch_inds, skin, composite, second_order_fused=False):
         ws_cl, center, extend = skin
         ppf = 0 if batch_inds is not None else ps.shape[1]
         out = lbs_forward(ps.reshape(-1, 3), A, trans, ws_cl, center, extend, batch_inds, ppf,
                           None if tps is None else tps.reshape(-1, 3))
         ctx.save_for_backward(ps, tps, A, trans, batch_inds)
         ctx.skin, ctx.composite, ctx.ppf = skin, composite, ppf
+        ctx.second_order_fused = second_order_fused
         return out.view(ps.shape)
 
     @staticmethod
     def backward(ctx, g):
         ps, tps, A, trans, batch_inds = ctx.saved_tensors
         need = ctx.needs_input_grad
+        if torch.is_grad_enabled() and ctx.second_order_fused and _inputs_only(need[2] or need[3]):
+            # create_graph=True for the point gradients only: (dps, dtps) as a differentiable op on the device
+            LbsTrainFunction.last_backward = "fused (create_graph, input gradient)"
+            dps, dtps = LbsVjpFunction.apply(ps.reshape(-1, 3), None if tps is None else tps.reshape(-1, 3), A,
+                                             g.reshape(-1, 3), batch_inds, ctx.ppf, ctx.skin)
+            dps = dps.view(ps.shape) if need[0] else None
+            dtps = dtps.view(tps.shape) if (dtps is not None and need[1]) else None
+            return dps, dtps, None, None, None, None, None, None
         if torch.is_grad_enabled():
             LbsTrainFunction.last_backward = "autograd-composite (create_graph)"
             args = [ps, tps, A, trans]
@@ -528,7 +608,7 @@ class LbsTrainFunction(torch.autograd.Function):
                 diff = [t for t in ins if t is not None and t.requires_grad]
                 gr = iter(torch.autograd.grad([out], diff, [g], create_graph=True, allow_unused=True))
             res = [next(gr) if (t is not None and t.requires_grad) else None for t in ins]
-            return (*[r if n else None for r, n in zip(res, need[:4])], None, None, None)
+            return (*[r if n else None for r, n in zip(res, need[:4])], None, None, None, None)
         LbsTrainFunction.last_backward = "fused"
         ws_cl, center, extend = ctx.skin
         dps, dtps, dA, dtrans = lbs_backward(ps.reshape(-1, 3), A, g.reshape(-1, 3), ws_cl, center, extend, batch_inds,
@@ -536,7 +616,7 @@ class LbsTrainFunction(torch.autograd.Function):
                                              want_tps=need[1], want_A=need[2], want_trans=need[3])
         dps = dps.view(ps.shape) if dps is not None else None
         dtps = dtps.view(tps.shape) if dtps is not None else None
-        return dps, dtps, dA, dtrans, None, None, None
+        return dps, dtps, dA, dtrans, None, None, None, None
 
 
 # --------------------------------------------------------------------------------------------------
