@@ -686,14 +686,12 @@ def sdf_value_and_grad(x, packed, pe_w=None, mode=None, want_feat=False):
 
 
 # --------------------------------------------------------------------------------------------------
-# Training path: layer GEMMs that save their outputs for the backward (csrc/gemm3_tma.cu, first generation csrc/gemm3.cu)
+# Training path: layer GEMMs that save their outputs for the backward (csrc/gemm3_tma.cu)
 # --------------------------------------------------------------------------------------------------
+# Activation codes of the fp32-operand entries of csrc/gemm3.cu (mlp_fwd_layer, mlp_bwd_data_layer), which the ReLU
+# networks' create_graph input gradient (second_order.PlainMlpInputGradFunction) still runs on.
 ACT_NONE, ACT_SOFTPLUS100, ACT_RELU = 0, 1, 2
-# "planes": forward / backward-data layer GEMMs fed by TMA from fp16 hi / lo operand planes (csrc/gemm3_tma.cu);
-# "producers": the first-generation kernel that converts fp32 operands in its main loop (csrc/gemm3.cu).  The weight
-# gradient uses the latter in both settings.
 import os as _os
-TRAIN_GEMM = _os.environ.get("RECMV_TRAIN_GEMM", "planes")
 # create_graph=True input gradients: "1" = differentiable reverse chain on the tensor-core GEMMs (second_order.py), "0" = torch graph
 SECOND_ORDER_FUSED = _os.environ.get("RECMV_SECOND_ORDER", "1") != "0"
 _INPUT_GRAD_ONLY = [0]
@@ -734,7 +732,8 @@ def grad_dyn_scale(*cotangents):
 
 
 def mlp_bwd_data_layer(G, W, out_dim, in_dim, saved_input, act, G_prev, split=0, D2=None, out_scale=1.0, dyn_scale=None):
-    """G_prev[:, :split] = ((G[:, :out_dim] @ W) * out_scale)[:, :split] * act'(saved_input); columns >= split -> D2."""
+    """G_prev[:, :split] = ((G[:, :out_dim] @ W) * out_scale)[:, :split] * act'(saved_input); columns >= split -> D2.
+    fp32 operands (csrc/gemm3.cu); its product caller is second_order.PlainMlpInputGradFunction's reverse chain."""
     P = G.shape[0]
     with torch.cuda.device(G.device):
         check(_lib.load().recmv_mlp_bwd_data_layer(
@@ -746,7 +745,8 @@ def mlp_bwd_data_layer(G, W, out_dim, in_dim, saved_input, act, G_prev, split=0,
 
 
 def mlp_bwd_weight(Gs, Xs, out_dims, in_dims, out_scales=None, dyn_scale=None, want_bias=True):
-    """dW[l] = out_scale[l] * Gs[l][:, :out]^T @ Xs[l][:, :in] and db[l] = Gs[l][:, :out].sum(0), all layers in one launch."""
+    """dW[l] = out_scale[l] * Gs[l][:, :out]^T @ Xs[l][:, :in] and db[l] = Gs[l][:, :out].sum(0), all layers in one launch.
+    fp32 operands (csrc/gemm3.cu); its product caller is second_order.PlainMlpInputGradFunction's backward."""
     n = len(Gs)
     dev = Gs[0].device
     P = Gs[0].shape[0]
@@ -763,7 +763,8 @@ def mlp_bwd_weight(Gs, Xs, out_dims, in_dims, out_scales=None, dyn_scale=None, w
 
 
 def mlp_fwd_layer(X, W, bias, out_dim, in_dim, act, Y, pre_scale=1.0, split=0, Y2=None):
-    """Y[:, :split or out] (and Y2) = act(pre_scale * X[:, :in] @ W.T + bias) on the tensor cores (training forward, one layer)."""
+    """Y[:, :split or out] (and Y2) = act(pre_scale * X[:, :in] @ W.T + bias) on the tensor cores, one layer, fp32 operands
+    (csrc/gemm3.cu); its product caller is the tangent pass of second_order.PlainMlpInputGradFunction's backward."""
     P = X.shape[0]
     with torch.cuda.device(X.device):
         check(_lib.load().recmv_mlp_fwd_layer(_ptr(X), X.stride(0), _ptr(W), _ptr(bias), int(out_dim), int(in_dim), int(act),
@@ -773,7 +774,8 @@ def mlp_fwd_layer(X, W, bias, out_dim, in_dim, act, Y, pre_scale=1.0, split=0, Y
 
 
 def pe_forward(x, pe_w, bands, out, out2=None):
-    """out[:, :3 + 6 bands] (and out2) = positional encoding of x [P,3] with annealing weights pe_w."""
+    """out[:, :3 + 6 bands] (and out2) = positional encoding of x [P,3] with annealing weights pe_w.  Callers: the
+    translator and colour networks' training forwards build their input rows with it."""
     w = (c_float * (2 * bands))(*[float(v) for v in pe_w[:2 * bands]])
     with torch.cuda.device(x.device):
         check(_lib.load().recmv_pe_forward(_ptr(x), w, int(bands), _ptr(out), out.stride(0), _ptr(out2),
@@ -784,6 +786,12 @@ def pe_forward(x, pe_w, bands, out, out2=None):
 
 def _pad8(n):
     return (int(n) + 7) // 8 * 8
+
+
+def _plane_pair(rows, cols, dev, zero=False):
+    """(hi, lo) fp16 [rows, cols] operand-plane buffers."""
+    mk = torch.zeros if zero else torch.empty
+    return (mk((rows, cols), dtype=torch.float16, device=dev), mk((rows, cols), dtype=torch.float16, device=dev))
 
 
 def split_planes(t, rows, cols, scale, scale_dev=None, transpose=False, ldp=None):
@@ -941,7 +949,7 @@ def _sdf_composite(x, Ws, bs, pe_w):
 class SdfMlpTrainFunction(torch.autograd.Function):
     """ImplicitNetwork.forward with gradients (model/network.py:89-119 inside train.py:317-330), all GEMMs on the tensor cores
     in the engine's fp32-grade arithmetic (fp16 hi/lo split, 3 MMAs per product, fp32 accumulation): TMA-fed GEMMs on
-    operand planes (csrc/gemm3_tma.cu), or the first-generation csrc/gemm3.cu with RECMV_TRAIN_GEMM=producers.
+    operand planes (csrc/gemm3_tma.cu).
 
     forward : PE kernel + 9 layer launches  Y = softplus(X W^T + b)  whose outputs stay in HBM as the next layer's input
               AND as what the backward needs (16 KB per point -- what autograd keeps for the reference's graph); the skip
@@ -969,34 +977,22 @@ class SdfMlpTrainFunction(torch.autograd.Function):
               [torch.empty((P, 512), dtype=torch.float32, device=dev) for _ in range(8)]
         sdf = torch.empty((P, 1), dtype=torch.float32, device=dev)
         feat = torch.empty((P, 256), dtype=torch.float32, device=dev)
-        if TRAIN_GEMM == "planes":
-            # operands as fp16 hi / lo planes, TMA-fed GEMMs (csrc/gemm3_tma.cu): each layer writes its output in fp32
-            # (kept for the backward) AND as the next layer's A planes
-            xp = [(torch.empty((P, 64), dtype=torch.float16, device=dev), torch.empty((P, 64), dtype=torch.float16, device=dev))]
-            xp += [(torch.empty((P, 512), dtype=torch.float16, device=dev), torch.empty((P, 512), dtype=torch.float16, device=dev))
-                   for _ in range(8)]
-            pe_forward_planes(x, pe_w, 6, act[0], xp[0][0], xp[0][1])
-            pe_forward_planes(x, pe_w, 6, act[4][:, 473:], xp[4][0][:, 473:], xp[4][1][:, 473:])
-            for l in range(9):
-                o, i = Ws[l].shape
-                wp = weight_planes(W_in[l])
-                if l < 8:
-                    mlp_layer_planes(xp[l], wp, P, o, i, 5, act[l + 1], bias=bs[l], scale=_INV_SQRT2 if l == 4 else 1.0,
-                                     y_planes=xp[l + 1])
-                else:
-                    mlp_layer_planes(xp[8], wp, P, 257, 512, 4, sdf, bias=bs[8], split=1, Y2=feat)
-        else:
-            pe_forward(x, pe_w, 6, act[0], act[4][:, 473:])
-            for l in range(8):
-                mlp_fwd_layer(act[l], Ws[l], bs[l], Ws[l].shape[0], Ws[l].shape[1], ACT_SOFTPLUS100, act[l + 1],
-                              pre_scale=_INV_SQRT2 if l == 4 else 1.0)
-            mlp_fwd_layer(act[8], Ws[8], bs[8], 257, 512, ACT_NONE, sdf, split=1, Y2=feat)
+        # operands as fp16 hi / lo planes, TMA-fed GEMMs (csrc/gemm3_tma.cu): each layer writes its output in fp32
+        # (kept for the backward) AND as the next layer's A planes
+        xp = [_plane_pair(P, 64, dev)] + [_plane_pair(P, 512, dev) for _ in range(8)]
+        pe_forward_planes(x, pe_w, 6, act[0], xp[0][0], xp[0][1])
+        pe_forward_planes(x, pe_w, 6, act[4][:, 473:], xp[4][0][:, 473:], xp[4][1][:, 473:])
+        for l in range(9):
+            o, i = Ws[l].shape
+            wp = weight_planes(W_in[l])
+            if l < 8:
+                mlp_layer_planes(xp[l], wp, P, o, i, 5, act[l + 1], bias=bs[l], scale=_INV_SQRT2 if l == 4 else 1.0,
+                                 y_planes=xp[l + 1])
+            else:
+                mlp_layer_planes(xp[8], wp, P, 257, 512, 4, sdf, bias=bs[8], split=1, Y2=feat)
         ctx.pe_w, ctx.mode = [float(w) for w in pe_w], mode
-        ctx.has_planes = TRAIN_GEMM == "planes"
-        if ctx.has_planes:      # the layer inputs' operand planes feed the weight gradient too (recmv_mlp_wgrad_planes)
-            ctx.save_for_backward(x, *Wb, *act, *[t for pair in xp for t in pair])
-        else:
-            ctx.save_for_backward(x, *Wb, *act)
+        # the layer inputs' operand planes feed the weight gradient too (recmv_mlp_wgrad_planes)
+        ctx.save_for_backward(x, *Wb, *act, *[t for pair in xp for t in pair])
         return sdf, feat
 
     @staticmethod
@@ -1004,7 +1000,6 @@ class SdfMlpTrainFunction(torch.autograd.Function):
         saved = ctx.saved_tensors
         x, Ws, bs, act = saved[0], saved[1:10], saved[10:19], saved[19:28]
         P = x.shape[0]
-        dev = x.device
         need_x = ctx.needs_input_grad[0]
         need_w = any(ctx.needs_input_grad[4:])
         if torch.is_grad_enabled() and _inputs_only(need_w):
@@ -1012,8 +1007,7 @@ class SdfMlpTrainFunction(torch.autograd.Function):
             # chain as a differentiable op whose own backward is tangent + backward GEMMs on the tensor cores (second_order.py)
             from . import second_order
             SdfMlpTrainFunction.last_backward = "fused-tc (create_graph, input gradient)"
-            dx = second_order.sdf_input_grad(x, g_sdf, g_feat, ctx.pe_w, act, Ws, bs,
-                                             saved[28:46] if ctx.has_planes else ()) if need_x else None
+            dx = second_order.sdf_input_grad(x, g_sdf, g_feat, ctx.pe_w, act, Ws, bs, saved[28:46]) if need_x else None
             return (dx, None, None, None, *([None] * 18))
         if torch.is_grad_enabled():
             # create_graph=True with parameter gradients in the graph: differentiate a torch graph of the same network
@@ -1030,87 +1024,78 @@ class SdfMlpTrainFunction(torch.autograd.Function):
             res = [next(it) if t.requires_grad else None for t in [xi] + list(Ws) + list(bs)]
             return (res[0] if need_x else None, None, None, None, *res[1:])
         SdfMlpTrainFunction.last_backward = "fused-tc"
-        G8 = torch.zeros((P, 264), dtype=torch.float32, device=dev)
-        if g_sdf is not None:
-            G8[:, 0:1] = g_sdf
-        if g_feat is not None:
-            G8[:, 1:257] = g_feat
-        dyn = grad_dyn_scale(G8)
-        G = [None] * 9
-        G[8] = G8
-        dpe4 = torch.empty((P, 40), dtype=torch.float32, device=dev)
-        outs = [w.shape[0] for w in Ws]
-        ins = [w.shape[1] for w in Ws]
-        dx = None
-        planes = TRAIN_GEMM == "planes" and ctx.has_planes
-        GP = [None] * 9
-        if planes:
-            gp = split_planes(G8, P, 257, 64.0, scale_dev=dyn, ldp=264)       # cotangent planes carry 64 * dyn
-            GP[8] = gp
-            for l in range(8, 0, -1):
-                G[l - 1] = torch.empty((P, 512), dtype=torch.float32, device=dev)
-                gprev = (torch.empty((P, 512), dtype=torch.float16, device=dev), torch.empty((P, 512), dtype=torch.float16, device=dev))
-                wtp = weight_planes(Ws[l], transpose=True)                                     # [in][out]: B of backward-data
-                mlp_layer_planes(gp, wtp, P, ins[l], outs[l], 1, G[l - 1], saved_input=act[l], scale=_INV_SQRT2 if l == 4 else 1.0,
-                                 dyn=dyn, a_has_dyn=True, split=473 if l == 4 else 0, Y2=dpe4 if l == 4 else None,
-                                 y_planes=gprev, planes_with_dyn=True)
-                gp = gprev
-                GP[l - 1] = gp
-            if need_x:
-                dpe0 = torch.empty((P, 40), dtype=torch.float32, device=dev)
-                mlp_layer_planes(gp, weight_planes(Ws[0], transpose=True), P, ins[0], outs[0], 0, dpe0, dyn=dyn, a_has_dyn=True)
-                dx = pe_backward(x, dpe0, dpe4, ctx.pe_w, 6)
-        else:
-            for l in range(8, 0, -1):
-                G[l - 1] = torch.empty((P, 512), dtype=torch.float32, device=dev)
-                mlp_bwd_data_layer(G[l], Ws[l].detach(), outs[l], ins[l], act[l], ACT_SOFTPLUS100, G[l - 1],
-                                   split=473 if l == 4 else 0, D2=dpe4 if l == 4 else None,
-                                   out_scale=_INV_SQRT2 if l == 4 else 1.0, dyn_scale=dyn)
-            if need_x:
-                dpe0 = torch.empty((P, 40), dtype=torch.float32, device=dev)
-                mlp_bwd_data_layer(G[0], Ws[0], outs[0], ins[0], None, ACT_NONE, dpe0, dyn_scale=dyn)
-                dx = pe_backward(x, dpe0, dpe4, ctx.pe_w, 6)
+        dyn, _, GP, dpe0, dpe4 = sdf_reverse_chain(g_sdf, g_feat, act, Ws, need_x)
+        dx = pe_backward(x, dpe0, dpe4, ctx.pe_w, 6) if need_x else None
         dW, db = [None] * 9, [None] * 9
-        if need_w and planes:
+        if need_w:
             # weight gradient straight from the planes both passes wrote (MN-major operands, no transposed copies)
             xpl = saved[28:46]
             for l in range(9):
-                dW[l], db[l] = mlp_wgrad_planes(GP[l], (xpl[2 * l], xpl[2 * l + 1]), P, outs[l], ins[l],
+                o, i = Ws[l].shape
+                dW[l], db[l] = mlp_wgrad_planes(GP[l], (xpl[2 * l], xpl[2 * l + 1]), P, o, i,
                                                 _INV_SQRT2 if l == 4 else 1.0, dyn, want_bias=True)
-        elif need_w:
-            dW, db = mlp_bwd_weight(G, list(act), outs, ins, [_INV_SQRT2 if l == 4 else 1.0 for l in range(9)], dyn)
         return (dx, None, None, None, *dW, *db)
 
 
+def sdf_reverse_chain(g_sdf, g_feat, act, Ws, with_layer0=True):
+    """Backward-data chain of ImplicitNetwork on the operand-plane GEMMs, from the activations `act` its training forward
+    saved: cotangents g_sdf [P,1] / g_feat [P,256] (either may be None) -> (dyn, G, GP, dpe0, dpe4).  G[l] [P, 512] (G[8]
+    [P, 264]) is the fp32 cotangent at layer l's output and GP[l] its fp16 planes (carrying 64 * dyn); dpe4 [P, 40] is the
+    cotangent of the PE copy in layer 4's skip input, dpe0 [P, 40] that of layer 0's input (None without with_layer0).
+    The buffers are not zero-filled, and G[3][:, 473:] and column 39 of dpe0 / dpe4 are never written: layer 3 has 473
+    outputs (the skip's cotangent goes to dpe4) and the PE 39 columns, and every result is taken from within those widths."""
+    P, dev = act[0].shape[0], act[0].device
+    G8 = torch.zeros((P, 264), dtype=torch.float32, device=dev)
+    if g_sdf is not None:
+        G8[:, 0:1] = g_sdf.detach()
+    if g_feat is not None:
+        G8[:, 1:257] = g_feat.detach()
+    dyn = grad_dyn_scale(G8)
+    G, GP = [None] * 9, [None] * 9
+    G[8] = G8
+    dpe4 = torch.empty((P, 40), dtype=torch.float32, device=dev)
+    GP[8] = split_planes(G8, P, 257, 64.0, scale_dev=dyn, ldp=264)       # cotangent planes carry 64 * dyn
+    for l in range(8, 0, -1):
+        o, i = Ws[l].shape
+        G[l - 1] = torch.empty((P, 512), dtype=torch.float32, device=dev)
+        GP[l - 1] = _plane_pair(P, 512, dev)
+        wtp = weight_planes(Ws[l], transpose=True)                                     # [in][out]: B of backward-data
+        mlp_layer_planes(GP[l], wtp, P, i, o, 1, G[l - 1], saved_input=act[l], scale=_INV_SQRT2 if l == 4 else 1.0,
+                         dyn=dyn, a_has_dyn=True, split=473 if l == 4 else 0, Y2=dpe4 if l == 4 else None,
+                         y_planes=GP[l - 1], planes_with_dyn=True)
+    dpe0 = None
+    if with_layer0:
+        o, i = Ws[0].shape
+        dpe0 = torch.empty((P, 40), dtype=torch.float32, device=dev)
+        mlp_layer_planes(GP[0], weight_planes(Ws[0], transpose=True), P, i, o, 0, dpe0, dyn=dyn, a_has_dyn=True)
+    return dyn, G, GP, dpe0, dpe4
+
+
 def _plain_mlp_forward(X0, Ws, bs):
-    """ReLU MLP on the tensor cores layer GEMMs: returns (output [P, out_last], saved layer inputs [X0, X1, ...])."""
+    """ReLU MLP on the operand-plane layer GEMMs: returns (output [P, out_last], saved layer inputs [X0, X1, ...], their
+    operand planes as a flat hi, lo list)."""
     P, dev = X0.shape[0], X0.device
     Ws = [w.detach().contiguous().float() for w in Ws]
     bs = [b.detach().contiguous().float() for b in bs]
     acts = [X0]
     n = len(Ws)
-    planes = TRAIN_GEMM == "planes"
-    xp = split_planes(X0, P, Ws[0].shape[1], 64.0, ldp=_pad8(X0.shape[1])) if planes else None
+    xp = split_planes(X0, P, Ws[0].shape[1], 64.0, ldp=_pad8(X0.shape[1]))
     xplanes = []
     for l in range(n):
         o, i = Ws[l].shape
         last = l == n - 1
         Y = torch.empty((P, o if not last else ((o + 3) // 4) * 4), dtype=torch.float32, device=dev)
-        if planes:
-            yp = None if last else (torch.empty((P, _pad8(o)), dtype=torch.float16, device=dev),
-                                    torch.empty((P, _pad8(o)), dtype=torch.float16, device=dev))
-            mlp_layer_planes(xp, split_planes(Ws[l], o, i, 1024.0), P, o, i, 4 if last else 6, Y, bias=bs[l], y_planes=yp)
-            xplanes += [xp[0], xp[1]]
-            xp = yp
-        else:
-            mlp_fwd_layer(acts[l], Ws[l], bs[l], o, i, ACT_NONE if last else ACT_RELU, Y)
+        yp = None if last else _plane_pair(P, _pad8(o), dev)
+        mlp_layer_planes(xp, split_planes(Ws[l], o, i, 1024.0), P, o, i, 4 if last else 6, Y, bias=bs[l], y_planes=yp)
+        xplanes += [xp[0], xp[1]]
+        xp = yp
         acts.append(Y)
     return acts[-1][:, :Ws[-1].shape[0]], acts[:-1], xplanes
 
 
-def _plain_mlp_backward(g_out, Ws, acts, need_w, need_x0, xplanes=()):
+def _plain_mlp_backward(g_out, Ws, acts, need_w, need_x0, xplanes):
     """g_out [P, out_last] -> (dX0 [P, in_0 padded] or None, dW list, db list) for the ReLU MLP.  xplanes: the layer inputs'
-    operand planes from the forward (flat hi, lo list) -- with them the weight gradient runs on the planes as well."""
+    operand planes from the forward (flat hi, lo list), the weight gradient's second operand."""
     P, dev = g_out.shape[0], g_out.device
     n = len(Ws)
     o_last = Ws[-1].shape[0]
@@ -1118,37 +1103,28 @@ def _plain_mlp_backward(g_out, Ws, acts, need_w, need_x0, xplanes=()):
     G[n - 1] = torch.zeros((P, _pad8(o_last)), dtype=torch.float32, device=dev)
     G[n - 1][:, :o_last] = g_out
     dyn = grad_dyn_scale(G[n - 1])
-    planes = TRAIN_GEMM == "planes"
-    gp = split_planes(G[n - 1], P, o_last, 64.0, scale_dev=dyn, ldp=_pad8(o_last)) if planes else None
+    gp = split_planes(G[n - 1], P, o_last, 64.0, scale_dev=dyn, ldp=_pad8(o_last))
     GP = [None] * n
     GP[n - 1] = gp
     for l in range(n - 1, 0, -1):
         o, i = Ws[l].shape
         G[l - 1] = torch.empty((P, i), dtype=torch.float32, device=dev)
-        if planes:
-            gprev = (torch.empty((P, _pad8(i)), dtype=torch.float16, device=dev), torch.empty((P, _pad8(i)), dtype=torch.float16, device=dev))
-            mlp_layer_planes(gp, split_planes(Ws[l].detach(), o, i, 1024.0, transpose=True), P, i, o, 2, G[l - 1],
-                             saved_input=acts[l], dyn=dyn, a_has_dyn=True, y_planes=gprev, planes_with_dyn=True)
-            gp = gprev
-            GP[l - 1] = gp
-        else:
-            mlp_bwd_data_layer(G[l], Ws[l], o, i, acts[l], ACT_RELU, G[l - 1], dyn_scale=dyn)
+        gprev = _plane_pair(P, _pad8(i), dev)
+        mlp_layer_planes(gp, split_planes(Ws[l].detach(), o, i, 1024.0, transpose=True), P, i, o, 2, G[l - 1],
+                         saved_input=acts[l], dyn=dyn, a_has_dyn=True, y_planes=gprev, planes_with_dyn=True)
+        gp = gprev
+        GP[l - 1] = gp
     dX0 = None
     if need_x0:
         o, i = Ws[0].shape
         dX0 = torch.empty((P, ((i + 3) // 4) * 4), dtype=torch.float32, device=dev)
-        if planes:
-            mlp_layer_planes(gp, split_planes(Ws[0].detach(), o, i, 1024.0, transpose=True), P, i, o, 0, dX0, dyn=dyn,
-                             a_has_dyn=True)
-        else:
-            mlp_bwd_data_layer(G[0], Ws[0], o, i, None, ACT_NONE, dX0, dyn_scale=dyn)
+        mlp_layer_planes(gp, split_planes(Ws[0].detach(), o, i, 1024.0, transpose=True), P, i, o, 0, dX0, dyn=dyn,
+                         a_has_dyn=True)
     dW, db = [None] * n, [None] * n
-    if need_w and planes and len(xplanes) == 2 * n:
+    if need_w:
         for l in range(n):
             o, i = Ws[l].shape
             dW[l], db[l] = mlp_wgrad_planes(GP[l], (xplanes[2 * l], xplanes[2 * l + 1]), P, o, i, 1.0, dyn, want_bias=True)
-    elif need_w:
-        dW, db = mlp_bwd_weight(G, list(acts), [w.shape[0] for w in Ws], [w.shape[1] for w in Ws], None, dyn)
     return dX0, dW, db
 
 

@@ -9,22 +9,24 @@ The reference differentiates its networks twice on every training step:
 
 `ops.SdfMlpTrainFunction.backward` / `ops.TranslatorTrainFunction.backward` / `ops.RenderNetTrainFunction.backward` called
 with create_graph=True land here when only INPUT gradients are requested (the three call sites above): the reverse chain
-runs on the same backward-data GEMMs as the first-order path, and is itself an autograd Function whose backward is
+is itself an autograd Function whose backward is
 
     upward   : the network's tangent (JVP) pass  tz_l = tu_l W_l^T,  tu_{l+1} = act'(z_l) * tz_l       (9 layer GEMMs)
     local    : zb_l = act''(z_l) * u_{l+1} * tz_l  = 100 (1 - s_l) h_{l+1} tz_l   for softplus_100 (0 for ReLU)
     downward : an ordinary backward-data pass that picks zb_l up at every layer                       (8 layer GEMMs)
-    weights  : dW_l = h_{l+1}^T tu_l + zb_l^T a_l  (two weight-gradient launches over all layers),  db_l = sum zb_l
+    weights  : dW_l = h_{l+1}^T tu_l + zb_l^T a_l,  db_l = sum zb_l
 
-with h_{l+1} the first-order cotangent at z_l.  Everything heavy is a 3xfp16 wgmma GEMM: the SDF network's passes run on the
-operand-plane kernels of csrc/gemm3_tma.cu, each followed by one element-wise launch that also writes the next GEMM's
-planes; the translator and colour networks' reverse chain still runs on csrc/gemm3.cu with torch element-wise ops.  The
-positional encoding's own VJP is a torch graph (so its second derivative comes from autograd).  A request that ALSO wants parameter gradients with a graph (loss.backward(create_graph=
-True)) still takes the torch-composite fallback."""
+with h_{l+1} the first-order cotangent at z_l.  Everything heavy is a 3xfp16 wgmma GEMM.  The SDF network's reverse chain is
+the first-order path's own (ops.sdf_reverse_chain), and all its passes run on the operand-plane kernels of
+csrc/gemm3_tma.cu, each followed by one element-wise launch that also writes the next GEMM's planes.  The translator and
+colour networks' reverse chain and its backward (PlainMlpInputGradFunction) run on the fp32-operand GEMM entries of
+csrc/gemm3.cu with torch element-wise ops; it is the one product caller of those entries.  The positional encoding's own
+VJP is a torch graph (so its second derivative comes from autograd).  A request that ALSO wants parameter gradients with a
+graph (loss.backward(create_graph=True)) still takes the torch-composite fallback."""
 import torch
 
 from . import ops
-from .ops import (ACT_NONE, ACT_RELU, ACT_SOFTPLUS100, _INV_SQRT2, grad_dyn_scale, mlp_bwd_data_layer, mlp_bwd_weight,
+from .ops import (ACT_NONE, ACT_RELU, _INV_SQRT2, _plane_pair, grad_dyn_scale, mlp_bwd_data_layer, mlp_bwd_weight,
                   mlp_fwd_layer, mlp_layer_planes, pe_backward, split_planes)
 
 
@@ -46,83 +48,52 @@ class SdfMlpPeGradFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x, g_sdf, g_feat, pe_w, *rest):
-        act, Ws, bs, xplanes = rest[:9], rest[9:18], rest[18:27], rest[27:]
-        P, dev = x.shape[0], x.device
-        Wd = [w.detach().contiguous().float() for w in Ws]
-        outs = [w.shape[0] for w in Wd]
-        ins = [w.shape[1] for w in Wd]
-        G8 = torch.zeros((P, 264), dtype=torch.float32, device=dev)
-        if g_sdf is not None:
-            G8[:, 0:1] = g_sdf.detach()
-        if g_feat is not None:
-            G8[:, 1:257] = g_feat.detach()
-        dyn = grad_dyn_scale(G8)
-        G = [None] * 9
-        G[8] = G8
-        dpe4 = torch.zeros((P, 40), dtype=torch.float32, device=dev)
-        dpe0 = torch.zeros((P, 40), dtype=torch.float32, device=dev)
-        if ops.TRAIN_GEMM == "planes":
-            gp = split_planes(G8, P, 257, 64.0, scale_dev=dyn, ldp=264)
-            GP = [None] * 9
-            GP[8] = gp
-            for l in range(8, 0, -1):
-                G[l - 1] = torch.zeros((P, 512), dtype=torch.float32, device=dev)
-                gprev = _plane_pair(P, 512, dev)
-                GP[l - 1] = gprev
-                mlp_layer_planes(gp, ops.weight_planes(Ws[l], transpose=True), P, ins[l], outs[l], 1, G[l - 1],
-                                 saved_input=act[l], scale=_INV_SQRT2 if l == 4 else 1.0, dyn=dyn, a_has_dyn=True,
-                                 split=473 if l == 4 else 0, Y2=dpe4 if l == 4 else None, y_planes=gprev, planes_with_dyn=True)
-                gp = gprev
-            mlp_layer_planes(gp, ops.weight_planes(Ws[0], transpose=True), P, ins[0], outs[0], 0, dpe0,
-                             dyn=dyn, a_has_dyn=True)
-        else:
-            for l in range(8, 0, -1):
-                G[l - 1] = torch.zeros((P, 512), dtype=torch.float32, device=dev)
-                mlp_bwd_data_layer(G[l], Wd[l], outs[l], ins[l], act[l], ACT_SOFTPLUS100, G[l - 1], split=473 if l == 4 else 0,
-                                   D2=dpe4 if l == 4 else None, out_scale=_INV_SQRT2 if l == 4 else 1.0, dyn_scale=dyn)
-            mlp_bwd_data_layer(G[0], Wd[0], outs[0], ins[0], None, ACT_NONE, dpe0, dyn_scale=dyn)
+        act, Ws, xplanes = rest[:9], rest[9:18], rest[27:]
+        dyn, G, GP, dpe0, dpe4 = ops.sdf_reverse_chain(g_sdf, g_feat, act, Ws)
         ctx.pe_w = [float(w) for w in pe_w]
-        ctx.dims = (outs, ins)
-        ctx.wgrad_planes = ops.TRAIN_GEMM == "planes" and len(xplanes) == 18
-        extra = ([t for pair in GP for t in pair] + list(xplanes)) if ctx.wgrad_planes else []
-        ctx.save_for_backward(x, dyn, *act, *Ws, *G, *extra)
+        ctx.dims = ([w.shape[0] for w in Ws], [w.shape[1] for w in Ws])
+        ctx.save_for_backward(x, dyn, *act, *Ws, *G, *[t for pair in GP for t in pair], *xplanes)
         return (dpe0 + dpe4)[:, :39].contiguous()
 
     @staticmethod
     @torch.autograd.function.once_differentiable
     def backward(ctx, q):
+        """On the TMA-fed plane GEMMs (csrc/gemm3_tma.cu): every layer is ONE GEMM launch plus ONE element-wise launch that
+        also writes the next GEMM's operand planes."""
         saved = ctx.saved_tensors
         x, dyn = saved[0], saved[1]
         act, Ws, G = saved[2:11], saved[11:20], saved[20:29]
+        GPl, XPl = saved[29:47], saved[47:65]
         outs, ins = ctx.dims
         need = ctx.needs_input_grad
         need_x, need_g = need[0], need[1] or need[2]
         need_w = any(need[13:31])
         P, dev = x.shape[0], x.device
-        Wd = [w.detach().contiguous().float() for w in Ws]
         dq = grad_dyn_scale(q)
         inv_dq = 1.0 / dq
-        if ops.TRAIN_GEMM == "planes":
-            res = SdfMlpPeGradFunction._backward_planes(ctx, q, x, dyn, act, Ws, G, outs, ins, need, need_x, need_g, need_w, dq,
-                                                        inv_dq, saved[29:])
-            return (*res, *([None] * (len(need) - len(res))))
+        sc = [_INV_SQRT2 if l == 4 else 1.0 for l in range(9)]
         # ---- upward: tangent pass with tangent of PE = q (scaled into [1,2) by dq; everything below is linear in it) ----
         U = [torch.zeros((P, 64), dtype=torch.float32, device=dev)] + \
             [torch.zeros((P, 512), dtype=torch.float32, device=dev) for _ in range(8)]
         U[0][:, :39] = q * dq
         U[4][:, 473:] = U[0][:, :39]
+        up = up0 = split_planes(U[0], P, 39, 64.0, ldp=64)
+        UP = [up0] + [None] * 8
         inj = [None] * 8
         tz = None
         for l in range(9):
             o = outs[l]
-            tz = torch.empty((P, 512 if l < 8 else 260), dtype=torch.float32, device=dev)
-            mlp_fwd_layer(U[l], Wd[l], None, o, ins[l], ACT_NONE, tz, pre_scale=_INV_SQRT2 if l == 4 else 1.0)
+            tz = torch.empty((P, 512 if l < 8 else 264), dtype=torch.float32, device=dev)
+            mlp_layer_planes(up, ops.weight_planes(Ws[l]), P, o, ins[l], 4, tz, scale=sc[l])
             if l < 8:
-                e = torch.exp(-100.0 * act[l + 1][:, :o])               # 1 - s_l,  s_l = softplus_100'(z_l)
-                t = tz[:, :o]
-                U[l + 1][:, :o] = (1.0 - e) * t
+                un = _plane_pair(P, 512, dev, zero=True)
                 inj[l] = torch.zeros((P, 512), dtype=torch.float32, device=dev)
-                inj[l][:, :o] = 100.0 * e * G[l][:, :o] * t             # softplus'' * u_{l+1} * tz = 100 (1 - s) h tz
+                ops.softplus_tangent_planes(tz, act[l + 1], G[l], o, U[l + 1], un, inj[l])
+                if l == 3:      # layer 4 reads [tangent of a_4 (473) | tangent of PE (39)]
+                    un[0][:, 473:] = up0[0][:, :39]
+                    un[1][:, 473:] = up0[1][:, :39]
+                up = un
+                UP[l + 1] = un
         g_bar = tz[:, :257] * inv_dq if need_g else None
         # ---- downward: backward-data pass that collects the local terms ----
         dx = None
@@ -131,113 +102,41 @@ class SdfMlpPeGradFunction(torch.autograd.Function):
             dyn2 = grad_dyn_scale(*inj)
             Zb = [None] * 8
             Zb[7] = inj[7]
+            zp = split_planes(Zb[7], P, 512, 64.0, scale_dev=dyn2, ldp=512)
+            ZP = [None] * 8
+            ZP[7] = zp
             dpe4 = torch.zeros((P, 40), dtype=torch.float32, device=dev)
             for l in range(7, 0, -1):
                 Zb[l - 1] = torch.zeros((P, 512), dtype=torch.float32, device=dev)
-                mlp_bwd_data_layer(Zb[l], Wd[l], outs[l], ins[l], act[l], ACT_SOFTPLUS100, Zb[l - 1],
-                                   split=473 if l == 4 else 0, D2=dpe4 if l == 4 else None,
-                                   out_scale=_INV_SQRT2 if l == 4 else 1.0, dyn_scale=dyn2)
-                Zb[l - 1] += inj[l - 1]
+                mlp_layer_planes(zp, ops.weight_planes(Ws[l], transpose=True), P, ins[l], outs[l], 1, Zb[l - 1],
+                                 saved_input=act[l], scale=sc[l], dyn=dyn2, a_has_dyn=True, split=473 if l == 4 else 0,
+                                 Y2=dpe4 if l == 4 else None)
+                zp = _plane_pair(P, 512, dev, zero=True)
+                ops.add_split_planes(Zb[l - 1], inj[l - 1], outs[l - 1], zp, 64.0, dyn2)
+                ZP[l - 1] = zp
             if need_x:
                 dpe0 = torch.zeros((P, 40), dtype=torch.float32, device=dev)
-                mlp_bwd_data_layer(Zb[0], Wd[0], outs[0], ins[0], None, ACT_NONE, dpe0, dyn_scale=dyn2)
+                mlp_layer_planes(zp, ops.weight_planes(Ws[0], transpose=True), P, ins[0], outs[0], 0, dpe0,
+                                 dyn=dyn2, a_has_dyn=True)
                 dx = pe_backward(x, dpe0, dpe4, ctx.pe_w, 6) * inv_dq
             if need_w:
-                sc = [_INV_SQRT2 if l == 4 else 1.0 for l in range(9)]
-                dW1, _ = mlp_bwd_weight(list(G), U, outs, ins, sc, dyn, want_bias=False)
-                dW2, db2 = mlp_bwd_weight(Zb, list(act[:8]), outs[:8], ins[:8], sc[:8], dyn2, want_bias=True)
+                # both outer products straight from the planes the passes wrote (recmv_mlp_wgrad_planes)
                 for l in range(9):
-                    dW[l] = (dW1[l] + dW2[l]) * inv_dq if l < 8 else dW1[l] * inv_dq
-                    db[l] = db2[l] * inv_dq if l < 8 else None      # the input gradient does not depend on the last bias
+                    w1 = ops.mlp_wgrad_planes((GPl[2 * l], GPl[2 * l + 1]), UP[l], P, outs[l], ins[l], sc[l], dyn)
+                    if l < 8:
+                        w2, b2 = ops.mlp_wgrad_planes(ZP[l], (XPl[2 * l], XPl[2 * l + 1]), P, outs[l], ins[l], sc[l], dyn2,
+                                                      want_bias=True)
+                        w1 = w1 + w2
+                        db[l] = b2 * inv_dq
+                    dW[l] = w1 * inv_dq
         g_sdf_bar = g_bar[:, 0:1].contiguous() if (need[1] and g_bar is not None) else None
         g_feat_bar = g_bar[:, 1:257].contiguous() if (need[2] and g_bar is not None) else None
         return (dx, g_sdf_bar, g_feat_bar, None, *([None] * 9), *dW, *db, *([None] * (len(need) - 31)))
 
 
-def _sdf_backward_planes(ctx, q, x, dyn, act, Ws, G, outs, ins, need, need_x, need_g, need_w, dq, inv_dq, extra=()):
-    """The backward of SdfMlpPeGradFunction on the TMA-fed plane GEMMs (csrc/gemm3_tma.cu): every layer is ONE GEMM launch plus
-    ONE element-wise launch that also writes the next GEMM's operand planes."""
-    P, dev = x.shape[0], x.device
-    sc = [_INV_SQRT2 if l == 4 else 1.0 for l in range(9)]
-    # ---- upward: tangent pass ----
-    U = [torch.zeros((P, 64), dtype=torch.float32, device=dev)] + \
-        [torch.zeros((P, 512), dtype=torch.float32, device=dev) for _ in range(8)]
-    U[0][:, :39] = q * dq
-    U[4][:, 473:] = U[0][:, :39]
-    up = up0 = split_planes(U[0], P, 39, 64.0, ldp=64)
-    UP = [up0] + [None] * 8
-    inj = [None] * 8
-    tz = None
-    for l in range(9):
-        o = outs[l]
-        tz = torch.empty((P, 512 if l < 8 else 264), dtype=torch.float32, device=dev)
-        mlp_layer_planes(up, ops.weight_planes(Ws[l]), P, o, ins[l], 4, tz, scale=sc[l])
-        if l < 8:
-            un = (torch.zeros((P, 512), dtype=torch.float16, device=dev), torch.zeros((P, 512), dtype=torch.float16, device=dev))
-            inj[l] = torch.zeros((P, 512), dtype=torch.float32, device=dev)
-            ops.softplus_tangent_planes(tz, act[l + 1], G[l], o, U[l + 1], un, inj[l])
-            if l == 3:      # layer 4 reads [tangent of a_4 (473) | tangent of PE (39)]
-                un[0][:, 473:] = up0[0][:, :39]
-                un[1][:, 473:] = up0[1][:, :39]
-            up = un
-            UP[l + 1] = un
-    g_bar = tz[:, :257] * inv_dq if need_g else None
-    # ---- downward: backward-data pass that collects the local terms ----
-    dx = None
-    dW, db = [None] * 9, [None] * 9
-    if need_x or need_w:
-        dyn2 = grad_dyn_scale(*inj)
-        Zb = [None] * 8
-        Zb[7] = inj[7]
-        zp = split_planes(Zb[7], P, 512, 64.0, scale_dev=dyn2, ldp=512)
-        ZP = [None] * 8
-        ZP[7] = zp
-        dpe4 = torch.zeros((P, 40), dtype=torch.float32, device=dev)
-        for l in range(7, 0, -1):
-            Zb[l - 1] = torch.zeros((P, 512), dtype=torch.float32, device=dev)
-            mlp_layer_planes(zp, ops.weight_planes(Ws[l], transpose=True), P, ins[l], outs[l], 1, Zb[l - 1],
-                             saved_input=act[l], scale=sc[l], dyn=dyn2, a_has_dyn=True, split=473 if l == 4 else 0,
-                             Y2=dpe4 if l == 4 else None)
-            zp = _plane_pair(P, 512, dev, zero=True)
-            ops.add_split_planes(Zb[l - 1], inj[l - 1], outs[l - 1], zp, 64.0, dyn2)
-            ZP[l - 1] = zp
-        if need_x:
-            dpe0 = torch.zeros((P, 40), dtype=torch.float32, device=dev)
-            mlp_layer_planes(zp, ops.weight_planes(Ws[0], transpose=True), P, ins[0], outs[0], 0, dpe0,
-                             dyn=dyn2, a_has_dyn=True)
-            dx = pe_backward(x, dpe0, dpe4, ctx.pe_w, 6) * inv_dq
-        if need_w and getattr(ctx, "wgrad_planes", False):
-            # both outer products straight from the planes the passes wrote (recmv_mlp_wgrad_planes)
-            GPl, XPl = extra[:18], extra[18:36]
-            for l in range(9):
-                w1 = ops.mlp_wgrad_planes((GPl[2 * l], GPl[2 * l + 1]), UP[l], P, outs[l], ins[l], sc[l], dyn)
-                if l < 8:
-                    w2, b2 = ops.mlp_wgrad_planes(ZP[l], (XPl[2 * l], XPl[2 * l + 1]), P, outs[l], ins[l], sc[l], dyn2, want_bias=True)
-                    w1 = w1 + w2
-                    db[l] = b2 * inv_dq
-                dW[l] = w1 * inv_dq
-        elif need_w:
-            dW1, _ = mlp_bwd_weight(list(G), U, outs, ins, sc, dyn, want_bias=False)
-            dW2, db2 = mlp_bwd_weight(Zb, list(act[:8]), outs[:8], ins[:8], sc[:8], dyn2, want_bias=True)
-            for l in range(9):
-                dW[l] = (dW1[l] + dW2[l]) * inv_dq if l < 8 else dW1[l] * inv_dq
-                db[l] = db2[l] * inv_dq if l < 8 else None      # the input gradient does not depend on the last bias
-    g_sdf_bar = g_bar[:, 0:1].contiguous() if (need[1] and g_bar is not None) else None
-    g_feat_bar = g_bar[:, 1:257].contiguous() if (need[2] and g_bar is not None) else None
-    return (dx, g_sdf_bar, g_feat_bar, None, *([None] * 9), *dW, *db)
-
-
-SdfMlpPeGradFunction._backward_planes = staticmethod(_sdf_backward_planes)
-
-
-def _plane_pair(rows, cols, dev, zero=False):
-    mk = torch.zeros if zero else torch.empty
-    return (mk((rows, cols), dtype=torch.float16, device=dev), mk((rows, cols), dtype=torch.float16, device=dev))
-
-
-def sdf_input_grad(x, g_sdf, g_feat, pe_w, act, Ws, bs, xplanes=()):
+def sdf_input_grad(x, g_sdf, g_feat, pe_w, act, Ws, bs, xplanes):
     """dx of ImplicitNetwork as a twice-differentiable expression (the create_graph=True branch of
-    ops.SdfMlpTrainFunction.backward).  xplanes: the forward's layer-input planes (18 tensors) when it ran on planes."""
+    ops.SdfMlpTrainFunction.backward).  xplanes: the forward's 18 layer-input operand planes (flat hi, lo list)."""
     u0 = SdfMlpPeGradFunction.apply(x, g_sdf, g_feat, pe_w, *act, *Ws, *bs, *xplanes)
     return pe_vjp_torch(x, u0, pe_w, 6)
 

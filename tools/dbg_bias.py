@@ -1,6 +1,7 @@
 """Systematic (signed) relative error of the training GEMM chain vs float64: projection coefficient <ours, true>/<true, true> - 1."""
-import sys, torch
-sys.path.insert(0, '/root/repo')
+import os, sys, torch
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
 from recmv_b200 import ops, synth, testing
 from recmv_b200.model import getTmpSdf
 dev = "cuda:0"
@@ -19,13 +20,11 @@ for pseed in (None, 101):
     xd = x.double().requires_grad_(True)
     sdf64, feat64 = ops._sdf_composite(xd, [w.double() for w in Ws], [b.double() for b in bs], pe_w)
     (g64,) = torch.autograd.grad(sdf64.sum(), xd)
-    for mode in ("planes", "gemm3"):
-        ops.TRAIN_GEMM = mode
-        xi = x.clone().requires_grad_(True)
-        sdf, feat = ops.SdfMlpTrainFunction.apply(xi, pe_w, None, None, *Ws, *bs)
-        (g,) = torch.autograd.grad(sdf.sum(), xi)
-        print(f"net {pseed} {mode}: forward sdf proj {proj(sdf, sdf64):+.2e} feat {proj(feat, feat64):+.2e}  grad proj {proj(g, g64):+.2e}  "
-              f"grad max err {float((g.double() - g64).abs().max() / g64.abs().max()):.2e}")
+    xi = x.clone().requires_grad_(True)
+    sdf, feat = ops.SdfMlpTrainFunction.apply(xi, pe_w, None, None, *Ws, *bs)
+    (g,) = torch.autograd.grad(sdf.sum(), xi)
+    print(f"net {pseed} training Function: forward sdf proj {proj(sdf, sdf64):+.2e} feat {proj(feat, feat64):+.2e}  "
+          f"grad proj {proj(g, g64):+.2e}  grad max err {float((g.double() - g64).abs().max() / g64.abs().max()):.2e}")
     xi = x.clone().requires_grad_(True)
     s32, _ = ops._sdf_composite(xi, Ws, bs, pe_w)
     (g32,) = torch.autograd.grad(s32.sum(), xi)
