@@ -34,6 +34,13 @@ constexpr int kPrologueWarp = kProducerWarp + 2;  // warps 10, 11: one thread pe
 constexpr int kPrologueWarps = 2;
 constexpr int kThreads = 32 * (kPrologueWarp + kPrologueWarps);   // 12 warps = three whole warpgroups
 constexpr int kRowsPerCta = 64;
+// Per-thread register budgets after setmaxnreg.  The launch gives every thread 65536 / 384 = 168 registers and the CTA
+// owns exactly that pool, so setmaxnreg.inc can only hand the MMA warpgroups what the third warpgroup (producers +
+// prologue) gave back with setmaxnreg.dec; a larger request would wait forever.
+constexpr int kLaunchRegs = 168, kMmaRegs = 200, kAuxRegs = 104;
+static_assert(kLaunchRegs * kThreads <= 65536, "one CTA per SM at the launch bound");
+static_assert(2 * kMmaRegs + kAuxRegs <= 3 * kLaunchRegs && kMmaRegs % 8 == 0 && kAuxRegs % 8 == 0,
+              "setmaxnreg: the two MMA warpgroups get what the third one releases");
 #ifndef RECMV_TC_TWO_SWEEPS
 #define RECMV_TC_TWO_SWEEPS 1   // last layer, parity mode: correction MMAs first, hi*hi MMAs in a second sweep
 #endif
@@ -288,45 +295,9 @@ sdf_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams prm) {
   if (warp >= kProducerWarp && warp < kPrologueWarp && lane == 0) prefetch_tmap(&tmap);
   __syncthreads();
 
-  if (warp >= kProducerWarp && warp < kPrologueWarp) {
-    // ====== TMA producers: warp 8 + g streams the weight boxes of warpgroup g, in the order that warpgroup consumes them ======
-    const int g = warp - kProducerWarp;
-    if (lane == 0) {
-      unsigned long long* stall = stall_begin(true, 2 + g);
-      const long long t_loop = stall_now();
-      int slot = 0;
-      uint32_t phase = 0;   // parity of the ring's current pass
-      for (long long it = 0; it < n_iter; ++it) {
-        for (int l = 0; l < kNumLayers; ++l) {
-          const int nkb = NetT::nkb(l), nt_own = own_tiles(NetT::ntiles(l, prm.last_tiles), g);
-          // last layer, parity mode: sweep 0 streams (w_hi, w_lo) for the correction MMAs, sweep 1 streams w_hi again
-          const int nsweep = (kTwoSweeps && kPasses == 3 && l == kNumLayers - 1) ? 2 : 1;
-          for (int sweep = 0; sweep < nsweep; ++sweep) {
-            const int nplanes = (kPasses == 3 && sweep == 0) ? 2 : 1;
-            for (int i = 0; i < nkb; ++i) {
-              const int kbi = NetT::kb_at(l, i);
-              const int panel = NetT::pbase(l) + (kbi == 8 ? nkb - 1 : kbi);   // the PE block is the layer's last panel
-              for (int t = 0; t < nt_own; ++t) {
-                for (int plane = 0; plane < nplanes; ++plane) {
-                  for (int half = 0; half < 2; ++half) {
-                    const long long t0 = stall_now();
-                    mbar_wait(EMPTY(g, slot), phase ^ 1u, abort_flag, prm.status, 100 + g * kSlots + slot);
-                    stall_add(stall, true, kStEmpty, t0);
-                    mbar_expect_tx_local(FULL(g, slot), kSlotBytes);
-                    tma_load_2d(SLOT(g, slot), &tmap, FULL(g, slot), 32 * half,
-                                (plane * NetT::kPanels + panel) * 512 + (2 * g + t) * 128);
-                    if (++slot == kSlots) { slot = 0; phase ^= 1u; }
-                  }
-                }
-              }
-            }
-          }
-        }
-      }
-      stall_add(stall, true, kStProducerTotal, t_loop);
-      stall_end(stall, true);
-    }
-  } else if (warp < kMmaWarps) {
+  if (warp < kMmaWarps) {
+    // the two MMA warpgroups take the registers the third one released (two accumulators + the epilogue)
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kMmaRegs));
     // ================================ MMA warpgroups + epilogue =========================================
     const int g = warp >> 2, wq = warp & 3;
     const bool signaller = (threadIdx.x & 127) == 0;
@@ -597,137 +568,179 @@ sdf_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams prm) {
     stall_add(stall, signaller, kStConsumerTotal, t_loop);
     stall_end(stall, signaller);
   } else {
-    // ================================ prologue for the next tile ========================
-    const int row = (warp - kPrologueWarp) * 32 + lane;
-    for (long long it = 0; it < n_iter; ++it) {
-      const long long tile = tile_of(it);
-      const long long p = kJvp ? tile * kPtsPerTile + (row >> 2) : tile * kPtsPerTile + row;
-      bool ok = true;
-      if (kNet == 2) {
-        // colour-network input row, 8 columns at a time straight into the activation buffer (K blocks 0..4)
-        float head[40];   // [p 3 | PE4(v) 27 | n 3 | feat 0..6]
-#pragma unroll
-        for (int e = 0; e < 40; ++e) head[e] = 0.f;
-        const bool live = p < Ptot;
-        const float* ft = prm.feats + (size_t)(live ? p : 0) * 256;
-        if (live) {
-          float pe[39];
-          positional_encode(__ldg(prm.view_dirs + 3 * p), __ldg(prm.view_dirs + 3 * p + 1), __ldg(prm.view_dirs + 3 * p + 2),
-                            prm.pw.w, pe);   // the first 27 entries of a 6-band encoding are the 4-band encoding
-#pragma unroll
-          for (int e = 0; e < 3; ++e) { head[e] = __ldg(prm.src.x + 3 * p + e); head[30 + e] = __ldg(prm.normals + 3 * p + e); }
-#pragma unroll
-          for (int e = 0; e < 27; ++e) head[3 + e] = pe[e];
-#pragma unroll
-          for (int e = 0; e < 7; ++e) head[33 + e] = __ldg(ft + e);
-        }
-        if (it > 0) mbar_wait(BAR(kBarPeFree), (uint32_t)((it - 1) & 1), abort_flag, prm.status, 400);
-#pragma unroll 1
-        for (int chunk = 0; chunk < 40; ++chunk) {
-          float v[8];
-#pragma unroll
-          for (int e = 0; e < 8; ++e) {
-            const int col = 8 * chunk + e;              // feature j sits in column 33 + j
-            v[e] = (live && col >= 40 && col < 289) ? __ldg(ft + (col - 33)) : 0.f;
-          }
-          if (chunk < 5) {
-#pragma unroll
-            for (int c5 = 0; c5 < 5; ++c5)
-              if (chunk == c5) {
-#pragma unroll
-                for (int e = 0; e < 8; ++e) v[e] = head[8 * c5 + e];
+    // producers and prologue: one setmaxnreg for the whole warpgroup (.aligned), before it splits into roles
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kAuxRegs));
+    if (warp < kPrologueWarp) {
+      // ====== TMA producers: warp 8 + g streams the weight boxes of warpgroup g, in the order that warpgroup consumes them ======
+      const int g = warp - kProducerWarp;
+      if (lane == 0) {
+        unsigned long long* stall = stall_begin(true, 2 + g);
+        const long long t_loop = stall_now();
+        int slot = 0;
+        uint32_t phase = 0;   // parity of the ring's current pass
+        for (long long it = 0; it < n_iter; ++it) {
+          for (int l = 0; l < kNumLayers; ++l) {
+            const int nkb = NetT::nkb(l), nt_own = own_tiles(NetT::ntiles(l, prm.last_tiles), g);
+            // last layer, parity mode: sweep 0 streams (w_hi, w_lo) for the correction MMAs, sweep 1 streams w_hi again
+            const int nsweep = (kTwoSweeps && kPasses == 3 && l == kNumLayers - 1) ? 2 : 1;
+            for (int sweep = 0; sweep < nsweep; ++sweep) {
+              const int nplanes = (kPasses == 3 && sweep == 0) ? 2 : 1;
+              for (int i = 0; i < nkb; ++i) {
+                const int kbi = NetT::kb_at(l, i);
+                const int panel = NetT::pbase(l) + (kbi == 8 ? nkb - 1 : kbi);   // the PE block is the layer's last panel
+                for (int t = 0; t < nt_own; ++t) {
+                  for (int plane = 0; plane < nplanes; ++plane) {
+                    for (int half = 0; half < 2; ++half) {
+                      const long long t0 = stall_now();
+                      mbar_wait(EMPTY(g, slot), phase ^ 1u, abort_flag, prm.status, 100 + g * kSlots + slot);
+                      stall_add(stall, true, kStEmpty, t0);
+                      mbar_expect_tx_local(FULL(g, slot), kSlotBytes);
+                      tma_load_2d(SLOT(g, slot), &tmap, FULL(g, slot), 32 * half,
+                                  (plane * NetT::kPanels + panel) * 512 + (2 * g + t) * 128);
+                      if (++slot == kSlots) { slot = 0; phase ^= 1u; }
+                    }
+                  }
+                }
               }
+            }
           }
-#pragma unroll
-          for (int e = 0; e < 8; ++e) v[e] *= kActScale;
-          range_check8(v, prm.status, 1100);
-          uint4 hi, lo;
-          split8(v, hi, lo);
-          const uint32_t off = (uint32_t)(chunk >> 3) * 8192u + sw128_offset(row, chunk & 7);
-          st_shared_v4(base + kOffAHi + off, hi);
-          if (kPasses == 3) st_shared_v4(base + kOffALo + off, lo);
         }
-      } else if (kNet == 1) {
-        // deformer input row: [PE(p) (39) | cond[frame] (128) | 0 (25)] = three 64-wide K blocks written into the
-        // activation buffer itself (free again once the previous tile's last layer has been issued and done)
-        // (written 8 columns at a time; only the 40-wide head [PE | first cond value] lives in registers)
-        float head[40];
-#pragma unroll
-        for (int e = 0; e < 40; ++e) head[e] = 0.f;
-        const bool live = p < Ptot;
-        const bool value_row = !kJvp || (row & 3) == 0;
-        const float* cond = prm.conds;
-        if (live) {
-          const float x = __ldg(prm.src.x + 3 * p), y = __ldg(prm.src.x + 3 * p + 1), z = __ldg(prm.src.x + 3 * p + 2);
-          if (value_row) {
-            positional_encode(x, y, z, prm.pw.w, head);
-            long long f = prm.batch_inds ? prm.batch_inds[p] : (prm.points_per_frame > 0 ? p / prm.points_per_frame : 0);
-            f = f < 0 ? 0 : (f >= prm.num_frames ? prm.num_frames - 1 : f);
-            cond = prm.conds + (size_t)f * 128;
-            head[39] = __ldg(cond);
-          } else {
-            positional_encode_tangent(x, y, z, (row & 3) - 1, prm.pw.w, head);   // the condition does not depend on p
-          }
-#pragma unroll
-          for (int e = 0; e < 40; ++e) head[e] *= kActScale;
-        }
-        if (it > 0) mbar_wait(BAR(kBarPeFree), (uint32_t)((it - 1) & 1), abort_flag, prm.status, 400);
-#pragma unroll
-        for (int chunk = 0; chunk < 5; ++chunk) {          // columns 0..39
-          range_check8(head + 8 * chunk, prm.status, 1101);
-          uint4 hi, lo;
-          split8(head + 8 * chunk, hi, lo);
-          const uint32_t off = sw128_offset(row, chunk);
-          st_shared_v4(base + kOffAHi + off, hi);
-          if (kPasses == 3) st_shared_v4(base + kOffALo + off, lo);
-        }
-#pragma unroll 1
-        for (int chunk = 5; chunk < 24; ++chunk) {         // columns 40..191: cond[1..127] then zeros
-          float v[8];
-#pragma unroll
-          for (int e = 0; e < 8; ++e) {
-            const int ci = 8 * chunk + e - 39;             // index into the condition vector
-            v[e] = (live && value_row && ci < 128) ? __ldg(cond + ci) * kActScale : 0.f;
-          }
-          range_check8(v, prm.status, 1102);
-          uint4 hi, lo;
-          split8(v, hi, lo);
-          const uint32_t off = (uint32_t)(chunk >> 3) * 8192u + sw128_offset(row, chunk & 7);
-          st_shared_v4(base + kOffAHi + off, hi);
-          if (kPasses == 3) st_shared_v4(base + kOffALo + off, lo);
-        }
-      } else {
-        float pe[40];
-        if (p < Ptot) {
-          float cx, cy, cz;
-          ok = fetch_point(prm.src, p, cx, cy, cz);
-          if (!kJvp || (row & 3) == 0) {
-            positional_encode(cx, cy, cz, prm.pw.w, pe);
-          } else {
-            positional_encode_tangent(cx, cy, cz, (row & 3) - 1, prm.pw.w, pe);
-          }
-#pragma unroll
-          for (int e = 0; e < 39; ++e) pe[e] *= kActScale;
-        } else {
-#pragma unroll
-          for (int e = 0; e < 39; ++e) pe[e] = 0.f;
-        }
-        pe[39] = 0.f;
-        if (it > 0) mbar_wait(BAR(kBarPeFree), (uint32_t)((it - 1) & 1), abort_flag, prm.status, 400);
-        const uint4 zero = make_uint4(0, 0, 0, 0);
-#pragma unroll
-        for (int chunk = 0; chunk < 8; ++chunk) {
-          uint4 hi = zero, lo = zero;
-          if (chunk < 5) { range_check8(pe + 8 * chunk, prm.status, 1103); split8(pe + 8 * chunk, hi, lo); }
-          const uint32_t off = sw128_offset(row, chunk);
-          st_shared_v4(base + kOffPeHi + off, hi);
-          st_shared_v4(base + kOffPeLo + off, lo);
-        }
+        stall_add(stall, true, kStProducerTotal, t_loop);
+        stall_end(stall, true);
       }
-      valid[(it & 1) * 64 + row] = ok ? 1 : 0;
-      fence_proxy_async();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_local(BAR(kBarPeReady));
+    } else {
+      // ================================ prologue for the next tile ========================
+      const int row = (warp - kPrologueWarp) * 32 + lane;
+      for (long long it = 0; it < n_iter; ++it) {
+        const long long tile = tile_of(it);
+        const long long p = kJvp ? tile * kPtsPerTile + (row >> 2) : tile * kPtsPerTile + row;
+        bool ok = true;
+        if (kNet == 2) {
+          // colour-network input row, 8 columns at a time straight into the activation buffer (K blocks 0..4)
+          float head[40];   // [p 3 | PE4(v) 27 | n 3 | feat 0..6]
+#pragma unroll
+          for (int e = 0; e < 40; ++e) head[e] = 0.f;
+          const bool live = p < Ptot;
+          const float* ft = prm.feats + (size_t)(live ? p : 0) * 256;
+          if (live) {
+            float pe[39];
+            positional_encode(__ldg(prm.view_dirs + 3 * p), __ldg(prm.view_dirs + 3 * p + 1), __ldg(prm.view_dirs + 3 * p + 2),
+                              prm.pw.w, pe);   // the first 27 entries of a 6-band encoding are the 4-band encoding
+#pragma unroll
+            for (int e = 0; e < 3; ++e) { head[e] = __ldg(prm.src.x + 3 * p + e); head[30 + e] = __ldg(prm.normals + 3 * p + e); }
+#pragma unroll
+            for (int e = 0; e < 27; ++e) head[3 + e] = pe[e];
+#pragma unroll
+            for (int e = 0; e < 7; ++e) head[33 + e] = __ldg(ft + e);
+          }
+          if (it > 0) mbar_wait(BAR(kBarPeFree), (uint32_t)((it - 1) & 1), abort_flag, prm.status, 400);
+#pragma unroll 1
+          for (int chunk = 0; chunk < 40; ++chunk) {
+            float v[8];
+#pragma unroll
+            for (int e = 0; e < 8; ++e) {
+              const int col = 8 * chunk + e;              // feature j sits in column 33 + j
+              v[e] = (live && col >= 40 && col < 289) ? __ldg(ft + (col - 33)) : 0.f;
+            }
+            if (chunk < 5) {
+#pragma unroll
+              for (int c5 = 0; c5 < 5; ++c5)
+                if (chunk == c5) {
+#pragma unroll
+                  for (int e = 0; e < 8; ++e) v[e] = head[8 * c5 + e];
+                }
+            }
+#pragma unroll
+            for (int e = 0; e < 8; ++e) v[e] *= kActScale;
+            range_check8(v, prm.status, 1100);
+            uint4 hi, lo;
+            split8(v, hi, lo);
+            const uint32_t off = (uint32_t)(chunk >> 3) * 8192u + sw128_offset(row, chunk & 7);
+            st_shared_v4(base + kOffAHi + off, hi);
+            if (kPasses == 3) st_shared_v4(base + kOffALo + off, lo);
+          }
+        } else if (kNet == 1) {
+          // deformer input row: [PE(p) (39) | cond[frame] (128) | 0 (25)] = three 64-wide K blocks written into the
+          // activation buffer itself (free again once the previous tile's last layer has been issued and done)
+          // (written 8 columns at a time; only the 40-wide head [PE | first cond value] lives in registers)
+          float head[40];
+#pragma unroll
+          for (int e = 0; e < 40; ++e) head[e] = 0.f;
+          const bool live = p < Ptot;
+          const bool value_row = !kJvp || (row & 3) == 0;
+          const float* cond = prm.conds;
+          if (live) {
+            const float x = __ldg(prm.src.x + 3 * p), y = __ldg(prm.src.x + 3 * p + 1), z = __ldg(prm.src.x + 3 * p + 2);
+            if (value_row) {
+              positional_encode(x, y, z, prm.pw.w, head);
+              long long f = prm.batch_inds ? prm.batch_inds[p] : (prm.points_per_frame > 0 ? p / prm.points_per_frame : 0);
+              f = f < 0 ? 0 : (f >= prm.num_frames ? prm.num_frames - 1 : f);
+              cond = prm.conds + (size_t)f * 128;
+              head[39] = __ldg(cond);
+            } else {
+              positional_encode_tangent(x, y, z, (row & 3) - 1, prm.pw.w, head);   // the condition does not depend on p
+            }
+#pragma unroll
+            for (int e = 0; e < 40; ++e) head[e] *= kActScale;
+          }
+          if (it > 0) mbar_wait(BAR(kBarPeFree), (uint32_t)((it - 1) & 1), abort_flag, prm.status, 400);
+#pragma unroll
+          for (int chunk = 0; chunk < 5; ++chunk) {          // columns 0..39
+            range_check8(head + 8 * chunk, prm.status, 1101);
+            uint4 hi, lo;
+            split8(head + 8 * chunk, hi, lo);
+            const uint32_t off = sw128_offset(row, chunk);
+            st_shared_v4(base + kOffAHi + off, hi);
+            if (kPasses == 3) st_shared_v4(base + kOffALo + off, lo);
+          }
+#pragma unroll 1
+          for (int chunk = 5; chunk < 24; ++chunk) {         // columns 40..191: cond[1..127] then zeros
+            float v[8];
+#pragma unroll
+            for (int e = 0; e < 8; ++e) {
+              const int ci = 8 * chunk + e - 39;             // index into the condition vector
+              v[e] = (live && value_row && ci < 128) ? __ldg(cond + ci) * kActScale : 0.f;
+            }
+            range_check8(v, prm.status, 1102);
+            uint4 hi, lo;
+            split8(v, hi, lo);
+            const uint32_t off = (uint32_t)(chunk >> 3) * 8192u + sw128_offset(row, chunk & 7);
+            st_shared_v4(base + kOffAHi + off, hi);
+            if (kPasses == 3) st_shared_v4(base + kOffALo + off, lo);
+          }
+        } else {
+          float pe[40];
+          if (p < Ptot) {
+            float cx, cy, cz;
+            ok = fetch_point(prm.src, p, cx, cy, cz);
+            if (!kJvp || (row & 3) == 0) {
+              positional_encode(cx, cy, cz, prm.pw.w, pe);
+            } else {
+              positional_encode_tangent(cx, cy, cz, (row & 3) - 1, prm.pw.w, pe);
+            }
+#pragma unroll
+            for (int e = 0; e < 39; ++e) pe[e] *= kActScale;
+          } else {
+#pragma unroll
+            for (int e = 0; e < 39; ++e) pe[e] = 0.f;
+          }
+          pe[39] = 0.f;
+          if (it > 0) mbar_wait(BAR(kBarPeFree), (uint32_t)((it - 1) & 1), abort_flag, prm.status, 400);
+          const uint4 zero = make_uint4(0, 0, 0, 0);
+#pragma unroll
+          for (int chunk = 0; chunk < 8; ++chunk) {
+            uint4 hi = zero, lo = zero;
+            if (chunk < 5) { range_check8(pe + 8 * chunk, prm.status, 1103); split8(pe + 8 * chunk, hi, lo); }
+            const uint32_t off = sw128_offset(row, chunk);
+            st_shared_v4(base + kOffPeHi + off, hi);
+            st_shared_v4(base + kOffPeLo + off, lo);
+          }
+        }
+        valid[(it & 1) * 64 + row] = ok ? 1 : 0;
+        fence_proxy_async();
+        __syncwarp();
+        if (lane == 0) mbar_arrive_local(BAR(kBarPeReady));
+      }
     }
   }
 }
