@@ -229,48 +229,20 @@ RECMV_API int recmv_sdf_mlp_fwd_counted(const float* x, const void* packed, cons
 /* ---- A2/A3 training path: what `loss.backward()` (train.py:325) runs through model/network.py:89-119 ---------
  * (and through Deformer.py:171-206 / RenderNet.py:59-96 -- the entry points below are generic over the layer list).
  *
- * recmv_mlp_fwd_layer: Y = act(pre_scale * (X . W^T) + bias) for ONE layer on the tensor cores (3 fp16 MMAs per product, fp32
- *   accumulation) -- the TRAINING forward, whose layer outputs stay in HBM as the inputs the backward needs (what
- *   autograd would save): X [P][ldx] (in_dim columns used), W [out_dim][in_dim] row-major fp32 (nn.Linear layout),
- *   bias [out_dim] or NULL, act: 0 none, 1 softplus(beta 100, threshold 20), 2 ReLU.  Columns n < split -> Y[p*ldy+n],
- *   columns n >= split -> Y2[p*ldy2 + n - split] (split <= 0: all to Y; the SDF output layer splits sdf | features).
  * recmv_pe_forward: positional encoding rows (model/Embedder.py:43-50 with the annealing weights pe_w [2*bands] host)
  *   written as a saved layer input: out[p*ld + e], e < 3 + 6*bands; out2 (optional) gets the same row.
  *
- * recmv_mlp_bwd_data_layer: G_prev = (G . W) * act'(saved_input)  for ONE layer, on the tensor cores (3 fp16 MMAs per product):
- *   G [P][ldg] cotangent of the layer output (out_dim columns used), W [out_dim][in_dim] row-major fp32 (the
- *   nn.Linear layout -- no transposed copy), saved_input [P][lds] = the layer's input as saved by the forward
- *   (= the previous layer's activation output), act: 0 none, 1 softplus(beta 100) -> 1 - exp(-100 a), 2 ReLU -> a > 0.
- *   Columns n < split go to G_prev[p * ldgp + n] with the activation derivative; columns n >= split (the PE part
- *   of the SDF skip layer; split <= 0 = none) go to D2[p * ldd2 + n - split] untouched.  out_scale multiplies
- *   everything (1/sqrt2 for the SDF skip layer).  dyn_scale: optional DEVICE scalar, a power of two that brings
- *   max|G| near 1 before the fp16 split (gradients of mean-reduced losses are ~1/P); results are unscaled again.
- *
- * recmv_mlp_bwd_weight: for every layer l < num_layers in ONE launch:  dW[l] [out][in] = out_scale[l] * G[l]^T X[l]
- *   (reduction over the P samples, accumulated in chunks of 2048 samples; tile owner adds chunks in fp32 -- no atomics,
- *   deterministic) and db[l] [out] += column sums of G[l] (db must be zero-filled by the caller; may be NULL).
- *   G, ldg, X, ldx, out_dim, in_dim, dW, db, out_scale are HOST arrays of length num_layers (<= 10).
- *
  * recmv_pe_backward: dx [P,3] (+)= (d PE / d x)^T (g + g2): g [P][ldg] cotangent of the 3 + 6*bands encoding
  *   (model/Embedder.py:43-50 order), g2 optional second cotangent of the same encoding, pe_w [2*bands] host.       */
-RECMV_API int recmv_mlp_fwd_layer(const float* X, int64_t ldx, const float* W, const float* bias, int out_dim, int in_dim,
-                        int act, float pre_scale, int split, float* Y, int64_t ldy, float* Y2, int64_t ldy2, int64_t P,
-                        recmv_stream_t stream);
 RECMV_API int recmv_pe_forward(const float* x, const float* pe_w /*host*/, int bands, float* out, int64_t ld, float* out2,
                      int64_t ld2, int64_t P, recmv_stream_t stream);
-RECMV_API int recmv_mlp_bwd_data_layer(const float* G, int64_t ldg, const float* W, int out_dim, int in_dim,
-                             const float* saved_input, int64_t lds, int act, int split, float* G_prev, int64_t ldgp,
-                             float* D2, int64_t ldd2, float out_scale, const float* dyn_scale /*device*/, int64_t P,
-                             recmv_stream_t stream);
-RECMV_API int recmv_mlp_bwd_weight(int num_layers, const float* const* G, const int64_t* ldg, const float* const* X,
-                         const int64_t* ldx, const int* out_dim, const int* in_dim, float* const* dW, float* const* db,
-                         const float* out_scale, const float* dyn_scale /*device*/, int64_t P, recmv_stream_t stream);
 RECMV_API int recmv_pe_backward(const float* x, const float* g, int64_t ldg, const float* g2, int64_t ldg2,
                       const float* pe_w /*host*/, int bands, float* dx, int accumulate, int64_t P,
                       recmv_stream_t stream);
 
-/* Second-generation layer GEMMs: operands as fp16 hi / lo PLANES in HBM, fed by TMA (csrc/gemm3_tma.cu) -- every tensor a
- * later GEMM consumes is written in consumable form by its producer, the main loop converts nothing.
+/* Layer GEMMs (3 fp16 MMAs per product, fp32 accumulation): operands as fp16 hi / lo PLANES in HBM, fed by TMA
+ * (csrc/gemm3_tma.cu) -- every tensor a later GEMM consumes is written in consumable form by its producer, the main
+ * loop converts nothing.
  *  recmv_split_planes      : fp32 [R][C] (row stride ld) -> planes hi = fp16(s v), lo = fp16(s v - hi), s = scale * (*scale_dev
  *                            if given); transpose != 0 writes [C][R].  ldp = plane row stride in elements (multiple of 8, plane
  *                            base 16-byte aligned).  Weights: scale 1024 ([out][in] for the forward, transposed for

@@ -78,14 +78,7 @@ SIGNATURES = {
                                   c_int, c_void_p]),
     "recmv_sdf_mlp_fwd_grad": (c_int, [c_void_p, c_void_p, POINTER(c_float), c_void_p, c_void_p, c_void_p, c_int64,
                                        c_int, c_void_p]),
-    "recmv_mlp_fwd_layer": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_int, c_void_p,
-                                    c_int64, c_void_p, c_int64, c_int64, c_void_p]),
     "recmv_pe_forward": (c_int, [c_void_p, POINTER(c_float), c_int, c_void_p, c_int64, c_void_p, c_int64, c_int64, c_void_p]),
-    "recmv_mlp_bwd_data_layer": (c_int, [c_void_p, c_int64, c_void_p, c_int, c_int, c_void_p, c_int64, c_int, c_int,
-                                         c_void_p, c_int64, c_void_p, c_int64, c_float, c_void_p, c_int64, c_void_p]),
-    "recmv_mlp_bwd_weight": (c_int, [c_int, POINTER(c_void_p), POINTER(c_int64), POINTER(c_void_p), POINTER(c_int64),
-                                     POINTER(c_int), POINTER(c_int), POINTER(c_void_p), POINTER(c_void_p),
-                                     POINTER(c_float), c_void_p, c_int64, c_void_p]),
     "recmv_pe_backward": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_int64, POINTER(c_float), c_int, c_void_p,
                                   c_int, c_int64, c_void_p]),
     "recmv_split_planes": (c_int, [c_void_p, c_int64, c_int64, c_int, c_float, c_void_p, c_int, c_void_p, c_void_p, c_int64,

@@ -1,9 +1,8 @@
-// Training-path layer GEMMs, second generation: forward layers and backward-data with BOTH operands already split into
-// fp16 hi / lo planes in HBM and fed by TMA -- no conversion in the main loop.
+// Training-path layer GEMMs: forward layers and backward-data with BOTH operands already split into fp16 hi / lo planes in
+// HBM and fed by TMA -- no conversion in the main loop.  Every fp32 value a product reads is a = hi + lo of two fp16
+// values, and a product is 3 MMAs (hi*hi + lo*hi + hi*lo) with fp32 accumulation.
 //
-// gemm3.cu converts fp32 operands inside its main loop (eight producer warps: load -> scale -> split -> st.shared), and
-// that chain bounds it.  Here every tensor a later GEMM consumes is WRITTEN in consumable form by the kernel that
-// produces it:
+// Every tensor a later GEMM consumes is WRITTEN in consumable form by the kernel that produces it:
 //   * a layer's output  Y  -> fp32 [P][ld] (activation derivative, weight gradient) AND two fp16 planes [P][ldp]
 //     hi = fp16(64 y), lo = fp16(64 y - hi)  (K-major rows: exactly what the next layer's A operand is);
 //   * a cotangent       G  -> fp32 AND planes of 64 * dyn * g  (dyn = the call's power-of-two gradient scale, device scalar);
@@ -65,7 +64,8 @@ __device__ __forceinline__ float softplus100_fast(float z) {
 }  // namespace
 
 // One 64-wide K block of the 3-pass product (K-major operands) into a warpgroup's [64 x 128] accumulator: A rows
-// 64 g .. 64 g + 63 of the stage.  Correction products first, then hi*hi (see gemm3.cu).
+// 64 g .. 64 g + 63 of the stage.  Correction products first (they are 2^-11 of the result: added while the K block's
+// contribution is still small they cost no accumulator precision), then hi*hi.
 __device__ __forceinline__ void mma_kblock3_k(float (&acc)[64], uint32_t st, int g, bool first) {
   const uint64_t a_hi = smem_desc_sw128(st + (uint32_t)g * 8192u), a_lo = smem_desc_sw128(st + kPlane + (uint32_t)g * 8192u);
   const uint64_t b_hi = smem_desc_sw128(st + 2 * kPlane), b_lo = smem_desc_sw128(st + 3 * kPlane);
@@ -221,7 +221,7 @@ gemm3_tma_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_const
 // advances the start address by 16 rows = 2048 B.  So the weight gradient needs NO transposed copy of anything.
 // Work split: the output is at most 4 x 4 tiles, so the sample range is split over CTAs (grid = tiles x splits, one wave);
 // inside a CTA the accumulation runs in chunks of 32 K blocks, each chunk's accumulator added into fp32 registers (a
-// 10^5-sample reduction in one truncating accumulator would be cut short, gemm3.cu); partial tiles go to a workspace and
+// 10^5-sample reduction in one truncating accumulator would be cut short, DESIGN.md 5b); partial tiles go to a workspace and
 // are summed in split order by a second launch (deterministic).
 struct WgParams {
   float* ws;                 // [splits][tiles_m * 128][tiles_n * 128] raw partial sums (accumulator units, gain applied)
@@ -480,6 +480,47 @@ __global__ void __launch_bounds__(256) add_split_kernel(float* __restrict__ y, l
   }
 }
 
+// d PE / d x applied to a cotangent: dx_j = g[j] + sum_k f_k (w_sin_k cos(f_k x_j) g[3+6k+j] - w_cos_k sin(f_k x_j) g[3+6k+3+j])
+// (model/Embedder.py:43-50 order; `bands` = 6 for points, 4 for view directions).  g2: optional second cotangent of the
+// same encoding (the SDF network's skip connection), added before the contraction.
+__global__ void __launch_bounds__(256) pe_backward_kernel(const float* __restrict__ x, const float* __restrict__ g,
+                                                          long long ldg, const float* __restrict__ g2, long long ldg2,
+                                                          PeWeights pw, int bands, float* __restrict__ dx, long long P,
+                                                          int accumulate) {
+  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (i >= 3 * P) return;
+  const long long p = i / 3;
+  const int j = (int)(i - 3 * p);
+  const float* gp = g + p * ldg;
+  const float* gq = g2 ? g2 + p * ldg2 : nullptr;
+  auto G = [&](int e) { return gp[e] + (gq ? gq[e] : 0.f); };
+  const float xj = x[i];
+  float acc = G(j);
+  float f = 1.f;
+  for (int k = 0; k < bands; ++k) {
+    float sn, cs;
+    sincosf(xj * f, &sn, &cs);
+    acc += f * (pw.w[2 * k] * cs * G(3 + 6 * k + j) - pw.w[2 * k + 1] * sn * G(3 + 6 * k + 3 + j));
+    f *= 2.f;
+  }
+  dx[i] = accumulate ? dx[i] + acc : acc;
+}
+// positional encoding written as a saved layer input: out[p * ld + e], e < 3 + 6 * bands (model/Embedder.py:43-50);
+// out2 (optional) receives the same row (the SDF network's skip input)
+__global__ void __launch_bounds__(256) pe_forward_kernel(const float* __restrict__ x, PeWeights pw, int bands,
+                                                         float* __restrict__ out, long long ld, float* __restrict__ out2,
+                                                         long long ld2, long long P) {
+  const long long p = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (p >= P) return;
+  float pe[39];
+  positional_encode(x[3 * p], x[3 * p + 1], x[3 * p + 2], pw.w, pe);
+  const int n = 3 + 6 * bands;
+  for (int e = 0; e < n; ++e) {
+    out[p * ld + e] = pe[e];
+    if (out2) out2[p * ld2 + e] = pe[e];
+  }
+}
+
 // positional encoding as a saved layer input AND as operand planes.  One thread per (point, column): consecutive threads write
 // consecutive columns (the one-thread-per-point form wrote 39-element rows at a 2 KB stride from every lane: 139 us for 131 k
 // points under ncu).  Same arithmetic as positional_encode (common.cuh): w * sin / cos (2^k x), accurate sincosf.
@@ -574,6 +615,31 @@ extern "C" int recmv_add_split_planes(float* y, int64_t ldy, const float* addend
   if (s0) return s0;
   add_split_kernel<<<stride_grid(rows * (int64_t)cols, 256, 8), 256, 0, (cudaStream_t)stream>>>(
       y, ldy, addend, lda, rows, cols, scale, scale_dev, (__half*)y_hi, (__half*)y_lo, ldp, (DevStatus*)sd);
+  return launch_status();
+}
+
+extern "C" int recmv_pe_forward(const float* x, const float* pe_w, int bands, float* out, int64_t ld, float* out2,
+                                int64_t ld2, int64_t P, recmv_stream_t stream) {
+  if (P < 0 || bands < 0 || bands > 6) return RECMV_E_SHAPE;
+  if (P == 0) return RECMV_OK;
+  if (!x || !pe_w || !out) return RECMV_E_NULL;
+  PeWeights pw;
+  for (int i = 0; i < 12; ++i) pw.w[i] = i < 2 * bands ? pe_w[i] : 0.f;
+  pe_forward_kernel<<<(unsigned)((P + 255) / 256), 256, 0, (cudaStream_t)stream>>>(x, pw, bands, out, ld, out2, ld2, P);
+  return launch_status();
+}
+
+extern "C" int recmv_pe_backward(const float* x, const float* g, int64_t ldg, const float* g2, int64_t ldg2,
+                                 const float* pe_w, int bands, float* dx, int accumulate, int64_t P,
+                                 recmv_stream_t stream) {
+  if (P < 0 || bands < 0 || bands > 6) return RECMV_E_SHAPE;
+  if (P == 0) return RECMV_OK;
+  if (!x || !g || !pe_w || !dx) return RECMV_E_NULL;
+  PeWeights pw;
+  for (int i = 0; i < 12; ++i) pw.w[i] = i < 2 * bands ? pe_w[i] : 0.f;
+  const long long n = 3 * P;
+  pe_backward_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(x, g, ldg, g2, ldg2, pw, bands, dx, P,
+                                                                                   accumulate);
   return launch_status();
 }
 

@@ -167,7 +167,7 @@ __device__ __forceinline__ uint32_t sw128_elem(int row, int col) {
 }
 
 // Gain that undoes the tensor core's truncating fp32 accumulation after `kblocks` 64-wide K blocks of 3-pass MMAs into
-// one accumulator (the layer GEMMs of gemm3.cu / gemm3_tma.cu): the signed projection <ours, fp64> / <fp64, fp64> - 1 of
+// one accumulator (the layer GEMMs of gemm3_tma.cu): the signed projection <ours, fp64> / <fp64, fp64> - 1 of
 // a GEMM's output is ~ -(3.23 n - 1.5) 2^-24 after n K blocks (the first MMA overwrites the accumulator and loses
 // nothing; later ones drop a fraction of an ulp of a growing sum).
 __host__ __device__ __forceinline__ float acc_trunc_gain(int kblocks) {

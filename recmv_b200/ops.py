@@ -688,9 +688,6 @@ def sdf_value_and_grad(x, packed, pe_w=None, mode=None, want_feat=False):
 # --------------------------------------------------------------------------------------------------
 # Training path: layer GEMMs that save their outputs for the backward (csrc/gemm3_tma.cu)
 # --------------------------------------------------------------------------------------------------
-# Activation codes of the fp32-operand entries of csrc/gemm3.cu (mlp_fwd_layer, mlp_bwd_data_layer), which the ReLU
-# networks' create_graph input gradient (second_order.PlainMlpInputGradFunction) still runs on.
-ACT_NONE, ACT_SOFTPLUS100, ACT_RELU = 0, 1, 2
 import os as _os
 # create_graph=True input gradients: "1" = differentiable reverse chain on the tensor-core GEMMs (second_order.py), "0" = torch graph
 SECOND_ORDER_FUSED = _os.environ.get("RECMV_SECOND_ORDER", "1") != "0"
@@ -718,10 +715,6 @@ def _inputs_only(need_params):
 _INV_SQRT2 = 0.70710678118654752440
 
 
-def _ptr_array(tensors):
-    return (ctypes.c_void_p * len(tensors))(*[t.data_ptr() if t is not None else None for t in tensors])
-
-
 def grad_dyn_scale(*cotangents):
     """Device scalar 2^-floor(log2(max|g|)) (1 for an all-zero cotangent): brings the largest cotangent entry into
     [1, 2) before the fp16 hi/lo split of the backward GEMMs; no host synchronisation."""
@@ -729,48 +722,6 @@ def grad_dyn_scale(*cotangents):
     e = torch.floor(torch.log2(m.clamp_min(1e-30)))
     s = torch.exp2(-e.clamp(-100.0, 100.0))
     return torch.where(m > 0, s, torch.ones_like(s)).reshape(1).contiguous()
-
-
-def mlp_bwd_data_layer(G, W, out_dim, in_dim, saved_input, act, G_prev, split=0, D2=None, out_scale=1.0, dyn_scale=None):
-    """G_prev[:, :split] = ((G[:, :out_dim] @ W) * out_scale)[:, :split] * act'(saved_input); columns >= split -> D2.
-    fp32 operands (csrc/gemm3.cu); its product caller is second_order.PlainMlpInputGradFunction's reverse chain."""
-    P = G.shape[0]
-    with torch.cuda.device(G.device):
-        check(_lib.load().recmv_mlp_bwd_data_layer(
-            _ptr(G), G.stride(0), _ptr(W), int(out_dim), int(in_dim), _ptr(saved_input),
-            saved_input.stride(0) if saved_input is not None else 0, int(act), int(split), _ptr(G_prev), G_prev.stride(0),
-            _ptr(D2), D2.stride(0) if D2 is not None else 0, float(out_scale), _ptr(dyn_scale), P, _stream(G)),
-            "recmv_mlp_bwd_data_layer")
-    return G_prev
-
-
-def mlp_bwd_weight(Gs, Xs, out_dims, in_dims, out_scales=None, dyn_scale=None, want_bias=True):
-    """dW[l] = out_scale[l] * Gs[l][:, :out]^T @ Xs[l][:, :in] and db[l] = Gs[l][:, :out].sum(0), all layers in one launch.
-    fp32 operands (csrc/gemm3.cu); its product caller is second_order.PlainMlpInputGradFunction's backward."""
-    n = len(Gs)
-    dev = Gs[0].device
-    P = Gs[0].shape[0]
-    dW = [torch.empty((o, i), dtype=torch.float32, device=dev) for o, i in zip(out_dims, in_dims)]
-    db = [torch.zeros((o,), dtype=torch.float32, device=dev) for o in out_dims] if want_bias else None
-    scales = (c_float * n)(*[float(v) for v in (out_scales or [1.0] * n)])
-    with torch.cuda.device(dev):
-        check(_lib.load().recmv_mlp_bwd_weight(
-            n, _ptr_array(Gs), (c_int64 * n)(*[g.stride(0) for g in Gs]), _ptr_array(Xs),
-            (c_int64 * n)(*[x.stride(0) for x in Xs]), (ctypes.c_int * n)(*out_dims), (ctypes.c_int * n)(*in_dims),
-            _ptr_array(dW), _ptr_array(db) if db is not None else None, scales, _ptr(dyn_scale), P, _stream(Gs[0])),
-            "recmv_mlp_bwd_weight")
-    return dW, db
-
-
-def mlp_fwd_layer(X, W, bias, out_dim, in_dim, act, Y, pre_scale=1.0, split=0, Y2=None):
-    """Y[:, :split or out] (and Y2) = act(pre_scale * X[:, :in] @ W.T + bias) on the tensor cores, one layer, fp32 operands
-    (csrc/gemm3.cu); its product caller is the tangent pass of second_order.PlainMlpInputGradFunction's backward."""
-    P = X.shape[0]
-    with torch.cuda.device(X.device):
-        check(_lib.load().recmv_mlp_fwd_layer(_ptr(X), X.stride(0), _ptr(W), _ptr(bias), int(out_dim), int(in_dim), int(act),
-                                              float(pre_scale), int(split), _ptr(Y), Y.stride(0), _ptr(Y2),
-                                              Y2.stride(0) if Y2 is not None else 0, P, _stream(X)), "recmv_mlp_fwd_layer")
-    return Y
 
 
 def pe_forward(x, pe_w, bands, out, out2=None):
@@ -1093,33 +1044,39 @@ def _plain_mlp_forward(X0, Ws, bs):
     return acts[-1][:, :Ws[-1].shape[0]], acts[:-1], xplanes
 
 
-def _plain_mlp_backward(g_out, Ws, acts, need_w, need_x0, xplanes):
-    """g_out [P, out_last] -> (dX0 [P, in_0 padded] or None, dW list, db list) for the ReLU MLP.  xplanes: the layer inputs'
-    operand planes from the forward (flat hi, lo list), the weight gradient's second operand."""
+def plain_reverse_chain(g_out, Ws, acts, with_layer0=True):
+    """Backward-data chain of a ReLU MLP on the operand-plane GEMMs, from the layer inputs `acts` its training forward
+    saved: g_out [P, out_last] -> (dyn, GP, dX0).  GP[l] holds the planes of 64 * dyn * the cotangent at layer l's output
+    (after the ReLU derivative), dX0 [P, in_0 rounded up to 4] that of the network input (None without with_layer0)."""
     P, dev = g_out.shape[0], g_out.device
     n = len(Ws)
     o_last = Ws[-1].shape[0]
-    G = [None] * n
-    G[n - 1] = torch.zeros((P, _pad8(o_last)), dtype=torch.float32, device=dev)
-    G[n - 1][:, :o_last] = g_out
-    dyn = grad_dyn_scale(G[n - 1])
-    gp = split_planes(G[n - 1], P, o_last, 64.0, scale_dev=dyn, ldp=_pad8(o_last))
+    G = torch.zeros((P, _pad8(o_last)), dtype=torch.float32, device=dev)
+    G[:, :o_last] = g_out
+    dyn = grad_dyn_scale(G)
     GP = [None] * n
-    GP[n - 1] = gp
+    GP[n - 1] = split_planes(G, P, o_last, 64.0, scale_dev=dyn, ldp=_pad8(o_last))
     for l in range(n - 1, 0, -1):
         o, i = Ws[l].shape
-        G[l - 1] = torch.empty((P, i), dtype=torch.float32, device=dev)
-        gprev = _plane_pair(P, _pad8(i), dev)
-        mlp_layer_planes(gp, split_planes(Ws[l].detach(), o, i, 1024.0, transpose=True), P, i, o, 2, G[l - 1],
-                         saved_input=acts[l], dyn=dyn, a_has_dyn=True, y_planes=gprev, planes_with_dyn=True)
-        gp = gprev
-        GP[l - 1] = gp
+        G = torch.empty((P, i), dtype=torch.float32, device=dev)
+        GP[l - 1] = _plane_pair(P, _pad8(i), dev)
+        mlp_layer_planes(GP[l], split_planes(Ws[l].detach(), o, i, 1024.0, transpose=True), P, i, o, 2, G,
+                         saved_input=acts[l], dyn=dyn, a_has_dyn=True, y_planes=GP[l - 1], planes_with_dyn=True)
     dX0 = None
-    if need_x0:
+    if with_layer0:
         o, i = Ws[0].shape
         dX0 = torch.empty((P, ((i + 3) // 4) * 4), dtype=torch.float32, device=dev)
-        mlp_layer_planes(gp, split_planes(Ws[0].detach(), o, i, 1024.0, transpose=True), P, i, o, 0, dX0, dyn=dyn,
+        mlp_layer_planes(GP[0], split_planes(Ws[0].detach(), o, i, 1024.0, transpose=True), P, i, o, 0, dX0, dyn=dyn,
                          a_has_dyn=True)
+    return dyn, GP, dX0
+
+
+def _plain_mlp_backward(g_out, Ws, acts, need_w, need_x0, xplanes):
+    """g_out [P, out_last] -> (dX0 [P, in_0 padded] or None, dW list, db list) for the ReLU MLP.  xplanes: the layer inputs'
+    operand planes from the forward (flat hi, lo list), the weight gradient's second operand."""
+    P = g_out.shape[0]
+    n = len(Ws)
+    dyn, GP, dX0 = plain_reverse_chain(g_out, Ws, acts, need_x0)
     dW, db = [None] * n, [None] * n
     if need_w:
         for l in range(n):

@@ -16,18 +16,17 @@ is itself an autograd Function whose backward is
     downward : an ordinary backward-data pass that picks zb_l up at every layer                       (8 layer GEMMs)
     weights  : dW_l = h_{l+1}^T tu_l + zb_l^T a_l,  db_l = sum zb_l
 
-with h_{l+1} the first-order cotangent at z_l.  Everything heavy is a 3xfp16 wgmma GEMM.  The SDF network's reverse chain is
-the first-order path's own (ops.sdf_reverse_chain), and all its passes run on the operand-plane kernels of
-csrc/gemm3_tma.cu, each followed by one element-wise launch that also writes the next GEMM's planes.  The translator and
-colour networks' reverse chain and its backward (PlainMlpInputGradFunction) run on the fp32-operand GEMM entries of
-csrc/gemm3.cu with torch element-wise ops; it is the one product caller of those entries.  The positional encoding's own
-VJP is a torch graph (so its second derivative comes from autograd).  A request that ALSO wants parameter gradients with a
-graph (loss.backward(create_graph=True)) still takes the torch-composite fallback."""
+with h_{l+1} the first-order cotangent at z_l.  Everything heavy is a 3xfp16 wgmma GEMM on the operand-plane kernels of
+csrc/gemm3_tma.cu.  Each network's reverse chain is its first-order path's own (ops.sdf_reverse_chain,
+ops.plain_reverse_chain).  In the SDF network's backward every GEMM is followed by one element-wise launch that also writes
+the next GEMM's planes; the ReLU networks' tangent pass applies the ReLU mask in the GEMM epilogue and needs no such
+launch.  The positional encoding's own VJP is a torch graph (so its second derivative comes from autograd).  A request
+that ALSO wants parameter gradients with a graph (loss.backward(create_graph=True)) still takes the torch-composite
+fallback."""
 import torch
 
 from . import ops
-from .ops import (ACT_NONE, ACT_RELU, _INV_SQRT2, _plane_pair, grad_dyn_scale, mlp_bwd_data_layer, mlp_bwd_weight,
-                  mlp_fwd_layer, mlp_layer_planes, pe_backward, split_planes)
+from .ops import _INV_SQRT2, _pad8, _plane_pair, grad_dyn_scale, mlp_layer_planes, pe_backward, split_planes
 
 
 def pe_vjp_torch(x, u, pe_w, bands):
@@ -148,50 +147,41 @@ class PlainMlpInputGradFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, g_out, n, *rest):
         acts, Ws = rest[:n], rest[n:2 * n]
-        P, dev = g_out.shape[0], g_out.device
-        Wd = [w.detach().contiguous().float() for w in Ws]
-        o_last = Wd[-1].shape[0]
-        G = [None] * n
-        G[n - 1] = torch.zeros((P, ops._pad8(o_last)), dtype=torch.float32, device=dev)
-        G[n - 1][:, :o_last] = g_out.detach()
-        dyn = grad_dyn_scale(G[n - 1])
-        for l in range(n - 1, 0, -1):
-            o, i = Wd[l].shape
-            G[l - 1] = torch.zeros((P, i), dtype=torch.float32, device=dev)
-            mlp_bwd_data_layer(G[l], Wd[l], o, i, acts[l], ACT_RELU, G[l - 1], dyn_scale=dyn)
-        o, i = Wd[0].shape
-        dX0 = torch.zeros((P, ((i + 3) // 4) * 4), dtype=torch.float32, device=dev)
-        mlp_bwd_data_layer(G[0], Wd[0], o, i, None, ACT_NONE, dX0, dyn_scale=dyn)
+        dyn, GP, dX0 = ops.plain_reverse_chain(g_out, Ws, acts)
         ctx.n = n
-        ctx.save_for_backward(dyn, *acts, *Ws, *G)
-        return dX0[:, :i]
+        ctx.save_for_backward(dyn, *acts, *Ws, *[t for pair in GP for t in pair])
+        return dX0[:, :Ws[0].shape[1]]
 
     @staticmethod
     @torch.autograd.function.once_differentiable
     def backward(ctx, q):
+        """Tangent pass on the plane GEMMs: U_{l+1} = (U_l W_l^T) * [a_{l+1} > 0], one backward-data launch with the ReLU'
+        epilogue per layer (the [out][in] weight planes make it the forward product), then dW_l = h_{l+1}^T U_l from the
+        cotangent planes the forward saved and the tangent planes."""
         n = ctx.n
         saved = ctx.saved_tensors
         dyn = saved[0]
-        acts, Ws, G = saved[1:1 + n], saved[1 + n:1 + 2 * n], saved[1 + 2 * n:1 + 3 * n]
+        acts, Ws, GPl = saved[1:1 + n], saved[1 + n:1 + 2 * n], saved[1 + 2 * n:]
         need = ctx.needs_input_grad
         P, dev = q.shape[0], q.device
-        Wd = [w.detach().contiguous().float() for w in Ws]
         dq = grad_dyn_scale(q)
         inv_dq = 1.0 / dq
-        i0 = Wd[0].shape[1]
-        U = [torch.zeros((P, acts[0].shape[1]), dtype=torch.float32, device=dev)]
-        U[0][:, :i0] = q[:, :i0] * dq
-        tz = None
-        for l in range(n):
-            o, i = Wd[l].shape
-            last = l == n - 1
-            tz = torch.empty((P, o if not last else ((o + 3) // 4) * 4), dtype=torch.float32, device=dev)
-            mlp_fwd_layer(U[l], Wd[l], None, o, i, ACT_NONE, tz)
-            if not last:
-                U.append(torch.where(acts[l + 1][:, :o] > 0, tz, torch.zeros_like(tz)))
-        g_bar = (tz[:, :Wd[-1].shape[0]] * inv_dq).contiguous() if need[0] else None
+        i0 = Ws[0].shape[1]
+        UP = [split_planes(q * dq, P, i0, 64.0, ldp=_pad8(i0))]
+        for l in range(n - 1):
+            o, i = Ws[l].shape
+            un = _plane_pair(P, _pad8(o), dev)
+            mlp_layer_planes(UP[l], ops.weight_planes(Ws[l]), P, o, i, 2, torch.empty((P, o), dtype=torch.float32, device=dev),
+                             saved_input=acts[l + 1], y_planes=un)
+            UP.append(un)
+        g_bar = None
+        if need[0]:
+            o, i = Ws[-1].shape
+            tz = torch.empty((P, ((o + 3) // 4) * 4), dtype=torch.float32, device=dev)
+            mlp_layer_planes(UP[-1], ops.weight_planes(Ws[-1]), P, o, i, 0, tz)
+            g_bar = tz[:, :o] * inv_dq
         dW = [None] * n
         if any(need[2 + n:2 + 2 * n]):
-            dW1, _ = mlp_bwd_weight(list(G), U, [w.shape[0] for w in Wd], [w.shape[1] for w in Wd], None, dyn, want_bias=False)
-            dW = [w * inv_dq for w in dW1]
+            dW = [ops.mlp_wgrad_planes((GPl[2 * l], GPl[2 * l + 1]), UP[l], P, Ws[l].shape[0], Ws[l].shape[1], 1.0, dyn) * inv_dq
+                  for l in range(n)]
         return (g_bar, None, *([None] * n), *dW)

@@ -5,7 +5,8 @@ launches, ragged shapes, the operand planes they emit and their output bounds:
     recmv_mlp_wgrad_planes   gemm3_wgrad_kernel + the split-order reductions, and recmv_colsum (WG_SHAPES x WG_SIZES)
     split_planes (plain and transposed), pe_forward_planes, softplus_tangent_planes, add_split_planes, and the fp16 range
     report of the four kernels that split (tags 3500, 3600, 3700, 3710)
-    the SDF, translator and colour training steps and the eikonal term, end to end at multi-wave sizes
+    the SDF, translator and colour training steps, the ReLU networks' create_graph input gradient and the eikonal term,
+    end to end at multi-wave sizes
 
 gemm3_tma_kernel is persistent with a grid of min(tiles, SMs): CTA b walks tiles b, b + S, ... and carries the ring stage
 and parities, the accumulator, the TMA warp's run-ahead into the next tile and the epilogue's tile coordinates from one
@@ -50,6 +51,7 @@ OK, E_DTYPE, E_SHAPE, E_UNSUPPORTED, E_DEVICE = 0, -2, -3, -5, -6
 #   softplus_tangent             u 6.7e-8, inj 1.0e-7
 #   SDF step                     6.6e-6 (sdf, feat, dx, dW, db at 3wave+r and 131 072 points)
 #   translator / colour step     3.6e-6 given our ReLU masks (output, dX0, dW, db); 5 and 7 mask flips, all at |z| < 5e-6
+#   their create_graph dX0       5.6e-6 given our ReLU masks (the backward's g_out and dW)
 #   eikonal                      loss 3.4e-6, gradient / dx / parameter gradients 1.1e-5
 # test_gpu_train.py's 1.5e-6 single-layer bar was measured with cotangents of one scale at M >= 129.  The cotangents
 # here have a per-row log-normal scale and the outputs are as narrow as 39 columns or one row, so the largest |b| is a
@@ -177,6 +179,9 @@ LAYERS = [
     Layer("tangent", 4, 512, 512, bias=False, signed=True),
     # geometric-init output layer: every product positive, the accumulation's truncation bias does not average out
     Layer("same-sign", 4, 512, 257, split=1, y2=True, positive=True),
+    # the ReLU networks' tangent pass (second_order.PlainMlpInputGradFunction): backward-data modes on the [out][in] weight
+    # planes, so K and N are those of the forward layer
+    Layer("tr.tan0", 2, 167, 512), Layer("rgb.tan0", 2, 289, 512), Layer("tr.tan4", 0, 512, 3),
 ]
 BY_NAME = {l.name: l for l in LAYERS}
 LAYER_SIZES = ["1", "127", "129", "wave", "wave+1", "3wave+r"]
@@ -686,10 +691,8 @@ def test_sdf_forward_multi_wave_equals_single_wave_launches():
 PLAIN_NETS = {"translator": (167, 3), "colour": (289, 3)}
 
 
-@pytest.mark.parametrize("net", list(PLAIN_NETS))
-def test_relu_mlp_training_step_matches_fp64_given_our_masks(net):
-    """Translator (167 -> 512 x4 -> 3) and colour (289 -> 512 x4 -> 3) networks on the plane GEMMs, through the forward and
-    backward the training Functions run (ops._plain_mlp_forward / _plain_mlp_backward)."""
+def _plain_net(net):
+    """A ReLU network (d_in -> 512 x4 -> d_out) at 3wave+r rows: (Ws, bs, X0 [P, d_in padded to 8], output cotangent)."""
     d_in, d_out = PLAIN_NETS[net]
     P = _rows("3wave+r", 512)
     _assert_waves("3wave+r", P, 512)
@@ -700,12 +703,12 @@ def test_relu_mlp_training_step_matches_fp64_given_our_masks(net):
     X0 = torch.zeros((P, _pad8(d_in)), device=DEV)
     X0[:, :d_in] = torch.randn((P, d_in), generator=g, device=DEV) * 0.5
     cot = torch.randn((P, d_out), generator=g, device=DEV) / P
-    out, acts, xplanes = ops._plain_mlp_forward(X0, Ws, bs)
-    dX0, dW, db = ops._plain_mlp_backward(cot.contiguous(), Ws, acts, True, True, xplanes)
-    # float64 with OUR ReLU masks; the masks may differ from float64's only where |z| is at fp32 rounding level
-    Xd = X0[:, :d_in].double().requires_grad_(True)
-    Wd = [w.double().requires_grad_(True) for w in Ws]
-    bd = [b.double().requires_grad_(True) for b in bs]
+    return Ws, bs, X0, cot
+
+
+def _plain_f64_given_our_masks(Xd, Wd, bd, acts):
+    """The network in float64 with OUR ReLU masks (acts[l + 1] > 0) -> (output, mask flips against float64's own masks,
+    flips at |z| > 5e-6).  The masks may differ from float64's only where |z| is at fp32 rounding level."""
     h, flips, amb = Xd, 0, 0
     for l in range(5):
         z = torch.nn.functional.linear(h, Wd[l], bd[l])
@@ -717,12 +720,57 @@ def test_relu_mlp_training_step_matches_fp64_given_our_masks(net):
             h = z * ours.double()
         else:
             h = z
+    return h, flips, amb
+
+
+@pytest.mark.parametrize("net", list(PLAIN_NETS))
+def test_relu_mlp_training_step_matches_fp64_given_our_masks(net):
+    """Translator (167 -> 512 x4 -> 3) and colour (289 -> 512 x4 -> 3) networks on the plane GEMMs, through the forward and
+    backward the training Functions run (ops._plain_mlp_forward / _plain_mlp_backward)."""
+    d_in = PLAIN_NETS[net][0]
+    Ws, bs, X0, cot = _plain_net(net)
+    P = X0.shape[0]
+    out, acts, xplanes = ops._plain_mlp_forward(X0, Ws, bs)
+    dX0, dW, db = ops._plain_mlp_backward(cot.contiguous(), Ws, acts, True, True, xplanes)
+    Xd = X0[:, :d_in].double().requires_grad_(True)
+    Wd = [w.double().requires_grad_(True) for w in Ws]
+    bd = [b.double().requires_grad_(True) for b in bs]
+    h, flips, amb = _plain_f64_given_our_masks(Xd, Wd, bd, acts)
     assert amb == 0, (flips, amb)
     (h * cot.double()).sum().backward()
     errs = {"out": merr(out, h), "dX0": merr(dX0[:, :d_in], Xd.grad)}
     errs.update({f"W{l}": merr(dW[l], Wd[l].grad) for l in range(5)})
     errs.update({f"b{l}": merr(db[l], bd[l].grad) for l in range(5)})
     print(f"{net} step P={P}: {flips} mask flips (all at |z| < 5e-6); " + ", ".join(f"{k} {v:.1e}" for k, v in errs.items()))
+    assert max(errs.values()) < PLAIN_STEP_BOUND, errs
+
+
+@pytest.mark.parametrize("net", list(PLAIN_NETS))
+def test_relu_mlp_create_graph_input_grad_matches_fp64_given_our_masks(net):
+    """second_order.PlainMlpInputGradFunction, the create_graph input gradient of the translator and colour networks: its
+    forward is the first-order chain's dX0 bit for bit, and with the ReLU masks of the saved activations dX0 is linear in
+    g_out and in each weight, so the gradients its backward returns must match float64 double autograd under those masks."""
+    from recmv_b200 import second_order
+    d_in = PLAIN_NETS[net][0]
+    Ws, bs, X0, cot = _plain_net(net)
+    P = X0.shape[0]
+    _, acts, xplanes = ops._plain_mlp_forward(X0, Ws, bs)
+    first, _, _ = ops._plain_mlp_backward(cot.contiguous(), Ws, acts, False, True, xplanes)
+    q = _cotangents((P, d_in), _gen(d_in + 1), 1.0)
+    cot_t = cot.clone().requires_grad_(True)
+    Wl = [w.clone().requires_grad_(True) for w in Ws]
+    dX0 = second_order.PlainMlpInputGradFunction.apply(cot_t, 5, *acts, *Wl)
+    assert _equal_bits(dX0, first[:, :d_in])
+    (dX0 * q).sum().backward()
+    Xd = X0[:, :d_in].double().requires_grad_(True)
+    Wd = [w.double().requires_grad_(True) for w in Ws]
+    cd = cot.double().requires_grad_(True)
+    h, _, _ = _plain_f64_given_our_masks(Xd, Wd, [b.double() for b in bs], acts)
+    (dX64,) = torch.autograd.grad(h, Xd, cd, create_graph=True)
+    (dX64 * q.double()).sum().backward()
+    errs = {"dX0": merr(dX0, dX64), "g_out": merr(cot_t.grad, cd.grad)}
+    errs.update({f"W{l}": merr(Wl[l].grad, Wd[l].grad) for l in range(5)})
+    print(f"{net} create_graph input gradient P={P}: " + ", ".join(f"{k} {v:.1e}" for k, v in errs.items()))
     assert max(errs.values()) < PLAIN_STEP_BOUND, errs
 
 
