@@ -27,10 +27,11 @@ __device__ __forceinline__ Cell<T> make_cell(T gx, T gy, T gz, int D, int H, int
   T iy = clip_grad<T>(unnormalize(gy, H), H, &c.my);
   T iz = clip_grad<T>(unnormalize(gz, D), D, &c.mz);
   // NaN: clip_grad's comparisons are false for NaN -> passes through; the reference's max/min clip
-  // maps NaN to 0 in forward; keep that (mult = 1 is irrelevant for a NaN input).
-  if (!(ix == ix)) ix = (T)0;
-  if (!(iy == iy)) iy = (T)0;
-  if (!(iz == iz)) iz = (T)0;
+  // maps NaN to 0 in forward; keep that, and give the NaN axis no gradient (mult = 0), as the fused
+  // skinning kernels do (common.cuh skin_cell), so both LBSkinner paths agree on such a point.
+  if (!(ix == ix)) { ix = (T)0; c.mx = (T)0; }
+  if (!(iy == iy)) { iy = (T)0; c.my = (T)0; }
+  if (!(iz == iz)) { iz = (T)0; c.mz = (T)0; }
   int x0 = (int)floor(ix), y0 = (int)floor(iy), z0 = (int)floor(iz);
   c.x[0] = x0; c.x[1] = x0 + 1; c.y[0] = y0; c.y[1] = y0 + 1; c.z[0] = z0; c.z[1] = z0 + 1;
 #pragma unroll

@@ -103,6 +103,17 @@ def _gs_dims(inp, grid, layout):
     return N, C, D, H, W, P
 
 
+def _check_operand(t, like, shape, name):
+    """t must sit on like's device with like's dtype and the given shape: the kernels read it with like's element type
+    and extent, so anything else would be read as garbage."""
+    if t.device != like.device:
+        raise RuntimeError(f"{name} must be on {like.device}, got {t.device}")
+    if t.dtype != like.dtype:
+        raise RuntimeError(f"{name} must be {like.dtype}, got {t.dtype}")
+    if tuple(t.shape) != tuple(shape):
+        raise RuntimeError(f"{name} must have shape {tuple(shape)}, got {tuple(t.shape)}")
+
+
 def grid_sample3d_forward(inp, grid, layout=LAYOUT_NCDHW):
     """GridSamplerMine.forward(input, grid, 0, 1)  (MCAcc/cuda/GridSamplerMine.cpp:75-81)."""
     _check_input(inp, "input")
@@ -122,9 +133,10 @@ def grid_sample3d_backward(inp, grid, grad_out, layout=LAYOUT_NCDHW, need_grad_i
     """GridSamplerMine.backward(input, grid, grad_output, 0, 1) -> (grad_input, grad_grid)."""
     _check_input(inp, "input")
     _check_input(grid, "grid")
-    grad_out = grad_out.contiguous()
     code = _dtype_code(inp, "input")
     N, C, D, H, W, P = _gs_dims(inp, grid, layout)
+    _check_operand(grad_out, inp, (N, C) + tuple(grid.shape[1:4]), "grad_output")
+    grad_out = grad_out.contiguous()
     gi = torch.zeros_like(inp) if need_grad_input else None
     gg = torch.empty_like(grid)
     with torch.cuda.device(inp.device):
@@ -139,13 +151,16 @@ def grid_sample3d_dbackward(gg_input, gg_grid, inp, grid, grad_out, layout=LAYOU
     """GridSamplerMine.dbackward(ggI, ggG, input, grid, grad_output, 0, 1) -> (gI, gG, ggO)."""
     _check_input(inp, "input")
     _check_input(grid, "grid")
+    code = _dtype_code(inp, "input")
+    N, C, D, H, W, P = _gs_dims(inp, grid, layout)
+    _check_operand(grad_out, inp, (N, C) + tuple(grid.shape[1:4]), "grad_output")
+    _check_operand(gg_grid, grid, grid.shape, "gg_grid")
     grad_out = grad_out.contiguous()
     gg_grid = gg_grid.contiguous()
     if gg_input is not None:
+        _check_operand(gg_input, inp, inp.shape, "gg_input")
         gg_input = gg_input.contiguous()
-    code = _dtype_code(inp, "input")
-    N, C, D, H, W, P = _gs_dims(inp, grid, layout)
-    gi = torch.zeros_like(inp) if need_grad_input else None
+    gi =torch.zeros_like(inp) if need_grad_input else None
     gg = torch.empty_like(grid)
     ggo = torch.empty_like(grad_out)
     with torch.cuda.device(inp.device):
@@ -234,8 +249,11 @@ class _FrozenVoxelSampleBackward(torch.autograd.Function):
 def voxel_to_channels_last(ws):
     """[1,C,D,H,W] fp32 -> [D,H,W,C] (private, coalesced copy of LBSkinner.ws)."""
     _check_input(ws, "ws")
+    if ws.dtype != torch.float32 or ws.dim() != 5 or ws.size(0) != 1:
+        raise RuntimeError(f"voxel_to_channels_last expects a float32 [1,C,D,H,W] voxel, got {ws.dtype} "
+                           f"{tuple(ws.shape)}")
     _, C, D, H, W = ws.shape
-    out = torch.empty((D, H, W, C), dtype=torch.float32, device=ws.device)
+    out =torch.empty((D, H, W, C), dtype=torch.float32, device=ws.device)
     with torch.cuda.device(ws.device):
         check(_lib.load().recmv_voxel_to_channels_last(_ptr(ws), _ptr(out), C, D, H, W, _stream(ws)),
               "recmv_voxel_to_channels_last")
@@ -1396,6 +1414,13 @@ def fragment_decode(pix_to_face, bary, verts, faces, mask=None, camera=None):
     verts = verts.detach().contiguous().float()
     faces = faces.contiguous().long()
     npix = N * H * W
+    for t, name in ((bary, "bary"), (verts, "verts"), (faces, "faces"), (mask, "mask")):
+        if t is not None and t.device != dev:
+            raise RuntimeError(f"fragment_decode: {name} must be on {dev}, got {t.device}")
+    if tuple(bary.shape) != (N, H, W, K, 3):
+        raise RuntimeError(f"fragment_decode: bary must have shape {(N, H, W, K, 3)}, got {tuple(bary.shape)}")
+    if mask is not None and mask.numel() != npix:
+        raise RuntimeError(f"fragment_decode: mask must have {npix} elements (N*H*W), got {mask.numel()}")
     lib = _lib.load()
     scratch = torch.empty((lib.recmv_fragment_decode_scratch_bytes(npix),), dtype=torch.uint8, device=dev)
     ob, orow, ocol, ofi = (torch.empty((npix,), dtype=torch.int64, device=dev) for _ in range(4))
