@@ -369,6 +369,24 @@ RECMV_API int recmv_fragment_decode(const int64_t* pix_to_face, const float* bar
                           int64_t* out_col, float* out_pts, int64_t* out_finds, float* out_rays, int32_t* counters,
                           recmv_stream_t stream);
 
+/* ---- mesh rasterizer: the fragments recmv_fragment_decode reads ---------------------------------------------------
+ * replaces the pytorch3d MeshRasterizer of `maskRender` (model/network.py:307-322; faces_per_pixel 1, blur 0,
+ * perspective-correct, unclipped barycentrics, no culling of back faces).  verts [N,V,3] f32, faces [F,3] int64 shared by
+ * the N frames, camera = DEVICE float[N][16] {fx, fy, px, py, R[9] row-major, T[3]}: view X R + T, screen
+ * (px - fx X/Z, py - fy Y/Z), pixel (row, col) centred at (col, row).  A face is skipped when a vertex has Z <= z_clip or
+ * its doubled screen area |A| <= area_eps; it covers a pixel whose three barycentrics are >= 0; the smallest
+ * perspective-correct zbuf wins, ties to the lower packed index n*F + f (deterministic).  Outputs in the Fragments layout
+ * with K = 1: out_pix_to_face [N,H,W] int64 (packed), out_zbuf [N,H,W], out_bary [N,H,W,3] (perspective-corrected),
+ * out_dists [N,H,W] (NULL = not computed: signed squared NDC distance to the nearest edge); background = -1 in all.
+ * workspace: recmv_raster_workspace_bytes(N, F, H, W, capacity); capacity = (tile, face) pair-list entries.
+ * counters (DEVICE int32[4]) <- {covered pixels, skipped faces, pairs, overflow}.  No host synchronisation: when
+ * pairs > capacity, overflow = 1 and NO output is written -- re-run with capacity >= pairs.                           */
+RECMV_API int recmv_raster_workspace_bytes(int N, int64_t F, int H, int W, int64_t capacity, size_t* bytes);
+RECMV_API int recmv_rasterize_meshes(const float* verts, int V, const int64_t* faces, int64_t F, int N,
+                          const float* camera /*device[N][16]*/, int H, int W, float z_clip, float area_eps,
+                          void* workspace, int64_t capacity, int64_t* out_pix_to_face, float* out_zbuf, float* out_bary,
+                          float* out_dists, int32_t* counters /*device*/, recmv_stream_t stream);
+
 /* ---- A11 / (f2): the sweep of one pyramid level as a DEVICE WORKLIST (SURVEY 8b `recmv_c2f_sweep`) -----------------
  * replaces the coordinate-list bookkeeping of MCAcc/seg3d_lossless.py:306-428 (nonzero / unique / index scatter, a
  * host sync per step).  level / final_res are (W, H, D) = (x, y, z) lattice sizes (host).

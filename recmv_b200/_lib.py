@@ -118,7 +118,10 @@ SIGNATURES = {
     "recmv_fragment_decode": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int64, c_void_p,
                                       POINTER(c_float), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                       c_void_p, c_void_p]),
-    "recmv_c2f_done_up": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "recmv_raster_workspace_bytes": (c_int, [c_int, c_int64, c_int, c_int, c_int64, POINTER(c_size_t)]),
+    "recmv_rasterize_meshes": (c_int, [c_void_p, c_int, c_void_p, c_int64, c_int, c_void_p, c_int, c_int, c_float, c_float,
+                                       c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "recmv_c2f_done_up":(c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     "recmv_c2f_compact": (c_int, [c_void_p, POINTER(c_int), POINTER(c_int), POINTER(c_float), POINTER(c_float), c_void_p,
                                   c_void_p, c_void_p, c_int, c_void_p]),
     "recmv_c2f_scatter": (c_int, [c_void_p, c_void_p, c_void_p, c_int, POINTER(c_int), POINTER(c_int), c_void_p, c_void_p,

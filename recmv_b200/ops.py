@@ -1442,6 +1442,73 @@ def fragment_decode(pix_to_face, bary, verts, faces, mask=None, camera=None):
     return out + (orays[:n],) if camera is not None else out
 
 
+_raster_state = {}   # per device: grow-only workspace (its pair-list capacity) + counters and their pinned host copy
+
+
+def rasterize_meshes(verts, faces, cameras, H, W, z_clip=1e-6, area_eps=1e-8, want_dists=True, capacity=None,
+                     host_camera=False):
+    """Single-layer mesh rasterizer (recmv_rasterize_meshes).  verts [N,V,3] f32, faces [F,3] int64, cameras [N,16] f32
+    {fx, fy, px, py, R row-major, T}, all CUDA and contiguous.  Returns (pix_to_face [N,H,W,1] int64, zbuf [N,H,W,1],
+    bary [N,H,W,1,3], dists [N,H,W,1] or None, counts) with counts = {covered, skipped, pairs} as host ints.
+
+    One host read per call: the counters after the launch.  The (tile, face) pair list lives in a grow-only per-device
+    workspace; only when it overflowed is the call re-run, once, with a list of the reported size.  `capacity` sets the
+    list size of the first attempt (the retained one when None).  host_camera=True adds cameras[0] as 16 host floats to
+    the same read (what the fragment decode's view rays need)."""
+    for t, name in ((verts, "verts"), (faces, "faces"), (cameras, "cameras")):
+        _check_input(t, name)
+    dev = verts.device
+    if faces.device != dev or cameras.device != dev:
+        raise RuntimeError(f"rasterize_meshes: faces and cameras must be on {dev}")
+    if verts.dtype != torch.float32 or verts.dim() != 3 or verts.shape[2] != 3:
+        raise RuntimeError(f"rasterize_meshes: verts must be float32 [N,V,3], got {verts.dtype} {tuple(verts.shape)}")
+    if faces.dtype != torch.int64 or faces.dim() != 2 or faces.shape[1] != 3:
+        raise RuntimeError(f"rasterize_meshes: faces must be int64 [F,3], got {faces.dtype} {tuple(faces.shape)}")
+    N, V = int(verts.shape[0]), int(verts.shape[1])
+    F = int(faces.shape[0])
+    if cameras.dtype != torch.float32 or tuple(cameras.shape) != (N, 16):
+        raise RuntimeError(f"rasterize_meshes: cameras must be float32 [{N},16], got {cameras.dtype} {tuple(cameras.shape)}")
+    H, W = int(H), int(W)
+    lib = _lib.load()
+    st = _raster_state.setdefault(dev.index, {})
+    if st.get("counters") is None:
+        st["counters"] = torch.zeros((20,), dtype=torch.int32, device=dev)       # 4 counters + 16 camera floats
+        st["counters_host"] = torch.zeros((20,), dtype=torch.int32).pin_memory()
+    cap = int(capacity) if capacity is not None else max(st.get("capacity", 0), 2 * N * F + 4096)
+    p2f = torch.empty((N, H, W, 1), dtype=torch.int64, device=dev)
+    zbuf = torch.empty((N, H, W, 1), dtype=torch.float32, device=dev)
+    bary = torch.empty((N, H, W, 1, 3), dtype=torch.float32, device=dev)
+    dists = torch.empty((N, H, W, 1), dtype=torch.float32, device=dev) if want_dists else None
+    ctr = st["counters"]
+    with torch.cuda.device(dev):
+        stream = _stream(verts)
+        for _ in range(2):
+            nbytes = c_size_t(0)
+            check(lib.recmv_raster_workspace_bytes(N, F, H, W, cap, byref(nbytes)), "recmv_raster_workspace_bytes")
+            if st.get("ws") is None or st["ws"].numel() < nbytes.value:
+                st["ws"] = torch.empty((nbytes.value,), dtype=torch.uint8, device=dev)
+            st["capacity"] = max(st.get("capacity", 0), cap)
+            check(lib.recmv_rasterize_meshes(_ptr(verts), V, _ptr(faces), F, N, _ptr(cameras), H, W, float(z_clip),
+                                             float(area_eps), _ptr(st["ws"]), cap, _ptr(p2f), _ptr(zbuf), _ptr(bary),
+                                             _ptr(dists), _ptr(ctr), stream), "recmv_rasterize_meshes")
+            if host_camera and N > 0:
+                ctr[4:].copy_(cameras[0].view(torch.int32))
+            st["counters_host"].copy_(ctr, non_blocking=True)
+            torch.cuda.current_stream(dev).synchronize()
+            covered, skipped, pairs, overflow = (int(v) for v in st["counters_host"][:4])
+            if not overflow:
+                break
+            if pairs >= 0x7fffffff:
+                check(_lib.RECMV_E_RANGE, "recmv_rasterize_meshes (more than 2^31 - 1 tile / face pairs)")
+            cap = pairs   # grow once to the exact size, re-run (the workspace is kept for later calls)
+        else:
+            raise _lib.RecmvError("recmv_rasterize_meshes: pair list still too small after growing")
+    counts = {"covered": covered, "skipped": skipped, "pairs": pairs}
+    if host_camera:
+        counts["camera"] = st["counters_host"][4:].view(torch.float32).clone()
+    return p2f, zbuf, bary, dists, counts
+
+
 class C2fLevel:
     """Device worklist of one pyramid level (recmv_c2f_refine / recmv_sdf_mlp_fwd_counted / recmv_c2f_scatter_list /
     recmv_c2f_mark_conflicts): one fused full-grid pass builds the level and its worklist, conflict rounds are driven by

@@ -46,6 +46,24 @@ def FindSurfacePsRays(TmpVs, TmpFaces, frags, camera, gt_masks=None):
     return ops.fragment_decode(frags.pix_to_face, frags.bary_coords, TmpVs, TmpFaces, gt_masks, camera)
 
 
+def FindSurfacePsMesh(TmpVs, TmpFaces, defVs, cameras, H, W, gt_masks=None):
+    """Rasterize the deformed meshes defVs [N,V,3] (faces TmpFaces, one camera per frame, recmv_b200.raster) and decode
+    the fragments against the canonical mesh TmpVs with camera 0's view rays and the mask filter (FindSurfacePsRays):
+    what `find_surface_ps` + `sample_train_ray` compute with `maskRender` (OptimGarmentNetwork.py:742-783, 1006-1050).
+    cameras: reference-camera attributes or (focal_length, principal_point, R, T).  Host reads: the rasterizer's counters
+    (which carry camera 0 to the host) and the decode's row count.  Returns (batch, row, col, init points, face ids,
+    rays)."""
+    from .. import ops
+    from ..raster import camera_rows
+    if not defVs.is_cuda:
+        raise RuntimeError("FindSurfacePsMesh runs on CUDA tensors only (no CPU path)")
+    cam = camera_rows(cameras, int(defVs.shape[0]), defVs.device)
+    p2f, _, bary, _, counts = ops.rasterize_meshes(defVs.detach().float().contiguous(), TmpFaces.long().contiguous(), cam,
+                                                   H, W, want_dists=False, host_camera=True)
+    c = counts["camera"]
+    return ops.fragment_decode(p2f, bary, TmpVs, TmpFaces, gt_masks, (c[0], c[1], c[2], c[3], c[4:13].view(3, 3)))
+
+
 # The three Optimize* entry points run the whole loop on the device (one C call) when both networks are on the
 # tensor-core engine; set False to force the step-by-step torch loop (`_solve`, which also serves CPU tensors, the
 # fp32 SIMT mode and deformers other than [MLPTranslator, LBSkinner]).

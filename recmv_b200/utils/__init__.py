@@ -6,7 +6,7 @@ from .. import ops as _ops
 from ..model.Embedder import annealing_weights  # noqa: F401  (utils/utils.py:40-46)
 from ..ops import FastDiff3x3MinvFunction  # noqa: F401    (utils/utils.py:8-18)
 from . import FindSurfacePs as _fsp
-from .FindSurfacePs import (FindSurfacePs, FindSurfacePsRays, OptimizeGarmentSurfacePs, OptimizeGarmentSurfaceSinlge,  # noqa: F401
+from .FindSurfacePs import (FindSurfacePs, FindSurfacePsMesh, FindSurfacePsRays, OptimizeGarmentSurfacePs, OptimizeGarmentSurfaceSinlge,  # noqa: F401
                             OptimizeSurfacePs)
 
 
