@@ -2,10 +2,11 @@
  *
  * Every entry point takes raw DEVICE pointers (unless a parameter says "host"), plain sizes and a
  * cudaStream_t passed as void*.  No torch types.  Return value: 0 = ok, negative = argument error
- * (RECMV_E_*), positive = cudaError_t raised by the launch.  Nothing here allocates result storage
- * of data-dependent size: marching cubes is a count call followed by an emit call.  All kernels run
- * on the caller's stream and never synchronise the device, except recmv_mc_count (it has to return
- * two integers to the host, like the reference's blocking cudaMemcpy at MCGpu/CudaKernels.cu:628).
+ * (RECMV_E_*), positive = cudaError_t raised by the launch.  All kernels run on the caller's stream
+ * and no entry point waits for the work it queued (marching cubes copies its case tables to the
+ * device once, on its first call per device).  Nothing here allocates result storage:
+ * results of data-dependent size go into caller buffers of a given capacity, and the counts and an
+ * overflow flag are written to device memory (re-run with larger buffers when the flag is set).
  *
  * Each block cites the reference interface (path:line under /root/reference) it replaces.
  */
@@ -113,18 +114,14 @@ RECMV_API int recmv_lbsw_smooth(float* buf_a, float* buf_b, int D, int H, int W,
  * Deterministic: vertices and faces come out in the order a sequential sweep of the reference
  * kernel (cell index ascending) would create them; faces int64 with the reference's reversed
  * winding; vertices referenced on the far boundary planes get index -1 exactly as the reference.
- * count: fills host V,F (blocks on the stream).  emit: must follow count on the same stream with
- * the same sdf/iso/scratch; writes verts [V,3] = v*step+origin and faces [F,3].                 */
+ * recmv_mc_run is one call with NO host synchronisation (the reference blocks on a cudaMemcpy
+ * between its two kernels, MCGpu/CudaKernels.cu:628): classify + count + scan + emit of
+ * verts [V,3] = v*step+origin and faces [F,3] into caller-provided buffers of capacity cap_verts /
+ * cap_faces rows, with scratch of recmv_mc_scratch_bytes.  counts (DEVICE, int32[4]) receives
+ * {V, F, overflow, 0}; overflow != 0 = a buffer was too small: rows that fit are valid, re-run with
+ * V / F rows.  Rows beyond V / F are left untouched.  V >= 2^25 exceeds the packed vertex ids:
+ * overflow is then set whatever the capacity.                                                    */
 RECMV_API int recmv_mc_scratch_bytes(int NX, int NY, int NZ, size_t* bytes /*host*/);
-RECMV_API int recmv_mc_count(const float* sdf, int NX, int NY, int NZ, float iso, void* scratch,
-                   int64_t* num_verts /*host*/, int64_t* num_faces /*host*/, recmv_stream_t stream);
-RECMV_API int recmv_mc_emit(const float* sdf, int NX, int NY, int NZ, float iso, void* scratch,
-                  const float step[3] /*host*/, const float origin[3] /*host*/, float* verts,
-                  int64_t* faces, recmv_stream_t stream);
-/* One call, NO host synchronisation (the reference blocks on a cudaMemcpy between its two kernels,
- * MCGpu/CudaKernels.cu:628): classify + count + scan + emit into caller-provided buffers of capacity cap_verts /
- * cap_faces rows.  counts (DEVICE, int32[4]) receives {V, F, overflow, 0}; overflow != 0 = a buffer was too small
- * (re-run with V / F rows).  Rows beyond V / F are left untouched.                                              */
 RECMV_API int recmv_mc_run(const float* sdf, int NX, int NY, int NZ, float iso, void* scratch,
                  const float step[3] /*host*/, const float origin[3] /*host*/, float* verts, int64_t cap_verts,
                  int64_t* faces, int64_t cap_faces, int32_t* counts /*device*/, recmv_stream_t stream);
@@ -221,7 +218,7 @@ RECMV_API int recmv_sdf_pack_weights(const float* W_all, const float* b_all, voi
 RECMV_API int recmv_sdf_mlp_fwd(const float* x, const void* packed, const float* pe_w /*host*/,
                       float* out_sdf, float* out_feat, int64_t P, int mode, recmv_stream_t stream);
 /* the same with the point count read from DEVICE memory: *count_dev points (clamped to `capacity`, for which the launch
- * is sized) -- consumer of device-built worklists (recmv_c2f_compact).  TC modes only.                             */
+ * is sized) -- consumer of device-built worklists (recmv_c2f_refine, recmv_c2f_mark_conflicts).  TC modes only.  */
 RECMV_API int recmv_sdf_mlp_fwd_counted(const float* x, const void* packed, const float* pe_w /*host*/, float* out_sdf,
                               float* out_feat, int64_t capacity, const int* count_dev, int mode,
                               recmv_stream_t stream);
@@ -389,35 +386,22 @@ RECMV_API int recmv_rasterize_meshes(const float* verts, int V, const int64_t* f
 
 /* ---- A11 / (f2): the sweep of one pyramid level as a DEVICE WORKLIST (SURVEY 8b `recmv_c2f_sweep`) -----------------
  * replaces the coordinate-list bookkeeping of MCAcc/seg3d_lossless.py:306-428 (nonzero / unique / index scatter, a
- * host sync per step).  level / final_res are (W, H, D) = (x, y, z) lattice sizes (host).
- *  recmv_c2f_done_up      : done_up[2z,2y,2x] = done[z,y,x], 0 elsewhere.
- *  recmv_c2f_compact      : voxels with todo != 0 -> idx_out[i] (flat level index), points_out[i] = the query point of
- *                           batch_eval (:89-100), bit-identical arithmetic; counters (device int32[2] = {count, overflow},
- *                           zeroed by the caller) is advanced with one atomic per warp; order is unspecified.
+ * host sync per step).  level / final_res are (W, H, D) = (x, y, z) lattice sizes (host).  A worklist is idx_out[i]
+ * (flat level index) and points_out[i] (the query point of batch_eval, :89-100, bit-identical arithmetic), in no
+ * particular order; counters (device int32[2] = {count, overflow}, zeroed by the caller) is advanced atomically and
+ * overflow is set when more than `capacity` voxels are appended.
+ *  recmv_c2f_refine       : coarse level (D,H,W) -> fine level (2D-1,2H-1,2W-1) in one full-grid pass: upsampled values
+ *                           (order as recmv_interp2x_boundary3d_fwd), the level's done lattice (done_fine[2z,2y,2x] =
+ *                           done_coarse[z,y,x], 0 elsewhere), and the worklist of the voxels to query: not done and in
+ *                           the 3x3x3 dilation of the mixed-stencil flags, evaluated exactly from a coarse "mixed cell"
+ *                           mask (mixed_scratch, (D-1)(H-1)(W-1) bytes).
  *  recmv_sdf_mlp_fwd_counted (above): evaluates points_out[0 .. *counters) without the host knowing the count.
- *  recmv_c2f_scatter      : occ[idx] = vals, done[idx] = 1, calculated[final-lattice position] = 1; a sign flip against
- *                           the interpolated value sets conflict_flag[idx] (caller zeroes it); stats (device int32[2])
- *                           += {queried, conflicts}.
- *  recmv_c2f_conflict_todo: todo = dilate3x3x3(conflict_flag) & ~calculated[z*sz, y*sy, x*sx]  (:392-420).          */
-RECMV_API int recmv_c2f_done_up(const uint8_t* done, int D, int H, int W, uint8_t* done_up, recmv_stream_t stream);
-RECMV_API int recmv_c2f_compact(const uint8_t* todo, const int level[3] /*host*/, const int final_res[3] /*host*/,
-                      const float b_min[3] /*host*/, const float b_max[3] /*host*/, int32_t* idx_out, float* points_out,
-                      int32_t* counters, int capacity, recmv_stream_t stream);
-RECMV_API int recmv_c2f_scatter(const int32_t* idx, const float* vals, const int32_t* counters, int capacity,
-                      const int level[3] /*host*/, const int final_res[3] /*host*/, float* occ, uint8_t* done,
-                      uint8_t* calculated, uint8_t* conflict_flag, float balance_value, int32_t* stats,
-                      recmv_stream_t stream);
-RECMV_API int recmv_c2f_conflict_todo(const uint8_t* conflict_flag, const uint8_t* calculated, const int level[3] /*host*/,
-                            const int final_res[3] /*host*/, uint8_t* todo, recmv_stream_t stream);
-/* The fused form Seg3dLossless._forward_device uses -- ONE full-grid pass per level instead of four:
- *  recmv_c2f_refine       : coarse level (D,H,W) -> fine level (2D-1,2H-1,2W-1): upsampled values (order as
- *                           recmv_interp2x_boundary3d_fwd), the level's done lattice, and the voxels to query appended to
- *                           (idx_out, points_out).  The 3x3x3 dilation of the mixed-stencil flags is evaluated exactly
- *                           from a coarse "mixed cell" mask (mixed_scratch, (D-1)(H-1)(W-1) bytes).
- *  recmv_c2f_scatter_list : as recmv_c2f_scatter, conflicts appended to conflict_list / conflict_count (zeroed by the
- *                           caller); clears the claim bytes of the consumed voxels.
- *  recmv_c2f_mark_conflicts: next worklist = not-yet-evaluated 3x3x3 neighbours of the conflicting voxels, each claimed
- *                           once through `claim` (level-lattice bytes, 4-byte aligned, all zero between rounds).      */
+ *  recmv_c2f_scatter_list : occ[idx] = vals, done[idx] = 1, calculated[final-lattice position] = 1, claim[idx] = 0; a
+ *                           sign flip against the interpolated value appends idx to conflict_list / conflict_count
+ *                           (device int32, zeroed by the caller); stats[0] (device int32) += queried.
+ *  recmv_c2f_mark_conflicts: next worklist = the 3x3x3 neighbours of the conflicting voxels not yet evaluated at any
+ *                           level (calculated[z*sz, y*sy, x*sx] == 0, :392-420), each claimed once through `claim`
+ *                           (level-lattice bytes, 4-byte aligned, all zero between rounds).                            */
 RECMV_API int recmv_c2f_refine(const float* occ_coarse, const uint8_t* done_coarse, int D, int H, int W,
                      const int final_res[3] /*host*/, const float b_min[3] /*host*/, const float b_max[3] /*host*/,
                      float balance_value, int order, uint8_t* mixed_scratch, float* occ_fine, uint8_t* done_fine,

@@ -54,10 +54,6 @@ SIGNATURES = {
                                      c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "recmv_lbsw_smooth": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p]),
     "recmv_mc_scratch_bytes": (c_int, [c_int, c_int, c_int, POINTER(c_size_t)]),
-    "recmv_mc_count": (c_int, [c_void_p, c_int, c_int, c_int, c_float, c_void_p, POINTER(c_int64),
-                               POINTER(c_int64), c_void_p]),
-    "recmv_mc_emit": (c_int, [c_void_p, c_int, c_int, c_int, c_float, c_void_p, POINTER(c_float),
-                              POINTER(c_float), c_void_p, c_void_p, c_void_p]),
     "recmv_mc_run": (c_int, [c_void_p, c_int, c_int, c_int, c_float, c_void_p, POINTER(c_float), POINTER(c_float), c_void_p,
                              c_int64, c_void_p, c_int64, c_void_p, c_void_p]),
     "recmv_lbs_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int,
@@ -121,12 +117,6 @@ SIGNATURES = {
     "recmv_raster_workspace_bytes": (c_int, [c_int, c_int64, c_int, c_int, c_int64, POINTER(c_size_t)]),
     "recmv_rasterize_meshes": (c_int, [c_void_p, c_int, c_void_p, c_int64, c_int, c_void_p, c_int, c_int, c_float, c_float,
                                        c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
-    "recmv_c2f_done_up":(c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
-    "recmv_c2f_compact": (c_int, [c_void_p, POINTER(c_int), POINTER(c_int), POINTER(c_float), POINTER(c_float), c_void_p,
-                                  c_void_p, c_void_p, c_int, c_void_p]),
-    "recmv_c2f_scatter": (c_int, [c_void_p, c_void_p, c_void_p, c_int, POINTER(c_int), POINTER(c_int), c_void_p, c_void_p,
-                                  c_void_p, c_void_p, c_float, c_void_p, c_void_p]),
-    "recmv_c2f_conflict_todo": (c_int, [c_void_p, c_void_p, POINTER(c_int), POINTER(c_int), c_void_p, c_void_p]),
     "recmv_c2f_refine": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, POINTER(c_int), POINTER(c_float), POINTER(c_float),
                                  c_float, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
     "recmv_c2f_scatter_list": (c_int, [c_void_p, c_void_p, c_void_p, c_int, POINTER(c_int), POINTER(c_int), c_void_p,

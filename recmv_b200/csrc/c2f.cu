@@ -137,10 +137,8 @@ __global__ void __launch_bounds__(256) c2f_todo_kernel(const unsigned char* __re
 }
 
 // ---- device worklist of the sweep (Seg3dLossless._forward, MCAcc/seg3d_lossless.py:306-428) ---------------------------
-// todo mask -> (flat level index, query point) list, appended with one warp-aggregated atomic per warp; the order is
-// irrelevant: the fused SDF kernel evaluates every point independently and results are scattered back by index.
-// Query point exactly as batch_eval (:89-100): c = coords / res + (1 / res) / 2;  p = c * (b_max - b_min) + b_min,
-// every operation rounded separately (no FMA contraction), so the values equal the torch path's bit for bit.
+// Voxels to query -> (flat level index, query point) list; the order is irrelevant: the fused SDF kernel evaluates every
+// point independently and results are scattered back by index.
 struct C2fGeom {
   int D, H, W;          // level lattice
   int sx, sy, sz;       // level step in final-lattice units
@@ -149,89 +147,16 @@ struct C2fGeom {
   float res[3];         // final resolution as float (x, y, z)
   float ext[3], bmin[3];
 };
-__global__ void __launch_bounds__(256) c2f_compact_kernel(const unsigned char* __restrict__ todo, C2fGeom g,
-                                                          int* __restrict__ idx_out, float* __restrict__ pts_out,
-                                                          int* __restrict__ counters /*[0]=count [1]=overflow*/, int cap) {
-  const long long total = (long long)g.D * g.H * g.W;
-  const int lane = threadIdx.x & 31;
-  for (long long i0 = (blockIdx.x * (long long)blockDim.x + threadIdx.x) - lane; i0 < total; i0 += (long long)gridDim.x * blockDim.x) {
-    const long long i = i0 + lane;
-    const bool on = i < total && todo[i] != 0;
-    const unsigned m = __ballot_sync(0xffffffffu, on);
-    if (m == 0u) continue;
-    int base = 0;
-    if (lane == 0) base = atomicAdd(counters, __popc(m));
-    base = __shfl_sync(0xffffffffu, base, 0);
-    if (!on) continue;
-    const int slot = base + __popc(m & ((1u << lane) - 1u));
-    if (slot >= cap) { counters[1] = 1; continue; }
-    const int x = (int)(i % g.W), y = (int)((i / g.W) % g.H), z = (int)(i / ((long long)g.W * g.H));
-    idx_out[slot] = (int)i;
-    const float c[3] = {(float)(x * g.sx), (float)(y * g.sy), (float)(z * g.sz)};
+
+// Query point of level voxel (x, y, z) -> pts[0..3), exactly as batch_eval (:89-100): c = coords / res + (1 / res) / 2;
+// p = c * (b_max - b_min) + b_min, every operation rounded separately (no FMA contraction), so the values equal the torch
+// path's bit for bit.
+__device__ __forceinline__ void c2f_query_point(const C2fGeom& g, int x, int y, int z, float* __restrict__ pts) {
+  const float c[3] = {(float)(x * g.sx), (float)(y * g.sy), (float)(z * g.sz)};
 #pragma unroll
-    for (int a = 0; a < 3; ++a) {
-      const float u = __fadd_rn(__fdiv_rn(c[a], g.res[a]), g.inv_step2[a]);
-      pts_out[3 * (size_t)slot + a] = __fadd_rn(__fmul_rn(u, g.ext[a]), g.bmin[a]);
-    }
-  }
-}
-
-// queried values -> level grid; marks done / calculated; a sign flip against the interpolated value is a conflict
-// (seg3d_lossless.py:372-376): flag it for the next round and count it
-__global__ void __launch_bounds__(256) c2f_scatter_kernel(const int* __restrict__ idx, const float* __restrict__ vals,
-                                                          const int* __restrict__ counters, int cap, C2fGeom g,
-                                                          float* __restrict__ occ, unsigned char* __restrict__ done,
-                                                          unsigned char* __restrict__ calculated,
-                                                          unsigned char* __restrict__ cflag, float balance,
-                                                          int* __restrict__ stats /*[0]+=queried [1]+=conflicts*/) {
-  const int n = min(counters[0], cap);
-  int conflicts = 0;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    const int j = idx[i];
-    const float v = vals[i], it = occ[j];
-    occ[j] = v;
-    done[j] = 1;
-    const int x = j % g.W, y = (j / g.W) % g.H, z = j / (g.W * g.H);
-    calculated[((size_t)(z * g.sz) * g.Hf + (size_t)(y * g.sy)) * g.Wf + (size_t)(x * g.sx)] = 1;
-    if (__fmul_rn(__fsub_rn(it, balance), __fsub_rn(v, balance)) < 0.f) { cflag[j] = 1; ++conflicts; }
-  }
-  conflicts = __reduce_add_sync(0xffffffffu, conflicts);
-  if ((threadIdx.x & 31) == 0 && conflicts) atomicAdd(stats + 1, conflicts);
-  if (blockIdx.x == 0 && threadIdx.x == 0) atomicAdd(stats, n);
-}
-
-// todo = dilate3x3x3(flag) & ~calculated[z*sz, y*sy, x*sx]   (conflict rounds: "not evaluated at ANY level")
-__global__ void __launch_bounds__(256) c2f_todo_strided_kernel(const unsigned char* __restrict__ flag,
-                                                               const unsigned char* __restrict__ calculated, C2fGeom g,
-                                                               unsigned char* __restrict__ todo) {
-  const long long total = (long long)g.D * g.H * g.W;
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-    const int x = (int)(i % g.W), y = (int)((i / g.W) % g.H), z = (int)(i / ((long long)g.W * g.H));
-    unsigned char r = 0;
-    if (!calculated[((size_t)(z * g.sz) * g.Hf + (size_t)(y * g.sy)) * g.Wf + (size_t)(x * g.sx)]) {
-      for (int dz = -1; dz <= 1 && !r; ++dz) {
-        const int zz = z + dz;
-        if (zz < 0 || zz >= g.D) continue;
-        for (int dy = -1; dy <= 1 && !r; ++dy) {
-          const int yy = y + dy;
-          if (yy < 0 || yy >= g.H) continue;
-          const unsigned char* row = flag + ((long long)zz * g.H + yy) * g.W;
-          r = (x > 0 && row[x - 1]) || row[x] || (x < g.W - 1 && row[x + 1]);
-        }
-      }
-    }
-    todo[i] = r;
-  }
-}
-
-// done_up[2z, 2y, 2x] = done[z, y, x], zero elsewhere (the level's "already evaluated" lattice)
-__global__ void __launch_bounds__(256) c2f_done_up_kernel(const unsigned char* __restrict__ done, int D, int H, int W,
-                                                          unsigned char* __restrict__ up) {
-  const int d = 2 * D - 1, h = 2 * H - 1, w = 2 * W - 1;
-  const long long total = (long long)d * h * w;
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-    const int x = (int)(i % w), y = (int)((i / w) % h), z = (int)(i / ((long long)w * h));
-    up[i] = ((x | y | z) & 1) ? 0 : done[((long long)(z >> 1) * H + (y >> 1)) * W + (x >> 1)];
+  for (int a = 0; a < 3; ++a) {
+    const float u = __fadd_rn(__fdiv_rn(c[a], g.res[a]), g.inv_step2[a]);
+    pts[a] = __fadd_rn(__fmul_rn(u, g.ext[a]), g.bmin[a]);
   }
 }
 
@@ -256,8 +181,8 @@ __global__ void __launch_bounds__(256) c2f_cell_mixed_kernel(const float* __rest
   }
 }
 
-// upsample + done lattice + todo decision + worklist append, one pass over the fine level (replaces interp2x + done_up +
-// todo mask + compact: four full-grid passes)
+// upsample + done lattice + todo decision + worklist append (one warp-aggregated atomic per warp), one pass over the
+// fine level
 template <int kOrder>
 __global__ void __launch_bounds__(256) c2f_refine_kernel(const float* __restrict__ occ_c, const unsigned char* __restrict__ done_c,
                                                          const unsigned char* __restrict__ mixed, int D, int H, int W /*coarse*/,
@@ -296,12 +221,7 @@ __global__ void __launch_bounds__(256) c2f_refine_kernel(const float* __restrict
     const int slot = base + __popc(m & ((1u << lane) - 1u));
     if (slot >= cap) { counters[1] = 1; continue; }
     idx_out[slot] = (int)i;
-    const float c[3] = {(float)(x * g.sx), (float)(y * g.sy), (float)(z * g.sz)};
-#pragma unroll
-    for (int a = 0; a < 3; ++a) {
-      const float u = __fadd_rn(__fdiv_rn(c[a], g.res[a]), g.inv_step2[a]);
-      pts_out[3 * (size_t)slot + a] = __fadd_rn(__fmul_rn(u, g.ext[a]), g.bmin[a]);
-    }
+    c2f_query_point(g, x, y, z, pts_out + 3 * (size_t)slot);
   }
 }
 
@@ -324,12 +244,7 @@ __global__ void __launch_bounds__(256) c2f_mark_kernel(const int* __restrict__ c
     const int slot = atomicAdd(counters, 1);
     if (slot >= cap) { counters[1] = 1; continue; }
     idx_out[slot] = (int)i;
-    const float c[3] = {(float)(x * g.sx), (float)(y * g.sy), (float)(z * g.sz)};
-#pragma unroll
-    for (int a = 0; a < 3; ++a) {
-      const float u = __fadd_rn(__fdiv_rn(c[a], g.res[a]), g.inv_step2[a]);
-      pts_out[3 * (size_t)slot + a] = __fadd_rn(__fmul_rn(u, g.ext[a]), g.bmin[a]);
-    }
+    c2f_query_point(g, x, y, z, pts_out + 3 * (size_t)slot);
   }
 }
 
@@ -378,52 +293,6 @@ C2fGeom make_geom(const int level[3], const int final_res[3], const float b_min[
 }  // namespace recmv
 
 using namespace recmv;
-
-// ---- recmv_c2f_*: the sweep of one pyramid level without host round trips (SURVEY 8b `recmv_c2f_sweep`) ---------------
-// level / final_res: (W, H, D) lattice sizes (x, y, z); counters: device int32[2] {count, overflow}, zeroed by the caller
-// before recmv_c2f_compact; stats: device int32[2] {queried, conflicts}, accumulated.
-extern "C" int recmv_c2f_compact(const uint8_t* todo, const int level[3], const int final_res[3], const float b_min[3],
-                                 const float b_max[3], int32_t* idx_out, float* points_out, int32_t* counters,
-                                 int capacity, recmv_stream_t stream) {
-  if (!todo || !level || !final_res || !b_min || !b_max || !idx_out || !points_out || !counters) return RECMV_E_NULL;
-  if (level[0] <= 0 || level[1] <= 0 || level[2] <= 0 || capacity <= 0) return RECMV_E_SHAPE;
-  const C2fGeom g = make_geom(level, final_res, b_min, b_max);
-  const int64_t total = (int64_t)g.D * g.H * g.W;
-  if (total > 2000000000LL) return RECMV_E_RANGE;
-  c2f_compact_kernel<<<stride_grid(total, 256, 8), 256, 0, (cudaStream_t)stream>>>(todo, g, idx_out, points_out, counters, capacity);
-  return launch_status();
-}
-
-extern "C" int recmv_c2f_scatter(const int32_t* idx, const float* vals, const int32_t* counters, int capacity,
-                                 const int level[3], const int final_res[3], float* occ, uint8_t* done,
-                                 uint8_t* calculated, uint8_t* conflict_flag, float balance_value, int32_t* stats,
-                                 recmv_stream_t stream) {
-  if (!idx || !vals || !counters || !level || !final_res || !occ || !done || !calculated || !conflict_flag || !stats)
-    return RECMV_E_NULL;
-  if (capacity <= 0) return RECMV_E_SHAPE;
-  const float z3[3] = {0.f, 0.f, 0.f};
-  const C2fGeom g = make_geom(level, final_res, z3, z3);
-  c2f_scatter_kernel<<<stride_grid(capacity, 256, 4), 256, 0, (cudaStream_t)stream>>>(idx, vals, counters, capacity, g, occ, done,
-                                                                                  calculated, conflict_flag, balance_value, stats);
-  return launch_status();
-}
-
-extern "C" int recmv_c2f_conflict_todo(const uint8_t* conflict_flag, const uint8_t* calculated, const int level[3],
-                                       const int final_res[3], uint8_t* todo, recmv_stream_t stream) {
-  if (!conflict_flag || !calculated || !level || !final_res || !todo) return RECMV_E_NULL;
-  const float z3[3] = {0.f, 0.f, 0.f};
-  const C2fGeom g = make_geom(level, final_res, z3, z3);
-  c2f_todo_strided_kernel<<<stride_grid((int64_t)g.D * g.H * g.W, 256, 16), 256, 0, (cudaStream_t)stream>>>(conflict_flag, calculated, g, todo);
-  return launch_status();
-}
-
-extern "C" int recmv_c2f_done_up(const uint8_t* done, int D, int H, int W, uint8_t* done_up, recmv_stream_t stream) {
-  if (!done || !done_up) return RECMV_E_NULL;
-  if (D <= 0 || H <= 0 || W <= 0) return RECMV_E_SHAPE;
-  const int64_t total = (int64_t)(2 * D - 1) * (2 * H - 1) * (2 * W - 1);
-  c2f_done_up_kernel<<<stride_grid(total, 256, 16), 256, 0, (cudaStream_t)stream>>>(done, D, H, W, done_up);
-  return launch_status();
-}
 
 extern "C" int recmv_interp2x_boundary3d_fwd(const float* input, float* output, uint8_t* is_boundary, int NC, int D,
                                              int H, int W, float balance_value, int order, recmv_stream_t stream) {

@@ -5,7 +5,7 @@ namespace recmv {
 unsigned long long g_launch_count = 0;
 }
 
-extern "C" int recmv_version(void) { return 100; }  // 0.1.0 -> round 1
+extern "C" int recmv_version(void) { return 101; }  // ABI version: raised whenever an export is removed or changes
 
 extern "C" int64_t recmv_launch_count(void) { return (int64_t)recmv::g_launch_count; }
 

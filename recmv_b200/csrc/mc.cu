@@ -438,54 +438,18 @@ int mc_emit_passes(const float* sdf, int NX, int NY, int NZ, float iso, const Mc
                    const float origin[3], float* verts, int64_t cap_v, int64_t* faces, int64_t cap_f, cudaStream_t st) {
   const int grid = (sc.nb * 32 + kMcWarpBlock - 1) / kMcWarpBlock;
   const FastDiv dplane = FastDiv::make((unsigned)NY * NZ), dnz = FastDiv::make((unsigned)NZ);
-  if (verts) {
-    mc_emit_kernel<false><<<grid, kMcWarpBlock, 0, st>>>(sdf, NX, NY, NZ, iso, sc.bits, sc.block_sums, sc.cellinfo,
-                                                         step[0], step[1], step[2], origin[0], origin[1], origin[2],
-                                                         verts, nullptr, cap_v, sc.totals, sc.nb, dplane, dnz);
-    int s = launch_status();
-    if (s) return s;
-  }
-  if (faces) {
-    if (!verts) return RECMV_E_NULL;  // faces need the packed words written by the vertex pass
-    mc_emit_kernel<true><<<grid, kMcWarpBlock, 0, st>>>(sdf, NX, NY, NZ, iso, sc.bits, sc.block_sums, sc.cellinfo,
-                                                        0.f, 0.f, 0.f, 0.f, 0.f, 0.f, nullptr, (long long*)faces, cap_f,
-                                                        sc.totals, sc.nb, dplane, dnz);
-    int s = launch_status();
-    if (s) return s;
-  }
-  return RECMV_OK;
+  mc_emit_kernel<false><<<grid, kMcWarpBlock, 0, st>>>(sdf, NX, NY, NZ, iso, sc.bits, sc.block_sums, sc.cellinfo,
+                                                       step[0], step[1], step[2], origin[0], origin[1], origin[2],
+                                                       verts, nullptr, cap_v, sc.totals, sc.nb, dplane, dnz);
+  int s = launch_status();
+  if (s) return s;
+  // the faces read the packed vertex words the vertex pass wrote
+  mc_emit_kernel<true><<<grid, kMcWarpBlock, 0, st>>>(sdf, NX, NY, NZ, iso, sc.bits, sc.block_sums, sc.cellinfo,
+                                                      0.f, 0.f, 0.f, 0.f, 0.f, 0.f, nullptr, (long long*)faces, cap_f,
+                                                      sc.totals, sc.nb, dplane, dnz);
+  return launch_status();
 }
 }  // namespace
-
-extern "C" int recmv_mc_count(const float* sdf, int NX, int NY, int NZ, float iso, void* scratch,
-                              int64_t* num_verts, int64_t* num_faces, recmv_stream_t stream) {
-  if (!num_verts || !num_faces) return RECMV_E_NULL;
-  int s = mc_check(sdf, scratch, NX, NY, NZ);
-  if (s) return s;
-  cudaStream_t st = (cudaStream_t)stream;
-  McScratch sc = carve(scratch, NX, NY, NZ);
-  s = mc_classify(sdf, NX, NY, NZ, iso, sc, st);
-  if (s) return s;
-  int h[2] = {0, 0};
-  cudaError_t e = cudaMemcpyAsync(h, sc.totals, sizeof(h), cudaMemcpyDeviceToHost, st);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-  if (e != cudaSuccess) return (int)e;
-  *num_verts = h[0];
-  *num_faces = h[1];
-  if (h[0] >= (1 << 25)) return RECMV_E_RANGE;  // packed vertex ids are 26 bit signed-safe
-  return RECMV_OK;
-}
-
-extern "C" int recmv_mc_emit(const float* sdf, int NX, int NY, int NZ, float iso, void* scratch,
-                             const float step[3], const float origin[3], float* verts,
-                             int64_t* faces, recmv_stream_t stream) {
-  if (!step || !origin) return RECMV_E_NULL;
-  int s = mc_check(sdf, scratch, NX, NY, NZ);
-  if (s) return s;
-  // buffers were sized from recmv_mc_count's totals: no capacity limit
-  return mc_emit_passes(sdf, NX, NY, NZ, iso, carve(scratch, NX, NY, NZ), step, origin, verts, (int64_t)1 << 40, faces,
-                        (int64_t)1 << 40, (cudaStream_t)stream);
-}
 
 // One call, no host synchronisation: classify + count + scan + emit into caller-provided buffers of capacity
 // (cap_verts, cap_faces) rows.  counts (device, int32[4]) receives {V, F, overflow, 0}: with overflow != 0 at least one of

@@ -3,7 +3,7 @@ raise on non-zero status, wire autograd.  PyTorch is plumbing here (device memor
 autograd graph); all arithmetic happens in librecmv_b200.so.
 """
 import ctypes
-from ctypes import byref, c_float, c_int64, c_size_t
+from ctypes import byref, c_float, c_size_t
 
 import torch
 
@@ -357,27 +357,6 @@ def mc_gpu(sdfs, xstep=1.0, ystep=1.0, zstep=1.0, xmin=0.0, ymin=0.0, zmin=0.0, 
         else:
             raise _lib.RecmvError("recmv_mc_run: output buffers still too small after growing")
         return [st["verts"][:V].clone(), st["faces"][:F].clone()]
-
-
-def mc_gpu_two_call(sdfs, step=(1.0, 1.0, 1.0), origin=(0.0, 0.0, 0.0), iso=0.0):
-    """The count / emit pair of the C ABI (exact-size outputs; synchronises between the two calls like the reference)."""
-    _check_input(sdfs, "sdfs")
-    NX, NY, NZ = sdfs.shape
-    lib = _lib.load()
-    nbytes = c_size_t(0)
-    check(lib.recmv_mc_scratch_bytes(NX, NY, NZ, byref(nbytes)), "recmv_mc_scratch_bytes")
-    scratch = torch.empty((nbytes.value,), dtype=torch.uint8, device=sdfs.device)
-    V, F = c_int64(0), c_int64(0)
-    with torch.cuda.device(sdfs.device):
-        st = _stream(sdfs)
-        check(lib.recmv_mc_count(_ptr(sdfs), NX, NY, NZ, float(iso), _ptr(scratch), byref(V), byref(F), st), "recmv_mc_count")
-        verts = torch.empty((V.value, 3), dtype=torch.float32, device=sdfs.device)
-        faces = torch.empty((F.value, 3), dtype=torch.int64, device=sdfs.device)
-        if V.value > 0:
-            check(lib.recmv_mc_emit(_ptr(sdfs), NX, NY, NZ, float(iso), _ptr(scratch), (c_float * 3)(*step),
-                                    (c_float * 3)(*origin), _ptr(verts), _ptr(faces) if F.value > 0 else None, st),
-                  "recmv_mc_emit")
-    return [verts, faces]
 
 
 # --------------------------------------------------------------------------------------------------
@@ -1574,14 +1553,6 @@ class C2fLevel:
         """(queried so far, conflicts of the last round, overflow) -- the level's host synchronisation."""
         h = self.ctr.tolist()
         return h[4], h[2 + self.cur], h[1]
-
-
-def c2f_done_up(done_u8):
-    D, H, W = done_u8.shape
-    up = torch.empty((2 * D - 1, 2 * H - 1, 2 * W - 1), dtype=torch.uint8, device=done_u8.device)
-    with torch.cuda.device(up.device):
-        check(_lib.load().recmv_c2f_done_up(_ptr(done_u8), D, H, W, _ptr(up), _stream(up)), "recmv_c2f_done_up")
-    return up
 
 
 def surface_solve(cam_pos, rays, seeds, batch_inds, sdf_packed, sdf_pe_w, tr_packed, tr_pe_w, conds, skin, dthreshold,

@@ -108,8 +108,8 @@ def test_c2f_sweep_and_discretize_on_gpu():
                                          # the full production 'coarse' pyramid of train.py:42-48
                                          [(15, 21, 9), (29, 41, 17), (57, 81, 33), (113, 161, 65), (225, 321, 129)]])
 def test_c2f_device_worklist_is_bit_identical_to_the_torch_path(resolutions):
-    """Seg3dLossless with the sweep as a device worklist (recmv_c2f_compact / recmv_sdf_mlp_fwd_counted /
-    recmv_c2f_scatter / recmv_c2f_conflict_todo): same voxels re-queried, same query-point arithmetic -> the grid equals
+    """Seg3dLossless with the sweep as a device worklist (recmv_c2f_refine / recmv_sdf_mlp_fwd_counted /
+    recmv_c2f_scatter_list / recmv_c2f_mark_conflicts): same voxels re-queried, same query-point arithmetic -> the grid equals
     the torch-op path's (itself bit-identical to the reference class, tests/test_c2f_cpu.py) bit for bit, per-level
     statistics included; isotropic pyramid and the anisotropic 'coarse' pyramid of train.py:42-48 (halved)."""
     from recmv_b200 import testing
