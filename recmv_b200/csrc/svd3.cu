@@ -22,7 +22,8 @@ __device__ __forceinline__ void rotate_pair(float (&a)[3][3], float (&v)[3][3], 
   const float alpha = a[0][p] * a[0][p] + a[1][p] * a[1][p] + a[2][p] * a[2][p];
   const float beta = a[0][q] * a[0][q] + a[1][q] * a[1][q] + a[2][q] * a[2][q];
   const float gamma = a[0][p] * a[0][q] + a[1][p] * a[1][q] + a[2][p] * a[2][q];
-  if (fabsf(gamma) <= 1e-7f * sqrtf(alpha * beta) || gamma == 0.f) return;
+  // sqrt(alpha) sqrt(beta), not sqrt(alpha beta): the product is a fourth power of the entries and overflows from 1e10
+  if (fabsf(gamma) <= 1e-7f * (sqrtf(alpha) * sqrtf(beta)) || gamma == 0.f) return;
   rotated = true;
   const float zeta = (beta - alpha) / (2.f * gamma);
   const float t = copysignf(1.f, zeta) / (fabsf(zeta) + sqrtf(1.f + zeta * zeta));
