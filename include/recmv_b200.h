@@ -384,6 +384,30 @@ RECMV_API int recmv_rasterize_meshes(const float* verts, int V, const int64_t* f
                           void* workspace, int64_t capacity, int64_t* out_pix_to_face, float* out_zbuf, float* out_bary,
                           float* out_dists, int32_t* counters /*device*/, recmv_stream_t stream);
 
+/* ---- point rasterizer + alpha compositor: the silhouettes of `pcRender` ------------------------------------------
+ * replaces pytorch3d's PointsRasterizer + AlphaCompositor (model/CameraMine.py:347-415, weights 1 - d / r^2).
+ * points [N,P,3] f32 already projected: (NDC x, NDC y, view z); pixel (row, col) has its centre at NDC
+ * (1 - (2 col + 1) / W, 1 - (2 row + 1) / H).  A point with z < 0 is skipped; it covers a pixel when d < radius^2
+ * (strict, d = squared NDC distance).  Each pixel keeps the K (1..64; more is RECMV_E_RANGE) covering points with the
+ * smallest z, ties to the lower packed index n*P + p (deterministic), and composites them in order:
+ * T_0 = 1, image[g] += f alpha T, T *= 1 - alpha, alpha = 1 - d / radius^2, g = 0 when p < split_size, else 1.
+ * features [N,P] f32 (NULL = all ones).  num_images G = 1 or 2 (image 1 only gets points p >= split_size).
+ * out_images [G,N,H,W].  Fragments (each NULL = not written): out_idx [N,H,W,K] int64 packed, out_zbuf, out_dists
+ * [N,H,W,K], padded with -1.  workspace: recmv_points_raster_workspace_bytes(N, P, H, W, capacity), capacity =
+ * (tile, point) pair entries.  counters (DEVICE int32[4]) <- {covered pixels, skipped points, pairs, overflow}.  No host
+ * synchronisation: when pairs > capacity, overflow = 1 and NO output is written -- re-run with capacity >= pairs.
+ * The backward reads the forward's workspace unchanged (same arguments, pairs = counters[2]): grad_images [G,N,H,W],
+ * pair_scratch 2 * pairs floats, grad_points [N,P,3] (z component 0: the selection is piecewise constant).  It is
+ * summed in a fixed order without float atomics, so it is bit-identical from run to run and on any GPU.           */
+RECMV_API int recmv_points_raster_workspace_bytes(int N, int64_t P, int H, int W, int64_t capacity, size_t* bytes);
+RECMV_API int recmv_rasterize_points(const float* points, const float* features, int N, int64_t P, int H, int W,
+                          float radius, int K, int64_t split_size, int num_images, void* workspace, int64_t capacity,
+                          float* out_images, int64_t* out_idx, float* out_zbuf, float* out_dists,
+                          int32_t* counters /*device*/, recmv_stream_t stream);
+RECMV_API int recmv_rasterize_points_backward(int N, int64_t P, int H, int W, float radius, int K, int64_t split_size,
+                          int num_images, const void* workspace, int64_t pairs, const float* grad_images,
+                          float* pair_scratch, float* grad_points, recmv_stream_t stream);
+
 /* ---- A11 / (f2): the sweep of one pyramid level as a DEVICE WORKLIST (SURVEY 8b `recmv_c2f_sweep`) -----------------
  * replaces the coordinate-list bookkeeping of MCAcc/seg3d_lossless.py:306-428 (nonzero / unique / index scatter, a
  * host sync per step).  level / final_res are (W, H, D) = (x, y, z) lattice sizes (host).  A worklist is idx_out[i]

@@ -1488,6 +1488,116 @@ def rasterize_meshes(verts, faces, cameras, H, W, z_clip=1e-6, area_eps=1e-8, wa
     return p2f, zbuf, bary, dists, counts
 
 
+_points_state = {}   # per device: the pair-list capacity of the first attempt + counters and their pinned host copy
+
+
+def _points_dims(points, features, K, split_size):
+    """(N, P, split) of a rasterize_points call; split_size None = P (every point in the first image)."""
+    _check_input(points, "points")
+    if points.dtype != torch.float32 or points.dim() != 3 or points.shape[2] != 3:
+        raise RuntimeError(f"rasterize_points: points must be float32 [N,P,3], got {points.dtype} {tuple(points.shape)}")
+    N, P = int(points.shape[0]), int(points.shape[1])
+    if features is not None:
+        _check_operand(features, points, (N, P), "features")
+        _check_input(features, "features")
+    if not 1 <= int(K) <= 64:
+        raise ValueError(f"rasterize_points: points_per_pixel must be in [1, 64], got {K}")
+    split = P if split_size is None else int(split_size)
+    if not 0 <= split <= P:
+        raise ValueError(f"rasterize_points: split_size must be in [0, {P}], got {split_size}")
+    return N, P, split
+
+
+def rasterize_points(points, features, H, W, radius, K, split_size=None, want_fragments=False, capacity=None):
+    """K-nearest point rasterizer + alpha compositor (recmv_rasterize_points).  points [N,P,3] f32 (NDC x, NDC y, view z),
+    features [N,P] f32 or None (ones), CUDA and contiguous.  split_size=None renders one image; an int s renders two,
+    points p < s into the first.  Returns (images [G,N,H,W], (idx [N,H,W,K] int64, zbuf, dists) or None, counts, ws)
+    with counts = {covered, skipped, pairs} as host ints and ws the per-call workspace the backward reads.
+
+    One host read per call: the counters after the launch.  Only when the (tile, point) pair list overflowed is the call
+    re-run, once, with a list of the reported size.  `capacity` sets the list size of the first attempt (by default the
+    largest pair count this device has seen, at least 8 pairs per point)."""
+    G = 1 if split_size is None else 2
+    N, P, split = _points_dims(points, features, K, split_size)
+    H, W, K = int(H), int(W), int(K)
+    dev = points.device
+    lib = _lib.load()
+    st = _points_state.setdefault(dev.index, {})
+    if st.get("counters") is None:
+        st["counters"] = torch.zeros((4,), dtype=torch.int32, device=dev)
+        st["counters_host"] = torch.zeros((4,), dtype=torch.int32).pin_memory()
+    cap = int(capacity) if capacity is not None else max(st.get("capacity", 0), 8 * N * P + 4096)
+    images = torch.empty((G, N, H, W), dtype=torch.float32, device=dev)
+    frags = tuple(torch.empty((N, H, W, K), dtype=dt, device=dev) for dt in (torch.int64, torch.float32, torch.float32)) \
+        if want_fragments else None
+    ctr = st["counters"]
+    with torch.cuda.device(dev):
+        stream = _stream(points)
+        for _ in range(2):
+            nbytes = c_size_t(0)
+            check(lib.recmv_points_raster_workspace_bytes(N, P, H, W, cap, byref(nbytes)),
+                  "recmv_points_raster_workspace_bytes")
+            ws = torch.empty((nbytes.value,), dtype=torch.uint8, device=dev)
+            check(lib.recmv_rasterize_points(_ptr(points), _ptr(features), N, P, H, W, float(radius), K, split, G,
+                                             _ptr(ws), cap, _ptr(images), *(_ptr(t) for t in (frags or (None,) * 3)),
+                                             _ptr(ctr), stream), "recmv_rasterize_points")
+            st["counters_host"].copy_(ctr, non_blocking=True)
+            torch.cuda.current_stream(dev).synchronize()
+            covered, skipped, pairs, overflow = (int(v) for v in st["counters_host"])
+            st["capacity"] = max(st.get("capacity", 0), pairs)
+            if not overflow:
+                break
+            if pairs >= 0x7fffffff:
+                check(_lib.RECMV_E_RANGE, "recmv_rasterize_points (more than 2^31 - 1 tile / point pairs)")
+            cap = pairs   # grow once to the exact size and re-run
+        else:
+            raise _lib.RecmvError("recmv_rasterize_points: pair list still too small after growing")
+    counts = {"covered": covered, "skipped": skipped, "pairs": pairs}
+    return images, frags, counts, ws
+
+
+def rasterize_points_backward(grad_images, ws, pairs, N, P, H, W, radius, K, split_size=None):
+    """grad_points [N,P,3] of rasterize_points (recmv_rasterize_points_backward) from the image cotangents
+    [G,N,H,W] and the forward's workspace `ws` and pair count; z components are 0."""
+    G = 1 if split_size is None else 2
+    split = P if split_size is None else int(split_size)
+    dev = ws.device
+    grad_images = grad_images.contiguous().float()
+    if grad_images.device != dev or tuple(grad_images.shape) != (G, N, H, W):
+        raise RuntimeError(f"rasterize_points_backward: grad_images must be [{G},{N},{H},{W}] on {dev}, got "
+                           f"{tuple(grad_images.shape)} on {grad_images.device}")
+    grad = torch.empty((N, P, 3), dtype=torch.float32, device=dev)
+    scratch = torch.empty((max(int(pairs), 1), 2), dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        check(_lib.load().recmv_rasterize_points_backward(N, P, H, W, float(radius), int(K), split, G, _ptr(ws), int(pairs),
+                                                          _ptr(grad_images), _ptr(scratch), _ptr(grad),
+                                                          _stream(grad_images)), "recmv_rasterize_points_backward")
+    return grad
+
+
+class RasterizePointsFunction(torch.autograd.Function):
+    """images [G,N,H,W] = rasterize_points(points, ...)[0], differentiable in the points' NDC x and y.  The fragments
+    (when asked) are returned after the images and carry no gradient; features must not require grad.  The forward's
+    binned lists are kept for the backward (no re-binning)."""
+
+    @staticmethod
+    def forward(ctx, points, features, H, W, radius, K, split_size=None, want_fragments=False):
+        if features is not None and features.requires_grad:
+            raise RuntimeError("rasterize_points: features must not require grad (no gradient is computed for them)")
+        images, frags, counts, ws = rasterize_points(points, features, H, W, radius, K, split_size, want_fragments)
+        ctx.ws, ctx.pairs = ws, counts["pairs"]
+        ctx.args = (int(points.shape[0]), int(points.shape[1]), int(H), int(W), float(radius), int(K), split_size)
+        if frags is None:
+            return images
+        ctx.mark_non_differentiable(*frags)
+        return (images,) + frags
+
+    @staticmethod
+    def backward(ctx, grad_images, *unused):
+        g = rasterize_points_backward(grad_images, ctx.ws, ctx.pairs, *ctx.args)
+        return g, None, None, None, None, None, None, None
+
+
 class C2fLevel:
     """Device worklist of one pyramid level (recmv_c2f_refine / recmv_sdf_mlp_fwd_counted / recmv_c2f_scatter_list /
     recmv_c2f_mark_conflicts): one fused full-grid pass builds the level and its worklist, conflict rounds are driven by
