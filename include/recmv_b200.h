@@ -408,6 +408,26 @@ RECMV_API int recmv_rasterize_points_backward(int N, int64_t P, int H, int W, fl
                           int num_images, const void* workspace, int64_t pairs, const float* grad_images,
                           float* pair_scratch, float* grad_points, recmv_stream_t stream);
 
+/* ---- vertex normals + hard Phong shading: the images of `maskRender` with a HardPhongShader ----------------------
+ * replaces pytorch3d's `Meshes.verts_normals_packed` and `HardPhongShader` (infer_fl.py:167; DESIGN section 1d).
+ * Normals: verts [N,V,3] f32, faces [F,3] int64 shared by the N frames -> out_normals [N,V,3].  Every (face, corner k)
+ * adds cross(v[k+1] - v[k], v[k+2] - v[k]) to its vertex, summed in increasing (face, corner) order without float
+ * atomics (bit-identical from run to run and on any GPU), then n / max(|n|, 1e-6).  A face with an index outside
+ * [0, V) adds nothing; an unreferenced vertex gets 0.  workspace: recmv_vertex_normals_workspace_bytes(V, F).
+ * No host synchronisation.
+ * Phong: pix_to_face [N,H,W] int64 packed m*F + f and bary [N,H,W,3] (perspective-corrected) from
+ * recmv_rasterize_meshes; verts, normals [N,V,3]; colors [N,V,3] or NULL (= 1); params DEVICE float[N][28] per frame
+ * {camera centre[3], light location[3], light ambient[3], light diffuse[3], light specular[3], material ambient[3],
+ * material diffuse[3], material specular[3], shininess, background[3]}.  out_rgba [N,H,W,4], 16-byte aligned:
+ * rgb = (ambient + diffuse) * colour + specular, alpha 1; background where pix_to_face is outside [0, N*F) or the face
+ * has an index outside [0, V).                                                                                      */
+RECMV_API int recmv_vertex_normals_workspace_bytes(int V, int64_t F, size_t* bytes);
+RECMV_API int recmv_vertex_normals(const float* verts, int N, int V, const int64_t* faces, int64_t F, void* workspace,
+                          float* out_normals, recmv_stream_t stream);
+RECMV_API int recmv_shade_phong(const int64_t* pix_to_face, const float* bary, int N, int H, int W, const float* verts,
+                          const float* normals, const float* colors, int V, const int64_t* faces, int64_t F,
+                          const float* params /*device[N][28]*/, float* out_rgba, recmv_stream_t stream);
+
 /* ---- A11 / (f2): the sweep of one pyramid level as a DEVICE WORKLIST (SURVEY 8b `recmv_c2f_sweep`) -----------------
  * replaces the coordinate-list bookkeeping of MCAcc/seg3d_lossless.py:306-428 (nonzero / unique / index scatter, a
  * host sync per step).  level / final_res are (W, H, D) = (x, y, z) lattice sizes (host).  A worklist is idx_out[i]

@@ -1598,6 +1598,77 @@ class RasterizePointsFunction(torch.autograd.Function):
         return g, None, None, None, None, None, None, None
 
 
+_normals_state = {}   # per device: grow-only workspace of the vertex-normal incidence sort
+
+SHADE_PARAMS = 28     # per-frame constants of recmv_shade_phong (include/recmv_b200.h)
+
+
+def vertex_normals(verts, faces):
+    """Area-weighted vertex normals (recmv_vertex_normals): verts [N,V,3] f32, faces [F,3] int64 shared by the N frames,
+    CUDA and contiguous -> [N,V,3] f32, n / max(|n|, 1e-6).  Summed in (face, corner) order without float atomics, so
+    bit-identical from run to run; no host synchronisation."""
+    for t, name in ((verts, "verts"), (faces, "faces")):
+        _check_input(t, name)
+    dev = verts.device
+    if faces.device != dev:
+        raise RuntimeError(f"vertex_normals: faces must be on {dev}")
+    if verts.dtype != torch.float32 or verts.dim() != 3 or verts.shape[2] != 3:
+        raise RuntimeError(f"vertex_normals: verts must be float32 [N,V,3], got {verts.dtype} {tuple(verts.shape)}")
+    if faces.dtype != torch.int64 or faces.dim() != 2 or faces.shape[1] != 3:
+        raise RuntimeError(f"vertex_normals: faces must be int64 [F,3], got {faces.dtype} {tuple(faces.shape)}")
+    N, V, F = int(verts.shape[0]), int(verts.shape[1]), int(faces.shape[0])
+    out = torch.empty((N, V, 3), dtype=torch.float32, device=dev)
+    lib = _lib.load()
+    st = _normals_state.setdefault(dev.index, {})
+    with torch.cuda.device(dev):
+        nbytes = c_size_t(0)
+        check(lib.recmv_vertex_normals_workspace_bytes(V, F, byref(nbytes)), "recmv_vertex_normals_workspace_bytes")
+        if st.get("ws") is None or st["ws"].numel() < max(nbytes.value, 1):
+            st["ws"] = torch.empty((max(nbytes.value, 1),), dtype=torch.uint8, device=dev)
+        check(lib.recmv_vertex_normals(_ptr(verts), N, V, _ptr(faces), F, _ptr(st["ws"]), _ptr(out), _stream(verts)),
+              "recmv_vertex_normals")
+    return out
+
+
+def shade_phong(frags, verts, normals, colors, faces, params):
+    """Hard Phong shading of K = 1 mesh fragments (recmv_shade_phong).  frags: an object with pix_to_face [N,H,W,1]
+    int64 and bary_coords [N,H,W,1,3] f32 (raster.Fragments), or the tuple of rasterize_meshes; verts, normals [N,V,3]
+    f32; colors [N,V,3] f32 or None (= 1); faces [F,3] int64; params [N,28] f32 per-frame constants (camera centre,
+    light location and colours, material colours, shininess, background).  All CUDA and contiguous.
+    Returns [N,H,W,4] f32 RGBA with alpha 1."""
+    p2f, bary = (frags.pix_to_face, frags.bary_coords) if hasattr(frags, "pix_to_face") else (frags[0], frags[2])
+    for t, name in ((p2f, "pix_to_face"), (bary, "bary_coords"), (verts, "verts"), (normals, "normals"),
+                    (faces, "faces"), (params, "params")) + (((colors, "colors"),) if colors is not None else ()):
+        _check_input(t, name)
+    dev = verts.device
+    if p2f.dtype != torch.int64 or p2f.dim() != 4 or p2f.shape[3] != 1:
+        raise RuntimeError(f"shade_phong: pix_to_face must be int64 [N,H,W,1], got {p2f.dtype} {tuple(p2f.shape)}")
+    N, H, W = (int(s) for s in p2f.shape[:3])
+    if bary.dtype != torch.float32 or tuple(bary.shape) != (N, H, W, 1, 3):
+        raise RuntimeError(f"shade_phong: bary_coords must be float32 [{N},{H},{W},1,3], got {bary.dtype} "
+                           f"{tuple(bary.shape)}")
+    if verts.dtype != torch.float32 or verts.dim() != 3 or verts.shape[0] != N or verts.shape[2] != 3:
+        raise RuntimeError(f"shade_phong: verts must be float32 [{N},V,3], got {verts.dtype} {tuple(verts.shape)}")
+    V = int(verts.shape[1])
+    for t, name in ((normals, "normals"), (colors, "colors")):
+        if t is not None and (t.dtype != torch.float32 or tuple(t.shape) != (N, V, 3)):
+            raise RuntimeError(f"shade_phong: {name} must be float32 [{N},{V},3], got {t.dtype} {tuple(t.shape)}")
+    if faces.dtype != torch.int64 or faces.dim() != 2 or faces.shape[1] != 3:
+        raise RuntimeError(f"shade_phong: faces must be int64 [F,3], got {faces.dtype} {tuple(faces.shape)}")
+    if params.dtype != torch.float32 or tuple(params.shape) != (N, SHADE_PARAMS):
+        raise RuntimeError(f"shade_phong: params must be float32 [{N},{SHADE_PARAMS}], got {params.dtype} "
+                           f"{tuple(params.shape)}")
+    for t in (p2f, bary, normals, faces, params, colors):
+        if t is not None and t.device != dev:
+            raise RuntimeError(f"shade_phong: every input must be on {dev}")
+    out = torch.empty((N, H, W, 4), dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        check(_lib.load().recmv_shade_phong(_ptr(p2f), _ptr(bary), N, H, W, _ptr(verts), _ptr(normals), _ptr(colors), V,
+                                            _ptr(faces), int(faces.shape[0]), _ptr(params), _ptr(out), _stream(verts)),
+              "recmv_shade_phong")
+    return out
+
+
 class C2fLevel:
     """Device worklist of one pyramid level (recmv_c2f_refine / recmv_sdf_mlp_fwd_counted / recmv_c2f_scatter_list /
     recmv_c2f_mark_conflicts): one fused full-grid pass builds the level and its worklist, conflict rounds are driven by

@@ -47,6 +47,67 @@ def rasterize_meshes(verts, faces, cameras, image_size, z_clip=1e-6, area_eps=1e
     return Fragments(p2f, zbuf, bary, dists)
 
 
+def vertex_normals(verts, faces):
+    """Per-vertex normals of N meshes with one face list (pytorch3d's `Meshes.verts_normals_padded` for meshes of equal
+    size): verts [N,V,3], faces [F,3] -> [N,V,3] f32, area-weighted, unit length (0 for an unreferenced vertex).
+    Deterministic (csrc/shade.cu, DESIGN section 1d).  Forward only; the inputs are used detached."""
+    if not verts.is_cuda:
+        raise RuntimeError("vertex_normals runs on CUDA tensors only (no CPU path)")
+    return ops.vertex_normals(verts.detach().float().contiguous(), faces.detach().long().contiguous())
+
+
+# pytorch3d's PointLights and Materials defaults
+DEFAULT_LIGHTS = {"location": (0.0, 1.0, 0.0), "ambient_color": (0.5,) * 3, "diffuse_color": (0.3,) * 3,
+                  "specular_color": (0.2,) * 3}
+DEFAULT_MATERIALS = {"ambient_color": (1.0,) * 3, "diffuse_color": (1.0,) * 3, "specular_color": (1.0,) * 3,
+                     "shininess": 64.0}
+
+
+def _rows(x, N, width, device, what):
+    """x (1 or N rows of `width` values) -> [N,width] f32 on `device`, one row broadcast to all frames."""
+    t = torch.as_tensor(x, dtype=torch.float32).detach().to(device).reshape(-1, width)
+    if t.shape[0] == 1:
+        return t.expand(N, width)
+    if t.shape[0] != N:
+        raise RuntimeError(f"shade_meshes: {t.shape[0]} rows of {what} for {N} frames")
+    return t
+
+
+def shade_params(cameras, lights, materials, background, N, device):
+    """[N,28] per-frame constants of ops.shade_phong, built on `device` without a host read: camera centre -R T,
+    light location and colours, material colours, shininess, background.  lights / materials are objects with
+    pytorch3d's attribute names (or None for its defaults)."""
+    cam = camera_rows(cameras, N, device)
+    R, T = cam[:, 4:13].view(N, 3, 3), cam[:, 13:16]
+    # element-wise, so one broadcast camera and N equal rows give the same bits
+    centre = -(R[:, :, 0] * T[:, 0:1] + R[:, :, 1] * T[:, 1:2] + R[:, :, 2] * T[:, 2:3])
+    lt = {k: getattr(lights, k) if lights is not None else v for k, v in DEFAULT_LIGHTS.items()}
+    mt = {k: getattr(materials, k) if materials is not None else v for k, v in DEFAULT_MATERIALS.items()}
+    parts = [centre] + [_rows(lt[k], N, 3, device, k) for k in ("location", "ambient_color", "diffuse_color",
+                                                                   "specular_color")]
+    parts += [_rows(mt[k], N, 3, device, k) for k in ("ambient_color", "diffuse_color", "specular_color")]
+    parts += [_rows(mt["shininess"], N, 1, device, "shininess"), _rows(background, N, 3, device, "background")]
+    return torch.cat(parts, 1).contiguous()
+
+
+def shade_meshes(verts, faces, fragments, cameras, colors=None, lights=None, materials=None, background=(1.0, 1.0, 1.0)):
+    """pytorch3d's HardPhongShader on the K = 1 fragments of rasterize_meshes (DESIGN section 1d): verts [N,V,3] world,
+    faces [F,3], colors [N,V,3] or [1,V,3] per-vertex colours (None = 1), cameras as for rasterize_meshes (the camera
+    centre -R T is the eye of the specular term), lights / materials with pytorch3d's attributes (None = its
+    defaults), each with 1 or N rows.  Returns [N,H,W,4]: rgb = (ambient + diffuse) * colour + specular, unclamped,
+    `background` where no face was hit, alpha 1.  Forward only; the inputs are used detached."""
+    if not verts.is_cuda:
+        raise RuntimeError("shade_meshes runs on CUDA tensors only (no CPU path)")
+    verts = verts.detach().float().contiguous()
+    faces = faces.detach().long().contiguous()
+    N, V = int(verts.shape[0]), int(verts.shape[1])
+    if colors is not None:
+        colors = torch.as_tensor(colors).detach().to(device=verts.device, dtype=torch.float32).reshape(-1, V, 3)
+        colors = colors.expand(N, V, 3).contiguous() if colors.shape[0] == 1 else colors.contiguous()
+    params = shade_params(cameras, lights, materials, background, N, verts.device)
+    return ops.shade_phong(fragments, verts, ops.vertex_normals(verts, faces), colors, faces, params)
+
+
 PointFragments = namedtuple("PointFragments", ["idx", "zbuf", "dists"])
 
 
