@@ -428,6 +428,25 @@ RECMV_API int recmv_shade_phong(const int64_t* pix_to_face, const float* bary, i
                           const float* normals, const float* colors, int V, const int64_t* faces, int64_t F,
                           const float* params /*device[N][28]*/, float* out_rgba, recmv_stream_t stream);
 
+/* ---- nearest neighbour (K = 1 knn_points): the feature-curve chamfer loss and template registration --------------
+ * replaces pytorch3d's KNN extension behind `knn_points` / `chamfer_distance` (DESIGN section 1e).
+ * p1 [N,P1,D] queries, p2 [N,P2,D] candidates, f32, D = 2 or 3; lengths1 / lengths2 DEVICE int64[N] or NULL (= P1, P2),
+ * clamped to [0, P] on the device.  d = (dx*dx + dy*dy) [+ dz*dz], dx = x1 - x2, each operation rounded in fp32 in
+ * that order (no FMA); the smallest d wins, on equal d the lower index.  out_dists [N,P1] f32, out_idx [N,P1] int64;
+ * rows i >= lengths1[n], and every row of a cloud with lengths2[n] == 0, get dists 0 and idx -1.  Non-finite
+ * coordinates never give an index outside [-1, lengths2).  The result does not depend on the launch shape or the SM
+ * count.  workspace: recmv_knn_workspace_bytes(N, P1, P2) (serves both the forward and the backward).
+ * Backward from grad_dists [N,P1]: grad_p1 [N,P1,D] = 2 g (p1_i - p2_idx_i); grad_p2 [N,P2,D] (NULL = not computed) =
+ * -sum over the queries i with idx_i = j of grad_p1_i, in increasing i.  Entries with idx outside [0, P2) add nothing.
+ * No float atomics: bit-identical from run to run and on any GPU.  No host synchronisation.                        */
+RECMV_API int recmv_knn_workspace_bytes(int N, int64_t P1, int64_t P2, size_t* bytes);
+RECMV_API int recmv_knn_nearest(const float* p1, const float* p2, const int64_t* lengths1, const int64_t* lengths2,
+                          int N, int64_t P1, int64_t P2, int D, void* workspace, float* out_dists, int64_t* out_idx,
+                          recmv_stream_t stream);
+RECMV_API int recmv_knn_nearest_backward(const float* p1, const float* p2, const int64_t* idx, const float* grad_dists,
+                          int N, int64_t P1, int64_t P2, int D, void* workspace, float* grad_p1, float* grad_p2,
+                          recmv_stream_t stream);
+
 /* ---- A11 / (f2): the sweep of one pyramid level as a DEVICE WORKLIST (SURVEY 8b `recmv_c2f_sweep`) -----------------
  * replaces the coordinate-list bookkeeping of MCAcc/seg3d_lossless.py:306-428 (nonzero / unique / index scatter, a
  * host sync per step).  level / final_res are (W, H, D) = (x, y, z) lattice sizes (host).  A worklist is idx_out[i]

@@ -126,6 +126,11 @@ SIGNATURES = {
     "recmv_vertex_normals": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int64, c_void_p, c_void_p, c_void_p]),
     "recmv_shade_phong": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p,
                                   c_int64, c_void_p, c_void_p, c_void_p]),
+    "recmv_knn_workspace_bytes": (c_int, [c_int, c_int64, c_int64, POINTER(c_size_t)]),
+    "recmv_knn_nearest": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int64, c_int64, c_int, c_void_p,
+                                  c_void_p, c_void_p, c_void_p]),
+    "recmv_knn_nearest_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int64, c_int64, c_int,
+                                           c_void_p, c_void_p, c_void_p, c_void_p]),
     "recmv_c2f_refine":(c_int, [c_void_p, c_void_p, c_int, c_int, c_int, POINTER(c_int), POINTER(c_float), POINTER(c_float),
                                  c_float, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
     "recmv_c2f_scatter_list": (c_int, [c_void_p, c_void_p, c_void_p, c_int, POINTER(c_int), POINTER(c_int), c_void_p,

@@ -9,7 +9,7 @@
 //   nothing; a vertex no face references gets 0.
 //   1. normals_keys_kernel   one thread per (face, corner) e = 3 f + k: key = its vertex (V for an invalid face), value e;
 //   2. CUB radix sort        stable, so each vertex's values stay in increasing e order;
-//   3. normals_bounds_kernel the [begin, end) range of every vertex in the sorted list;
+//   3. segment_bounds_kernel the [begin, end) range of every vertex in the sorted list (segments.cuh);
 //   4. normals_sum_kernel    one thread per (frame, vertex): sum its range in order and normalise.
 //
 // Hard Phong, one thread per pixel: interpolate world position, vertex normal and vertex colour of the winning face
@@ -17,9 +17,8 @@
 // `phong_shading` with `hard_rgb_blend`: alpha 1, background colour where no face was hit).
 #include <math.h>
 
-#include <cub/device/device_radix_sort.cuh>
-
 #include "common.cuh"
+#include "segments.cuh"
 
 namespace recmv {
 namespace {
@@ -38,17 +37,6 @@ __global__ void __launch_bounds__(kNormThreads) normals_keys_kernel(const long l
   const bool ok = a >= 0 && a < V && b >= 0 && b < V && c >= 0 && c < V;
   keys[e] = ok ? (unsigned)faces[e] : (unsigned)V;
   vals[e] = (unsigned)e;
-}
-
-__global__ void __launch_bounds__(kNormThreads) normals_bounds_kernel(const unsigned* __restrict__ keys, long long M,
-                                                                       int V, int* __restrict__ beg,
-                                                                       int* __restrict__ end) {
-  const long long i = blockIdx.x * (long long)kNormThreads + threadIdx.x;
-  if (i >= M) return;
-  const unsigned k = keys[i];
-  if (k >= (unsigned)V) return;
-  if (i == 0 || keys[i - 1] != k) beg[k] = (int)i;
-  if (i == M - 1 || keys[i + 1] != k) end[k] = (int)(i + 1);
 }
 
 __global__ void __launch_bounds__(kNormThreads) normals_sum_kernel(const float* __restrict__ verts, int V,
@@ -139,24 +127,6 @@ __global__ void __launch_bounds__(kShadeThreads) shade_phong_kernel(
   out[pix] = make_float4(rgb[0], rgb[1], rgb[2], 1.f);
 }
 
-size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
-
-int key_bits(int V) {   // bits that hold the keys 0..V (V = the invalid-face sentinel)
-  int bits = 1;
-  while (bits < 32 && (1ull << bits) <= (unsigned long long)V) ++bits;
-  return bits;
-}
-
-// CUB's temporary storage for the sort of M pairs; the same query in the size call and in the run.
-int sort_temp_bytes(long long M, int V, size_t* bytes) {
-  *bytes = 0;
-  if (M == 0) return RECMV_OK;
-  const cudaError_t e = cub::DeviceRadixSort::SortPairs(nullptr, *bytes, (const unsigned*)nullptr, (unsigned*)nullptr,
-                                                        (const unsigned*)nullptr, (unsigned*)nullptr, (int)M, 0,
-                                                        key_bits(V));
-  return e == cudaSuccess ? RECMV_OK : (int)e;
-}
-
 struct NormalsWs {
   unsigned *keys_in, *keys_out, *vals_in, *vals_out;
   int *beg, *end;
@@ -193,7 +163,7 @@ extern "C" int recmv_vertex_normals_workspace_bytes(int V, int64_t F, size_t* by
   if (s) return s;
   const long long M = 3 * (long long)F;
   size_t temp = 0;
-  s = sort_temp_bytes(M, V, &temp);
+  s = sort_temp_bytes(M, (unsigned)V, &temp);
   if (s) return s;
   *bytes = 4 * align256((size_t)M * 4) + 2 * align256((size_t)V * 4) + temp;
   return RECMV_OK;
@@ -217,15 +187,10 @@ extern "C" int recmv_vertex_normals(const float* verts, int N, int V, const int6
     normals_keys_kernel<<<nb, kNormThreads, 0, st>>>((const long long*)faces, M, V, w.keys_in, w.vals_in);
     s = launch_status();
     if (s) return s;
-    size_t temp = 0;
-    s = sort_temp_bytes(M, V, &temp);
+    s = sort_pairs(w.temp, w.keys_in, w.keys_out, w.vals_in, w.vals_out, M, (unsigned)V, st);
     if (s) return s;
-    e = cub::DeviceRadixSort::SortPairs(w.temp, temp, w.keys_in, w.keys_out, w.vals_in, w.vals_out, (int)M, 0,
-                                        key_bits(V), st);
-    if (e != cudaSuccess) return (int)e;
-    s = launch_status();
-    if (s) return s;
-    normals_bounds_kernel<<<nb, kNormThreads, 0, st>>>(w.keys_out, M, V, w.beg, w.end);
+    segment_bounds_kernel<<<(unsigned)((M + kSegThreads - 1) / kSegThreads), kSegThreads, 0, st>>>(
+        w.keys_out, M, (unsigned)V, w.beg, w.end);
     s = launch_status();
     if (s) return s;
   }

@@ -1669,6 +1669,92 @@ def shade_phong(frags, verts, normals, colors, faces, params):
     return out
 
 
+_knn_state = {}   # per device: grow-only workspace of the nearest-neighbour split minima and the backward's sort
+
+
+def _knn_workspace(dev, N, P1, P2):
+    nbytes = c_size_t(0)
+    check(_lib.load().recmv_knn_workspace_bytes(N, P1, P2, byref(nbytes)), "recmv_knn_workspace_bytes")
+    st = _knn_state.setdefault(dev.index, {})
+    if st.get("ws") is None or st["ws"].numel() < max(nbytes.value, 1):
+        st["ws"] = torch.empty((max(nbytes.value, 1),), dtype=torch.uint8, device=dev)
+    return st["ws"]
+
+
+def _knn_lengths(lengths, N, dev, name):
+    if lengths is None:
+        return None
+    _check_input(lengths, name)
+    if lengths.dtype != torch.int64 or tuple(lengths.shape) != (N,) or lengths.device != dev:
+        raise RuntimeError(f"knn_nearest: {name} must be int64 [{N}] on {dev}, got {lengths.dtype} "
+                           f"{tuple(lengths.shape)} on {lengths.device}")
+    return lengths
+
+
+def knn_nearest(p1, p2, lengths1=None, lengths2=None):
+    """Nearest neighbour of every p1 point in p2 (recmv_knn_nearest): p1 [N,P1,D], p2 [N,P2,D] f32, D = 2 or 3, lengths
+    int64 [N] on the device or None, all CUDA and contiguous.  Returns (dists [N,P1] f32 squared distance, idx [N,P1]
+    int64); padded rows (i >= lengths1, or lengths2 == 0) get 0 and -1.  Deterministic; no host synchronisation."""
+    for t, name in ((p1, "p1"), (p2, "p2")):
+        _check_input(t, name)
+        if t.dtype != torch.float32 or t.dim() != 3 or t.shape[2] not in (2, 3):
+            raise RuntimeError(f"knn_nearest: {name} must be float32 [N,P,2|3], got {t.dtype} {tuple(t.shape)}")
+    dev = p1.device
+    N, P1, D = (int(s) for s in p1.shape)
+    if p2.device != dev or p2.shape[0] != N or p2.shape[2] != D:
+        raise RuntimeError(f"knn_nearest: p2 must be [{N},P2,{D}] on {dev}, got {tuple(p2.shape)} on {p2.device}")
+    P2 = int(p2.shape[1])
+    l1, l2 = _knn_lengths(lengths1, N, dev, "lengths1"), _knn_lengths(lengths2, N, dev, "lengths2")
+    dists = torch.empty((N, P1), dtype=torch.float32, device=dev)
+    idx = torch.empty((N, P1), dtype=torch.int64, device=dev)
+    with torch.cuda.device(dev):
+        ws = _knn_workspace(dev, N, P1, P2)
+        check(_lib.load().recmv_knn_nearest(_ptr(p1), _ptr(p2), _ptr(l1), _ptr(l2), N, P1, P2, D, _ptr(ws), _ptr(dists),
+                                            _ptr(idx), _stream(p1)), "recmv_knn_nearest")
+    return dists, idx
+
+
+def knn_nearest_backward(p1, p2, idx, grad_dists, need_p2=True):
+    """(grad_p1 [N,P1,D], grad_p2 [N,P2,D] or None) of knn_nearest's dists (recmv_knn_nearest_backward), from its idx
+    and grad_dists [N,P1].  grad_p2 sums each candidate's queries in increasing index without float atomics."""
+    N, P1, D = (int(s) for s in p1.shape)
+    P2 = int(p2.shape[1])
+    dev = p1.device
+    grad_dists = grad_dists.contiguous().float()
+    if grad_dists.device != dev or tuple(grad_dists.shape) != (N, P1):
+        raise RuntimeError(f"knn_nearest_backward: grad_dists must be [{N},{P1}] on {dev}, got "
+                           f"{tuple(grad_dists.shape)} on {grad_dists.device}")
+    g1 = torch.empty((N, P1, D), dtype=torch.float32, device=dev)
+    g2 = torch.empty((N, P2, D), dtype=torch.float32, device=dev) if need_p2 else None
+    with torch.cuda.device(dev):
+        ws = _knn_workspace(dev, N, P1, P2)
+        check(_lib.load().recmv_knn_nearest_backward(_ptr(p1), _ptr(p2), _ptr(idx), _ptr(grad_dists), N, P1, P2, D,
+                                                     _ptr(ws), _ptr(g1), _ptr(g2), _stream(p1)),
+              "recmv_knn_nearest_backward")
+    return g1, g2
+
+
+class KnnNearestFunction(torch.autograd.Function):
+    """(dists, idx) = knn_nearest(p1, p2, lengths1, lengths2), differentiable in p1 and p2 through dists; idx carries no
+    gradient and the lengths none.  once_differentiable: no double backward."""
+
+    @staticmethod
+    def forward(ctx, p1, p2, lengths1=None, lengths2=None):
+        dists, idx = knn_nearest(p1, p2, lengths1, lengths2)
+        ctx.save_for_backward(p1, p2, idx)
+        ctx.mark_non_differentiable(idx)
+        return dists, idx
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_dists, unused_idx):
+        p1, p2, idx = ctx.saved_tensors
+        if grad_dists is None:
+            return None, None, None, None
+        g1, g2 = knn_nearest_backward(p1, p2, idx, grad_dists, need_p2=ctx.needs_input_grad[1])
+        return (g1 if ctx.needs_input_grad[0] else None), g2, None, None
+
+
 class C2fLevel:
     """Device worklist of one pyramid level (recmv_c2f_refine / recmv_sdf_mlp_fwd_counted / recmv_c2f_scatter_list /
     recmv_c2f_mark_conflicts): one fused full-grid pass builds the level and its worklist, conflict rounds are driven by

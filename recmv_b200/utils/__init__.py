@@ -3,11 +3,45 @@
 import torch
 
 from .. import ops as _ops
+from ..knn import chamfer_distance
 from ..model.Embedder import annealing_weights  # noqa: F401  (utils/utils.py:40-46)
 from ..ops import FastDiff3x3MinvFunction  # noqa: F401    (utils/utils.py:8-18)
 from . import FindSurfacePs as _fsp
 from .FindSurfacePs import (FindSurfacePs, FindSurfacePsMesh, FindSurfacePsRays, OptimizeGarmentSurfacePs, OptimizeGarmentSurfaceSinlge,  # noqa: F401
                             OptimizeSurfacePs)
+
+
+def _pad_points(t, P):
+    return t if t.shape[1] == P else torch.cat([t, t.new_zeros((t.shape[0], P - t.shape[1]) + tuple(t.shape[2:]))], 1)
+
+
+def fl_proj_loss(fl_pts_list, gt_fl_pts_list, fl_masks, proj_fl_weights=None):
+    """The feature-curve projection loss (engineer/core/fl_optimizer.py:72-110), batched: C curves with screen points
+    fl_pts [N,P_c,>=2] (x, y first), annotations gt [N,M_c,2], per-point visibility fl_masks [N,P_c,3] (the call site
+    expands one flag over the coordinates, so [..., 0] is read) and Python-number weights w_c (default 1).
+    S_{n,c} = sum-reduced chamfer distance of frame n's visible points and its annotations (0 with none visible),
+    V_c = frames with a visible point, Q_c = visible points; L = mean_c w_c sum_n S_{n,c} / (V_c or 1) / (Q_c or 1).
+    The C*N clouds go through one nearest-neighbour call per direction; visible points are compacted on the device by
+    a stable partition.  No host synchronisation in the forward or the backward."""
+    C = len(fl_pts_list)
+    N = int(fl_pts_list[0].shape[0])
+    dev = fl_pts_list[0].device
+    P = max(int(p.shape[1]) for p in fl_pts_list)
+    Ms = [int(g.shape[1]) for g in gt_fl_pts_list]
+    M = max(Ms)
+    x = torch.stack([_pad_points(p[..., :2], P) for p in fl_pts_list]).reshape(C * N, P, 2)
+    vis = torch.stack([_pad_points(m[..., 0] != 0, P) for m in fl_masks]).reshape(C * N, P)
+    order = torch.argsort((~vis).to(torch.uint8), dim=1, stable=True)     # visible points first, in their order
+    xc = torch.gather(x, 1, order[..., None].expand(-1, -1, 2)).contiguous()
+    lx = vis.sum(1)
+    y = torch.stack([_pad_points(g, M) for g in gt_fl_pts_list]).reshape(C * N, M, 2).contiguous()
+    ly = None if min(Ms) == M else torch.cat([torch.full((N,), m, dtype=torch.int64, device=dev) for m in Ms])
+    S = chamfer_distance(xc, y, lx, ly, batch_reduction=None, point_reduction="sum")[0].view(C, N).sum(1)
+    cnt = lx.view(C, N)
+    V, Q = (cnt > 0).sum(1), cnt.sum(1)
+    w = [1.0] * C if proj_fl_weights is None else [float(v) for v in proj_fl_weights]
+    w = torch.tensor(w, dtype=S.dtype).pin_memory().to(dev, non_blocking=True)
+    return (w * S / V.clamp_min(1) / Q.clamp_min(1)).sum() / C
 
 
 def compute_Jacobian(ps, ds, retain_graph, create_graph, allow_unused=False):
