@@ -24,6 +24,7 @@ import torch.nn.functional as F
 
 from .. import ops
 from .Embedder import get_embedder, ratio_to_weights
+from .packed import cached_pack
 
 
 def quat2mat(quat):
@@ -140,18 +141,11 @@ class MLPTranslator(nn.Module):
         self.mlp_mode = None
         self.train_fused = True   # grad-enabled forwards go through ops.TranslatorTrainFunction (False: torch graph)
         self.last_path = None
-        self._packed, self._packed_key = None, None
         self.fusable = (multires == 6 and feature_vector_size == 128 and not weight_norm)
 
     def packed_weights(self):
-        params = list(self.parameters())
-        key = tuple((p.data_ptr(), p._version) for p in params)
-        if self._packed is None or key != self._packed_key:
-            with torch.no_grad():
-                self._packed = ops.translator_pack_weights([getattr(self, "lin%d" % l).weight for l in range(5)],
-                                                           [getattr(self, "lin%d" % l).bias for l in range(5)])
-            self._packed_key = key
-        return self._packed
+        return cached_pack(self, lambda: ops.translator_pack_weights([getattr(self, "lin%d" % l).weight for l in range(5)],
+                                                                     [getattr(self, "lin%d" % l).bias for l in range(5)]))
 
     def forward(self, ps, conds, batch_inds=None, **kwargs):
         ratio = kwargs['ratio']['deformerRatio']

@@ -8,6 +8,7 @@ import torch.nn as nn
 
 from .. import ops
 from .Embedder import get_embedder, ratio_to_weights
+from .packed import cached_pack
 
 
 class RenderingNetwork_view_norm(nn.Module):
@@ -37,27 +38,23 @@ class RenderingNetwork_view_norm(nn.Module):
         self.mlp_mode = None
         self.train_fused = True   # grad-enabled forwards go through ops.RenderNetTrainFunction (False: torch graph)
         self.last_path = None
-        self._packed, self._packed_key = None, None
         self.fusable = (mode == 'idr' and multires_v == 4 and multires_n == 0 and feature_vector_size == 256
                         and d_in == 9 and d_out == 3 and list(dims[1:-1]) == [512] * 4)
 
+    def effective_weights(self):
+        Ws, bs = [], []
+        for l in range(self.num_layers - 1):
+            lin = getattr(self, "lin" + str(l))
+            if hasattr(lin, "weight_g"):
+                v, g = lin.weight_v, lin.weight_g
+                Ws.append(v * (g / v.norm(dim=1, keepdim=True)))
+            else:
+                Ws.append(lin.weight)
+            bs.append(lin.bias)
+        return Ws, bs
+
     def packed_weights(self):
-        params = list(self.parameters())
-        key = tuple((p.data_ptr(), p._version) for p in params)
-        if self._packed is None or key != self._packed_key:
-            with torch.no_grad():
-                Ws, bs = [], []
-                for l in range(self.num_layers - 1):
-                    lin = getattr(self, "lin" + str(l))
-                    if hasattr(lin, "weight_g"):
-                        v, g = lin.weight_v, lin.weight_g
-                        Ws.append(v * (g / v.norm(dim=1, keepdim=True)))
-                    else:
-                        Ws.append(lin.weight)
-                    bs.append(lin.bias)
-                self._packed = ops.rendernet_pack_weights(Ws, bs)
-            self._packed_key = key
-        return self._packed
+        return cached_pack(self, lambda: ops.rendernet_pack_weights(*self.effective_weights()))
 
     def forward(self, points, normals, view_dirs, feature_vectors, ratio):
         ratio = ratio['renderRatio']
@@ -73,15 +70,7 @@ class RenderingNetwork_view_norm(nn.Module):
             # training path: tensor-core layer GEMMs forward + backward (ops.RenderNetTrainFunction); tanh and the
             # weight-norm re-parametrisation stay (tiny) torch graphs
             self.last_path = "fused-train"
-            Ws, bs = [], []
-            for l in range(self.num_layers - 1):
-                lin = getattr(self, "lin" + str(l))
-                if hasattr(lin, "weight_g"):
-                    v, g = lin.weight_v, lin.weight_g
-                    Ws.append(v * (g / v.norm(dim=1, keepdim=True)))
-                else:
-                    Ws.append(lin.weight)
-                bs.append(lin.bias)
+            Ws, bs = self.effective_weights()
             pre = ops.RenderNetTrainFunction.apply(points.contiguous().float(), normals.contiguous().float(),
                                                    view_dirs.contiguous().float(), feature_vectors.contiguous().float(),
                                                    ratio_to_weights(self.multires_v, ratio), *Ws, *bs)

@@ -15,6 +15,7 @@ import torch.nn as nn
 
 from .. import ops
 from .Embedder import get_embedder, ratio_to_weights
+from .packed import cached_pack
 
 
 class ImplicitNetwork(nn.Module):
@@ -58,8 +59,6 @@ class ImplicitNetwork(nn.Module):
         self.mlp_mode = None  # None -> ops.DEFAULT_MLP_MODE
         self.train_fused = True   # grad-enabled forwards go through ops.SdfMlpTrainFunction (False: torch graph)
         self.last_path = None
-        self._packed = None
-        self._packed_key = None
         shapes = [tuple(getattr(self, "lin%d" % l).weight.shape) for l in range(self.num_layers - 1)]
         self._fusable = (shapes == ops.SDF_LAYER_SHAPES and tuple(self.skip_in) == (4,)
                          and multires == 6 and d_out == 1)
@@ -78,14 +77,7 @@ class ImplicitNetwork(nn.Module):
         return Ws, bs
 
     def packed_weights(self):
-        params = [p for p in self.parameters()]
-        key = tuple((p.data_ptr(), p._version) for p in params)
-        if self._packed is None or key != self._packed_key:
-            with torch.no_grad():
-                Ws, bs = self.effective_weights()
-                self._packed = ops.sdf_pack_weights(Ws, bs)
-            self._packed_key = key
-        return self._packed
+        return cached_pack(self, lambda: ops.sdf_pack_weights(*self.effective_weights()))
 
     def _pe_weights(self, ratio):
         ratio = ratio if type(ratio) == float or type(ratio) == int or ratio is None else ratio['sdfRatio']

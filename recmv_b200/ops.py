@@ -2,6 +2,7 @@
 raise on non-zero status, wire autograd.  PyTorch is plumbing here (device memory, streams,
 autograd graph); all arithmetic happens in librecmv_b200.so.
 """
+import contextlib
 import ctypes
 from ctypes import byref, c_float, c_size_t
 
@@ -20,6 +21,56 @@ def _stream(t):
 
 def _ptr(t):
     return ctypes.c_void_p(t.data_ptr()) if t is not None else None
+
+
+def _launch(name, like, *args):
+    """Call the export `name` with args and the current stream of like's device, under that device's guard; raise on a
+    non-zero status."""
+    with torch.cuda.device(like.device):
+        check(getattr(_lib.load(), name)(*args, _stream(like)), name)
+
+
+def _size(name, *args, dev=None):
+    """Value of a size query (`*_bytes`, `*_workspace`, `*_floats`): returned by the export, or written to a trailing
+    size_t* after a status that is checked.  dev: the device the size depends on (SM count, library sort sizes); the
+    query then runs under its guard."""
+    fn = getattr(_lib.load(), name)
+    with torch.cuda.device(dev) if dev is not None else contextlib.nullcontext():
+        if fn.restype is c_size_t:
+            return int(fn(*args))
+        n = c_size_t(0)
+        check(fn(*args, byref(n)), name)
+    return int(n.value)
+
+
+# (device index, name) -> what a call keeps on that device for the next one, like the MCGpu singleton
+# (MCGpu/CudaKernels.cu:524-604): grow-only buffers, pinned counters, and the rasterizers' pair-list capacities.
+# Every caller uses its own names.
+_scratch_cache = {}
+
+
+def _scratch(dev, name, rows, dtype=torch.uint8, tail=()):
+    """Grow-only per-device buffer [>= rows, *tail]: reallocated (contents dropped) only when the one kept is smaller."""
+    buf = _scratch_cache.get((dev.index, name))
+    if buf is None or buf.shape[0] < rows:
+        buf = _scratch_cache[(dev.index, name)] = torch.empty((rows,) + tuple(tail), dtype=dtype, device=dev)
+    return buf
+
+
+def _counters(dev, name, n):
+    """(int32 [n] device counters, their pinned host copy), zeroed when first made and kept per device."""
+    key = (dev.index, name)
+    if key not in _scratch_cache:
+        _scratch_cache[key] = (torch.zeros((n,), dtype=torch.int32, device=dev),
+                               torch.zeros((n,), dtype=torch.int32).pin_memory())
+    return _scratch_cache[key]
+
+
+def _read_counters(ctr, host):
+    """Copy the device counters to their pinned host copy and wait for the current stream: the call's one host sync."""
+    host.copy_(ctr, non_blocking=True)
+    torch.cuda.current_stream(ctr.device).synchronize()
+    return host
 
 
 def _check_input(t, name):
@@ -48,9 +99,7 @@ def minv3x3(ms):
     n = ms.size(0)
     invs = torch.empty((n, 3, 3), dtype=ms.dtype, device=ms.device)
     ok = torch.empty((n,), dtype=torch.uint8, device=ms.device)
-    with torch.cuda.device(ms.device):
-        check(_lib.load().recmv_minv3x3_fwd(_ptr(ms), _ptr(invs), _ptr(ok), n, code, _stream(ms)),
-              "recmv_minv3x3_fwd")
+    _launch("recmv_minv3x3_fwd", ms, _ptr(ms), _ptr(invs), _ptr(ok), n, code)
     return [invs, ok.view(torch.bool)]
 
 
@@ -63,9 +112,7 @@ def minv3x3_backward(grads, invs):
     code = _dtype_code(invs, "invs")
     n = invs.size(0)
     outs = torch.empty((n, 3, 3), dtype=invs.dtype, device=invs.device)
-    with torch.cuda.device(invs.device):
-        check(_lib.load().recmv_minv3x3_bwd(_ptr(grads), _ptr(invs), _ptr(outs), n, code,
-                                            _stream(invs)), "recmv_minv3x3_bwd")
+    _launch("recmv_minv3x3_bwd", invs, _ptr(grads), _ptr(invs), _ptr(outs), n, code)
     return outs
 
 
@@ -114,6 +161,16 @@ def _check_operand(t, like, shape, name):
         raise RuntimeError(f"{name} must have shape {tuple(shape)}, got {tuple(t.shape)}")
 
 
+def _expect(fn, name, t, dtype, shape, dev=None):
+    """Raise RuntimeError unless t is `dtype` with `shape` (ints fix an extent, letters leave it free) and, when dev is
+    given, sits on dev."""
+    if (t.dtype != dtype or t.dim() != len(shape) or (dev is not None and t.device != dev)
+            or any(isinstance(s, int) and t.shape[d] != s for d, s in enumerate(shape))):
+        on = f" on {dev}" if dev is not None else ""
+        raise RuntimeError(f"{fn}: {name} must be {dtype} [{','.join(map(str, shape))}]{on}, got {t.dtype} "
+                           f"{tuple(t.shape)} on {t.device}")
+
+
 def grid_sample3d_forward(inp, grid, layout=LAYOUT_NCDHW):
     """GridSamplerMine.forward(input, grid, 0, 1)  (MCAcc/cuda/GridSamplerMine.cpp:75-81)."""
     _check_input(inp, "input")
@@ -122,10 +179,7 @@ def grid_sample3d_forward(inp, grid, layout=LAYOUT_NCDHW):
     N, C, D, H, W, P = _gs_dims(inp, grid, layout)
     out = torch.empty((N, C, grid.size(1), grid.size(2), grid.size(3)), dtype=inp.dtype,
                       device=inp.device)
-    with torch.cuda.device(inp.device):
-        check(_lib.load().recmv_gridsample3d_fwd(_ptr(inp), _ptr(grid), _ptr(out), N, C, D, H, W, P,
-                                                 code, layout, _stream(inp)),
-              "recmv_gridsample3d_fwd")
+    _launch("recmv_gridsample3d_fwd", inp, _ptr(inp), _ptr(grid), _ptr(out), N, C, D, H, W, P, code, layout)
     return out
 
 
@@ -139,10 +193,8 @@ def grid_sample3d_backward(inp, grid, grad_out, layout=LAYOUT_NCDHW, need_grad_i
     grad_out = grad_out.contiguous()
     gi = torch.zeros_like(inp) if need_grad_input else None
     gg = torch.empty_like(grid)
-    with torch.cuda.device(inp.device):
-        check(_lib.load().recmv_gridsample3d_bwd(_ptr(inp), _ptr(grid), _ptr(grad_out), _ptr(gi),
-                                                 _ptr(gg), N, C, D, H, W, P, code, layout,
-                                                 _stream(inp)), "recmv_gridsample3d_bwd")
+    _launch("recmv_gridsample3d_bwd", inp, _ptr(inp), _ptr(grid), _ptr(grad_out), _ptr(gi), _ptr(gg), N, C, D, H, W, P,
+            code, layout)
     return gi, gg
 
 
@@ -163,11 +215,8 @@ def grid_sample3d_dbackward(gg_input, gg_grid, inp, grid, grad_out, layout=LAYOU
     gi =torch.zeros_like(inp) if need_grad_input else None
     gg = torch.empty_like(grid)
     ggo = torch.empty_like(grad_out)
-    with torch.cuda.device(inp.device):
-        check(_lib.load().recmv_gridsample3d_bwd2(_ptr(gg_input), _ptr(gg_grid), _ptr(inp), _ptr(grid),
-                                                  _ptr(grad_out), _ptr(gi), _ptr(gg), _ptr(ggo), N, C,
-                                                  D, H, W, P, code, layout, _stream(inp)),
-              "recmv_gridsample3d_bwd2")
+    _launch("recmv_gridsample3d_bwd2", inp, _ptr(gg_input), _ptr(gg_grid), _ptr(inp), _ptr(grid), _ptr(grad_out), _ptr(gi),
+            _ptr(gg), _ptr(ggo), N, C, D, H, W, P, code, layout)
     return gi, gg, ggo
 
 
@@ -254,9 +303,7 @@ def voxel_to_channels_last(ws):
                            f"{tuple(ws.shape)}")
     _, C, D, H, W = ws.shape
     out =torch.empty((D, H, W, C), dtype=torch.float32, device=ws.device)
-    with torch.cuda.device(ws.device):
-        check(_lib.load().recmv_voxel_to_channels_last(_ptr(ws), _ptr(out), C, D, H, W, _stream(ws)),
-              "recmv_voxel_to_channels_last")
+    _launch("recmv_voxel_to_channels_last", ws, _ptr(ws), _ptr(out), C, D, H, W)
     return out
 
 
@@ -274,9 +321,8 @@ def lbsw_knn_blend(verts, vert_ws, bmin, bmax, resolution, k, align_corners=Fals
     out = torch.empty((D, H, W, C), dtype=torch.float32, device=verts.device)
     idx = torch.empty((D * H * W, k), dtype=torch.int32, device=verts.device) if want_idx else None
     lo, hi = (c_float * 3)(*[float(v) for v in bmin]), (c_float * 3)(*[float(v) for v in bmax])
-    with torch.cuda.device(verts.device):
-        check(_lib.load().recmv_lbsw_knn_blend(_ptr(verts), _ptr(vert_ws), V, C, lo, hi, W, H, D, int(bool(align_corners)),
-                                               int(k), _ptr(out), _ptr(idx), _stream(verts)), "recmv_lbsw_knn_blend")
+    _launch("recmv_lbsw_knn_blend", verts, _ptr(verts), _ptr(vert_ws), V, C, lo, hi, W, H, D, int(bool(align_corners)),
+            int(k), _ptr(out), _ptr(idx))
     return (out, idx) if want_idx else out
 
 
@@ -291,32 +337,14 @@ def lbsw_smooth(ws_cl, times, zero_below=0.0):
     spare = torch.empty_like(ws_cl) if times >= 2 else None
     out = torch.empty((1, C, D, H, W), dtype=torch.float32, device=ws_cl.device)
     out_cl = torch.empty_like(ws_cl)
-    with torch.cuda.device(ws_cl.device):
-        check(_lib.load().recmv_lbsw_smooth(_ptr(ws_cl), _ptr(spare), D, H, W, int(times), float(zero_below), _ptr(out),
-                                            _ptr(out_cl), _stream(ws_cl)), "recmv_lbsw_smooth")
+    _launch("recmv_lbsw_smooth", ws_cl, _ptr(ws_cl), _ptr(spare), D, H, W, int(times), float(zero_below), _ptr(out),
+            _ptr(out_cl))
     return out, out_cl
 
 
 # --------------------------------------------------------------------------------------------------
 # MCGpu
 # --------------------------------------------------------------------------------------------------
-_mc_state = {}   # per device: grow-only scratch + output buffers (like the MCGpu singleton, MCGpu/CudaKernels.cu:524-604)
-
-
-def _mc_buffers(dev, nbytes, cap_v, cap_f):
-    st = _mc_state.setdefault(dev.index, {})
-    if st.get("scratch") is None or st["scratch"].numel() < nbytes:
-        st["scratch"] = torch.empty((nbytes,), dtype=torch.uint8, device=dev)
-    if st.get("verts") is None or st["verts"].shape[0] < cap_v:
-        st["verts"] = torch.empty((cap_v, 3), dtype=torch.float32, device=dev)
-    if st.get("faces") is None or st["faces"].shape[0] < cap_f:
-        st["faces"] = torch.empty((cap_f, 3), dtype=torch.int64, device=dev)
-    if st.get("counts") is None:
-        st["counts"] = torch.zeros((4,), dtype=torch.int32, device=dev)
-        st["counts_host"] = torch.zeros((4,), dtype=torch.int32).pin_memory()
-    return st
-
-
 def mc_gpu(sdfs, xstep=1.0, ystep=1.0, zstep=1.0, xmin=0.0, ymin=0.0, zmin=0.0, fTargetValue=0.0):
     """MCGpu.mc_gpu(sdfs, steps, mins, iso) -> [verts [V,3] f32, faces [F,3] i64]
     (MCGpu/MCGpu.cpp:20-56).  Wrong dtype returns [] exactly like the reference (:41-42).
@@ -330,33 +358,27 @@ def mc_gpu(sdfs, xstep=1.0, ystep=1.0, zstep=1.0, xmin=0.0, ymin=0.0, zmin=0.0, 
     if sdfs.dim() != 3 or min(sdfs.shape) <= 0:
         return []
     NX, NY, NZ = sdfs.shape
-    lib = _lib.load()
-    nbytes = c_size_t(0)
-    check(lib.recmv_mc_scratch_bytes(NX, NY, NZ, byref(nbytes)), "recmv_mc_scratch_bytes")
     dev = sdfs.device
-    prev = _mc_state.get(dev.index, {})
-    cap_v = max(4096, prev["verts"].shape[0] if prev.get("verts") is not None else 0)
-    cap_f = max(8192, prev["faces"].shape[0] if prev.get("faces") is not None else 0)
+    nbytes = _size("recmv_mc_scratch_bytes", NX, NY, NZ)
+    cap_v, cap_f = 4096, 8192     # at least; the output buffers kept from earlier calls may be larger
     step = (c_float * 3)(xstep, ystep, zstep)
     org = (c_float * 3)(xmin, ymin, zmin)
-    with torch.cuda.device(dev):
-        stream = _stream(sdfs)
-        for _ in range(2):
-            st = _mc_buffers(dev, nbytes.value, cap_v, cap_f)
-            check(lib.recmv_mc_run(_ptr(sdfs), NX, NY, NZ, float(fTargetValue), _ptr(st["scratch"]), step, org,
-                                   _ptr(st["verts"]), st["verts"].shape[0], _ptr(st["faces"]), st["faces"].shape[0],
-                                   _ptr(st["counts"]), stream), "recmv_mc_run")
-            st["counts_host"].copy_(st["counts"], non_blocking=True)
-            torch.cuda.current_stream(dev).synchronize()
-            V, F, overflow = (int(v) for v in st["counts_host"][:3])
-            if V >= (1 << 25):
-                check(_lib.RECMV_E_RANGE, "recmv_mc_run (more than 2^25 vertices)")
-            if not overflow:
-                break
-            cap_v, cap_f = int(V * 1.25) + 1024, int(F * 1.25) + 2048   # grow once, re-run (buffers are kept)
-        else:
-            raise _lib.RecmvError("recmv_mc_run: output buffers still too small after growing")
-        return [st["verts"][:V].clone(), st["faces"][:F].clone()]
+    for _ in range(2):
+        scratch = _scratch(dev, "mc_scratch", nbytes)
+        verts = _scratch(dev, "mc_verts", cap_v, torch.float32, (3,))
+        faces = _scratch(dev, "mc_faces", cap_f, torch.int64, (3,))
+        ctr, host = _counters(dev, "mc_counters", 4)
+        _launch("recmv_mc_run", sdfs, _ptr(sdfs), NX, NY, NZ, float(fTargetValue), _ptr(scratch), step, org, _ptr(verts),
+                verts.shape[0], _ptr(faces), faces.shape[0], _ptr(ctr))
+        V, F, overflow = (int(v) for v in _read_counters(ctr, host)[:3])
+        if V >= (1 << 25):
+            check(_lib.RECMV_E_RANGE, "recmv_mc_run (more than 2^25 vertices)")
+        if not overflow:
+            break
+        cap_v, cap_f = int(V * 1.25) + 1024, int(F * 1.25) + 2048   # grow once, re-run (buffers are kept)
+    else:
+        raise _lib.RecmvError("recmv_mc_run: output buffers still too small after growing")
+    return [verts[:V].clone(), faces[:F].clone()]
 
 
 # --------------------------------------------------------------------------------------------------
@@ -385,10 +407,8 @@ def lbs_forward(ps, A, trans, ws_cl, center, extend, batch_inds=None, points_per
     if batch_inds is not None:
         batch_inds = batch_inds.contiguous().long()
     vox = make_voxel(ws_cl, center, extend)
-    with torch.cuda.device(ps.device):
-        check(_lib.load().recmv_lbs_fwd(_ptr(ps), _ptr(tps), _ptr(A), _ptr(trans), _ptr(batch_inds),
-                                        int(points_per_frame), int(A.shape[0]), byref(vox), _ptr(out),
-                                        _ptr(wout), P, _stream(ps)), "recmv_lbs_fwd")
+    _launch("recmv_lbs_fwd", ps, _ptr(ps), _ptr(tps), _ptr(A), _ptr(trans), _ptr(batch_inds), int(points_per_frame),
+            int(A.shape[0]), byref(vox), _ptr(out), _ptr(wout), P)
     return (out, wout) if want_weights else out
 
 
@@ -402,11 +422,8 @@ def lbs_inverse(x_obs, A, trans, ws_cl, center, extend, batch_inds=None, points_
     if batch_inds is not None:
         batch_inds = batch_inds.contiguous().long()
     vox = make_voxel(ws_cl, center, extend)
-    with torch.cuda.device(x_obs.device):
-        check(_lib.load().recmv_lbs_inverse(_ptr(x_obs), _ptr(A), _ptr(trans), _ptr(batch_inds),
-                                            int(points_per_frame), int(A.shape[0]), byref(vox),
-                                            _ptr(xc), _ptr(valid), P, _stream(x_obs)),
-              "recmv_lbs_inverse")
+    _launch("recmv_lbs_inverse", x_obs, _ptr(x_obs), _ptr(A), _ptr(trans), _ptr(batch_inds), int(points_per_frame),
+            int(A.shape[0]), byref(vox), _ptr(xc), _ptr(valid), P)
     return xc, valid.view(torch.bool)
 
 
@@ -419,9 +436,8 @@ def bone_matrices(poses, Js, parents_i32, init_pose=None, want_A=True):
     G = torch.empty((F_, 24, 4, 4), dtype=torch.float32, device=dev)
     A = torch.empty((F_, 24, 4, 4), dtype=torch.float32, device=dev) if want_A else None
     ip = init_pose.contiguous().float() if init_pose is not None else None
-    with torch.cuda.device(dev):
-        check(_lib.load().recmv_bone_matrices(_ptr(poses), _ptr(Js.contiguous().float()), _ptr(parents_i32), _ptr(ip),
-                                              _ptr(G), _ptr(A), F_, _stream(poses)), "recmv_bone_matrices")
+    _launch("recmv_bone_matrices", poses, _ptr(poses), _ptr(Js.contiguous().float()), _ptr(parents_i32), _ptr(ip), _ptr(G),
+            _ptr(A), F_)
     return G, A
 
 
@@ -435,10 +451,8 @@ def bone_matrices_backward(poses, Js, parents_i32, init_pose, G, dG=None, dA=Non
     dG = dG.contiguous().float() if dG is not None else None
     dA = dA.contiguous().float() if dA is not None else None
     ip = init_pose.contiguous().float() if init_pose is not None else None
-    with torch.cuda.device(dev):
-        check(_lib.load().recmv_bone_matrices_backward(_ptr(poses), _ptr(Js.contiguous().float()), _ptr(parents_i32),
-                                                       _ptr(ip), _ptr(G.contiguous()), _ptr(dG), _ptr(dA), _ptr(dposes),
-                                                       F_, _stream(poses)), "recmv_bone_matrices_backward")
+    _launch("recmv_bone_matrices_backward", poses, _ptr(poses), _ptr(Js.contiguous().float()), _ptr(parents_i32), _ptr(ip),
+            _ptr(G.contiguous()), _ptr(dG), _ptr(dA), _ptr(dposes), F_)
     return dposes
 
 
@@ -481,15 +495,11 @@ def lbs_backward(ps, A, grad_out, ws_cl, center, extend, batch_inds=None, points
     dtps = torch.empty((P, 3), dtype=torch.float32, device=dev) if want_tps and tps is not None else None
     dA = torch.empty((F_, 24, 4, 4), dtype=torch.float32, device=dev) if want_A else None
     dtrans = torch.empty((F_, 3), dtype=torch.float32, device=dev) if want_trans else None
-    lib = _lib.load()
-    nbytes = c_size_t(0)
-    check(lib.recmv_lbs_backward_workspace_bytes(P, F_, byref(nbytes)), "recmv_lbs_backward_workspace_bytes")
-    work = torch.empty((max(int(nbytes.value), 16),), dtype=torch.uint8, device=dev) if (want_A or want_trans) else None
+    nbytes = _size("recmv_lbs_backward_workspace_bytes", P, F_)
+    work = torch.empty((max(nbytes, 16),), dtype=torch.uint8, device=dev) if (want_A or want_trans) else None
     vox = make_voxel(ws_cl, center, extend)
-    with torch.cuda.device(dev):
-        check(lib.recmv_lbs_backward(_ptr(ps), _ptr(tps), _ptr(A), None, _ptr(batch_inds), int(points_per_frame), F_,
-                                     byref(vox), _ptr(g), _ptr(dps), _ptr(dtps), _ptr(dA), _ptr(dtrans), _ptr(work), P,
-                                     _stream(ps)), "recmv_lbs_backward")
+    _launch("recmv_lbs_backward", ps, _ptr(ps), _ptr(tps), _ptr(A), None, _ptr(batch_inds), int(points_per_frame), F_,
+            byref(vox), _ptr(g), _ptr(dps), _ptr(dtps), _ptr(dA), _ptr(dtrans), _ptr(work), P)
     return dps, dtps, dA, dtrans
 
 
@@ -518,17 +528,12 @@ def lbs_vjp_backward(ps, A, grad_out, ws_cl, center, extend, batch_inds=None, po
     dps = torch.empty((P, 3), dtype=torch.float32, device=dev) if want_ps else None
     dtps = torch.empty((P, 3), dtype=torch.float32, device=dev) if want_tps and tps is not None else None
     dA = torch.empty((F_, 24, 4, 4), dtype=torch.float32, device=dev) if want_A else None
-    lib = _lib.load()
     work = None
     if want_A:
-        nbytes = c_size_t(0)
-        check(lib.recmv_lbs_backward_workspace_bytes(P, F_, byref(nbytes)), "recmv_lbs_backward_workspace_bytes")
-        work = torch.empty((max(int(nbytes.value), 16),), dtype=torch.uint8, device=dev)
+        work = torch.empty((max(_size("recmv_lbs_backward_workspace_bytes", P, F_), 16),), dtype=torch.uint8, device=dev)
     vox = make_voxel(ws_cl, center, extend)
-    with torch.cuda.device(dev):
-        check(lib.recmv_lbs_vjp_backward(_ptr(ps), _ptr(tps), _ptr(A), _ptr(batch_inds), int(points_per_frame), F_,
-                                         byref(vox), _ptr(g), _ptr(cot_ps), _ptr(cot_tps), _ptr(dg), _ptr(dps),
-                                         _ptr(dtps), _ptr(dA), _ptr(work), P, _stream(ps)), "recmv_lbs_vjp_backward")
+    _launch("recmv_lbs_vjp_backward", ps, _ptr(ps), _ptr(tps), _ptr(A), _ptr(batch_inds), int(points_per_frame), F_,
+            byref(vox), _ptr(g), _ptr(cot_ps), _ptr(cot_tps), _ptr(dg), _ptr(dps), _ptr(dtps), _ptr(dA), _ptr(work), P)
     return dg, dps, dtps, dA
 
 
@@ -598,14 +603,7 @@ class LbsTrainFunction(torch.autograd.Function):
             return dps, dtps, None, None, None, None, None, None
         if torch.is_grad_enabled():
             LbsTrainFunction.last_backward = "autograd-composite (create_graph)"
-            args = [ps, tps, A, trans]
-            ins = [t if (t is None or t.requires_grad) else t.detach() for t in args]
-            with torch.enable_grad():
-                out = ctx.composite(*ins)
-                diff = [t for t in ins if t is not None and t.requires_grad]
-                gr = iter(torch.autograd.grad([out], diff, [g], create_graph=True, allow_unused=True))
-            res = [next(gr) if (t is not None and t.requires_grad) else None for t in ins]
-            return (*[r if n else None for r, n in zip(res, need[:4])], None, None, None, None)
+            return (*_composite_grads(ctx.composite, [ps, tps, A, trans], [g]), None, None, None, None)
         LbsTrainFunction.last_backward = "fused"
         ws_cl, center, extend = ctx.skin
         dps, dtps, dA, dtrans = lbs_backward(ps.reshape(-1, 3), A, g.reshape(-1, 3), ws_cl, center, extend, batch_inds,
@@ -623,25 +621,31 @@ SDF_LAYER_SHAPES = [(512, 39), (512, 512), (512, 512), (473, 512), (512, 512), (
                     (512, 512), (257, 512)]
 
 
-def sdf_pack_weights(Ws, bs):
-    """Ws[l] [out,in] effective fp32 weights (weight-norm applied), bs[l] [out] -> packed device blob."""
-    dev = Ws[0].device
-    for (o, i), W, b in zip(SDF_LAYER_SHAPES, Ws, bs):
-        if tuple(W.shape) != (o, i) or tuple(b.shape) != (o,):
-            raise RuntimeError(f"unexpected SDF layer shape {tuple(W.shape)} (want {(o, i)})")
-    W_all = torch.cat([W.detach().reshape(-1).float() for W in Ws]).contiguous()
-    b_all = torch.cat([b.detach().reshape(-1).float() for b in bs]).contiguous()
-    lib = _lib.load()
-    nbytes = lib.recmv_sdf_packed_bytes()
-    # 1 KiB alignment for the TMA-visible planes
+def _aligned_blob(nbytes, dev):
+    """nbytes of device memory at a 1 KiB boundary (the TMA-visible weight planes need it)."""
     raw = torch.empty((nbytes + 1024,), dtype=torch.uint8, device=dev)
     off = (-raw.data_ptr()) % 1024
-    packed = raw[off:off + nbytes]
-    with torch.cuda.device(dev):
-        check(lib.recmv_sdf_pack_weights(_ptr(W_all), _ptr(b_all), _ptr(packed), _stream(W_all)),
-              "recmv_sdf_pack_weights")
-    packed._keepalive = raw
+    blob = raw[off:off + nbytes]
+    blob._keepalive = raw
+    return blob
+
+
+def _pack_weights(net, label, shapes, Ws, bs):
+    """Ws[l] [out,in], bs[l] [out] of the layers in `shapes` -> the device blob of recmv_{net}_pack_weights."""
+    for (o, i), W, b in zip(shapes, Ws, bs):
+        if tuple(W.shape) != (o, i) or tuple(b.shape) != (o,):
+            raise RuntimeError(f"unexpected {label} layer shape {tuple(W.shape)} (want {(o, i)})")
+    W_all = torch.cat([W.detach().reshape(-1).float() for W in Ws]).contiguous()
+    b_all = torch.cat([b.detach().reshape(-1).float() for b in bs]).contiguous()
+    dev = Ws[0].device
+    packed = _aligned_blob(_size(f"recmv_{net}_packed_bytes"), dev)
+    _launch(f"recmv_{net}_pack_weights", W_all, _ptr(W_all), _ptr(b_all), _ptr(packed))
     return packed
+
+
+def sdf_pack_weights(Ws, bs):
+    """Ws[l] [out,in] effective fp32 weights (weight-norm applied), bs[l] [out] -> packed device blob."""
+    return _pack_weights("sdf", "SDF", SDF_LAYER_SHAPES, Ws, bs)
 
 
 def _pe_array(pe_w):
@@ -659,9 +663,7 @@ def sdf_mlp_forward(x, packed, pe_w=None, mode=None, want_feat=True):
     P = x.shape[0]
     sdf = torch.empty((P, 1), dtype=torch.float32, device=x.device)
     feat = torch.empty((P, 256), dtype=torch.float32, device=x.device) if want_feat else None
-    with torch.cuda.device(x.device):
-        check(_lib.load().recmv_sdf_mlp_fwd(_ptr(x), _ptr(packed), _pe_array(pe_w), _ptr(sdf),
-                                            _ptr(feat), P, mode, _stream(x)), "recmv_sdf_mlp_fwd")
+    _launch("recmv_sdf_mlp_fwd", x, _ptr(x), _ptr(packed), _pe_array(pe_w), _ptr(sdf), _ptr(feat), P, mode)
     return sdf, feat
 
 
@@ -676,9 +678,8 @@ def sdf_value_and_grad(x, packed, pe_w=None, mode=None, want_feat=False):
     sdf = torch.empty((P, 1), dtype=torch.float32, device=x.device)
     grad = torch.empty((P, 3), dtype=torch.float32, device=x.device)
     feat = torch.empty((P, 256), dtype=torch.float32, device=x.device) if want_feat else None
-    with torch.cuda.device(x.device):
-        check(_lib.load().recmv_sdf_mlp_fwd_grad(_ptr(x), _ptr(packed), _pe_array(pe_w), _ptr(sdf), _ptr(feat),
-                                                 _ptr(grad), P, mode, _stream(x)), "recmv_sdf_mlp_fwd_grad")
+    _launch("recmv_sdf_mlp_fwd_grad", x, _ptr(x), _ptr(packed), _pe_array(pe_w), _ptr(sdf), _ptr(feat), _ptr(grad), P,
+            mode)
     return sdf, grad, feat
 
 
@@ -709,6 +710,24 @@ class input_grad_only:
 
 def _inputs_only(need_params):
     return SECOND_ORDER_FUSED and (not need_params or _INPUT_GRAD_ONLY[0] > 0)
+
+
+def _composite_grads(composite, inputs, cotangents):
+    """The create_graph=True backward of a training Function that is not its fused input gradient: differentiate the
+    torch composite `composite(*inputs)` (a tensor or a tuple of them) for the output cotangents with a graph.  An input
+    may be None; a None cotangent skips its output.  Returns one gradient per input, None where it does not require
+    grad."""
+    ins = [t if t is None or t.requires_grad else t.detach() for t in inputs]
+    with torch.enable_grad():
+        outs = composite(*ins)
+        outs = outs if isinstance(outs, tuple) else (outs,)
+        used = [(o, g) for o, g in zip(outs, cotangents) if g is not None]
+        diff = [t for t in ins if t is not None and t.requires_grad]
+        gr = iter(torch.autograd.grad([o for o, _ in used], diff, [g for _, g in used], create_graph=True,
+                                      allow_unused=True))
+    return [next(gr) if t is not None and t.requires_grad else None for t in ins]
+
+
 _INV_SQRT2 = 0.70710678118654752440
 
 
@@ -725,10 +744,8 @@ def pe_forward(x, pe_w, bands, out, out2=None):
     """out[:, :3 + 6 bands] (and out2) = positional encoding of x [P,3] with annealing weights pe_w.  Callers: the
     translator and colour networks' training forwards build their input rows with it."""
     w = (c_float * (2 * bands))(*[float(v) for v in pe_w[:2 * bands]])
-    with torch.cuda.device(x.device):
-        check(_lib.load().recmv_pe_forward(_ptr(x), w, int(bands), _ptr(out), out.stride(0), _ptr(out2),
-                                           out2.stride(0) if out2 is not None else 0, x.shape[0], _stream(x)),
-              "recmv_pe_forward")
+    _launch("recmv_pe_forward", x, _ptr(x), w, int(bands), _ptr(out), out.stride(0), _ptr(out2),
+            out2.stride(0) if out2 is not None else 0, x.shape[0])
     return out
 
 
@@ -749,9 +766,8 @@ def split_planes(t, rows, cols, scale, scale_dev=None, transpose=False, ldp=None
     shape = (cols, ldp) if transpose else (rows, ldp)
     hi = torch.zeros(shape, dtype=torch.float16, device=dev)
     lo = torch.zeros(shape, dtype=torch.float16, device=dev)
-    with torch.cuda.device(dev):
-        check(_lib.load().recmv_split_planes(_ptr(t), t.stride(0), int(rows), int(cols), float(scale), _ptr(scale_dev),
-                                             1 if transpose else 0, _ptr(hi), _ptr(lo), ldp, _stream(t)), "recmv_split_planes")
+    _launch("recmv_split_planes", t, _ptr(t), t.stride(0), int(rows), int(cols), float(scale), _ptr(scale_dev),
+            1 if transpose else 0, _ptr(hi), _ptr(lo), ldp)
     return hi, lo
 
 
@@ -781,10 +797,8 @@ def weight_planes(W, transpose=False):
 
 def pe_forward_planes(x, pe_w, bands, out, out_hi, out_lo):
     w = (c_float * (2 * bands))(*[float(v) for v in pe_w[:2 * bands]])
-    with torch.cuda.device(x.device):
-        check(_lib.load().recmv_pe_forward_planes(_ptr(x), w, int(bands), _ptr(out), out.stride(0) if out is not None else 0,
-                                                  _ptr(out_hi), _ptr(out_lo), out_hi.stride(0), x.shape[0], _stream(x)),
-              "recmv_pe_forward_planes")
+    _launch("recmv_pe_forward_planes", x, _ptr(x), w, int(bands), _ptr(out), out.stride(0) if out is not None else 0,
+            _ptr(out_hi), _ptr(out_lo), out_hi.stride(0), x.shape[0])
 
 
 def mlp_layer_planes(a_planes, b_planes, M, N, K, mode, Y, bias=None, saved_input=None, scale=1.0, dyn=None, a_has_dyn=False,
@@ -794,25 +808,18 @@ def mlp_layer_planes(a_planes, b_planes, M, N, K, mode, Y, bias=None, saved_inpu
     ah, al = a_planes
     bh, bl = b_planes
     yh, yl = y_planes if y_planes is not None else (None, None)
-    with torch.cuda.device(Y.device):
-        check(_lib.load().recmv_mlp_layer_planes(
+    _launch("recmv_mlp_layer_planes", Y,
             _ptr(ah), _ptr(al), ah.stride(0), _ptr(bh), _ptr(bl), bh.stride(0), int(M), int(N), int(K), int(mode), _ptr(bias),
             _ptr(saved_input), saved_input.stride(0) if saved_input is not None else 0, float(scale), _ptr(dyn),
             1 if a_has_dyn else 0, int(split), _ptr(Y), Y.stride(0), _ptr(Y2), Y2.stride(0) if Y2 is not None else 0, _ptr(yh),
-            _ptr(yl), yh.stride(0) if yh is not None else 0, 1 if planes_with_dyn else 0, _stream(Y)), "recmv_mlp_layer_planes")
+            _ptr(yl), yh.stride(0) if yh is not None else 0, 1 if planes_with_dyn else 0)
     return Y
 
 
-_WGRAD_WS = {}
-
-
 def _wgrad_workspace(dev):
-    key = (dev.type, dev.index)
-    if key not in _WGRAD_WS:
-        with torch.cuda.device(dev):
-            n = int(_lib.load().recmv_mlp_wgrad_workspace_floats())
-        _WGRAD_WS[key] = (torch.empty((n,), dtype=torch.float32, device=dev), torch.empty((128 * 512,), dtype=torch.float32, device=dev))
-    return _WGRAD_WS[key]
+    """fp32 scratch of the weight gradient: (the GEMM's split partials, sized for dev's SM count; the colsum partials)."""
+    return (_scratch(dev, "wgrad", _size("recmv_mlp_wgrad_workspace_floats", dev=dev), torch.float32),
+            _scratch(dev, "colsum", 128 * 512, torch.float32))
 
 
 def mlp_wgrad_planes(g_planes, x_planes, P, out_dim, in_dim, scale=1.0, dyn=None, want_bias=False):
@@ -824,10 +831,8 @@ def mlp_wgrad_planes(g_planes, x_planes, P, out_dim, in_dim, scale=1.0, dyn=None
     ws, _ = _wgrad_workspace(dev)
     dW = torch.empty((out_dim, in_dim), dtype=torch.float32, device=dev)
     db = torch.empty((out_dim,), dtype=torch.float32, device=dev) if want_bias else None
-    with torch.cuda.device(dev):
-        check(_lib.load().recmv_mlp_wgrad_planes(_ptr(gh), _ptr(gl), gh.stride(0), _ptr(xh), _ptr(xl), xh.stride(0), int(P),
-                                                 int(out_dim), int(in_dim), float(scale), _ptr(dyn), _ptr(ws), _ptr(dW), _ptr(db),
-                                                 _stream(gh)), "recmv_mlp_wgrad_planes")
+    _launch("recmv_mlp_wgrad_planes", gh, _ptr(gh), _ptr(gl), gh.stride(0), _ptr(xh), _ptr(xl), xh.stride(0), int(P),
+            int(out_dim), int(in_dim), float(scale), _ptr(dyn), _ptr(ws), _ptr(dW), _ptr(db))
     return (dW, db) if want_bias else dW
 
 
@@ -835,28 +840,22 @@ def colsum(G, cols):
     """sum over rows of G[:, :cols] (fp32, deterministic two-stage reduction): the bias gradient."""
     _, part = _wgrad_workspace(G.device)
     out = torch.empty((cols,), dtype=torch.float32, device=G.device)
-    with torch.cuda.device(G.device):
-        check(_lib.load().recmv_colsum(_ptr(G), G.stride(0), G.shape[0], int(cols), _ptr(part), _ptr(out), _stream(G)),
-              "recmv_colsum")
+    _launch("recmv_colsum", G, _ptr(G), G.stride(0), G.shape[0], int(cols), _ptr(part), _ptr(out))
     return out
 
 
 def softplus_tangent_planes(tz, a, h, cols, u, u_planes, inj, plane_scale=64.0):
     """u[:, :cols] = softplus_100'(z) * tz (+ planes), inj[:, :cols] = softplus_100''(z) * (h / softplus') * tz, from the saved
     softplus output a (second_order.py's tangent pass; one launch)."""
-    with torch.cuda.device(tz.device):
-        check(_lib.load().recmv_softplus_tangent_planes(
+    _launch("recmv_softplus_tangent_planes", tz,
             _ptr(tz), tz.stride(0), _ptr(a), a.stride(0), _ptr(h), h.stride(0), tz.shape[0], int(cols), float(plane_scale), _ptr(u),
-            u.stride(0), _ptr(u_planes[0]), _ptr(u_planes[1]), u_planes[0].stride(0), _ptr(inj), inj.stride(0), _stream(tz)),
-            "recmv_softplus_tangent_planes")
+            u.stride(0), _ptr(u_planes[0]), _ptr(u_planes[1]), u_planes[0].stride(0), _ptr(inj), inj.stride(0))
 
 
 def add_split_planes(y, addend, cols, y_planes, scale=64.0, scale_dev=None):
     """y[:, :cols] += addend[:, :cols] in place, and the planes of the sum scaled scale (* scale_dev)."""
-    with torch.cuda.device(y.device):
-        check(_lib.load().recmv_add_split_planes(_ptr(y), y.stride(0), _ptr(addend), addend.stride(0), y.shape[0], int(cols),
-                                                 float(scale), _ptr(scale_dev), _ptr(y_planes[0]), _ptr(y_planes[1]),
-                                                 y_planes[0].stride(0), _stream(y)), "recmv_add_split_planes")
+    _launch("recmv_add_split_planes", y, _ptr(y), y.stride(0), _ptr(addend), addend.stride(0), y.shape[0], int(cols),
+            float(scale), _ptr(scale_dev), _ptr(y_planes[0]), _ptr(y_planes[1]), y_planes[0].stride(0))
 
 
 def pe_backward(x, g, g2, pe_w, bands, dx=None):
@@ -866,9 +865,8 @@ def pe_backward(x, g, g2, pe_w, bands, dx=None):
     if dx is None:
         dx = torch.empty((P, 3), dtype=torch.float32, device=x.device)
     w = (c_float * (2 * bands))(*[float(v) for v in pe_w[:2 * bands]])
-    with torch.cuda.device(x.device):
-        check(_lib.load().recmv_pe_backward(_ptr(x), _ptr(g), g.stride(0), _ptr(g2), g2.stride(0) if g2 is not None else 0,
-                                            w, int(bands), _ptr(dx), 1 if acc else 0, P, _stream(x)), "recmv_pe_backward")
+    _launch("recmv_pe_backward", x, _ptr(x), _ptr(g), g.stride(0), _ptr(g2), g2.stride(0) if g2 is not None else 0, w,
+            int(bands), _ptr(dx), 1 if acc else 0, P)
     return dx
 
 
@@ -960,17 +958,10 @@ class SdfMlpTrainFunction(torch.autograd.Function):
         if torch.is_grad_enabled():
             # create_graph=True with parameter gradients in the graph: differentiate a torch graph of the same network
             SdfMlpTrainFunction.last_backward = "autograd-composite (create_graph)"
-            xi = x if x.requires_grad else x.detach().requires_grad_(need_x)
-            with torch.enable_grad():
-                sdf, feat = _sdf_composite(xi, Ws, bs, ctx.pe_w)
-                ins = [t for t in [xi] + list(Ws) + list(bs) if t.requires_grad]
-                outs, gos = [sdf], [g_sdf if g_sdf is not None else torch.zeros_like(sdf)]
-                if g_feat is not None:
-                    outs.append(feat); gos.append(g_feat)
-                gr = torch.autograd.grad(outs, ins, gos, create_graph=True, allow_unused=True)
-            it = iter(gr)
-            res = [next(it) if t.requires_grad else None for t in [xi] + list(Ws) + list(bs)]
-            return (res[0] if need_x else None, None, None, None, *res[1:])
+            g_sdf = g_sdf if g_sdf is not None else x.new_zeros((P, 1))     # the sdf output is always differentiated
+            res = _composite_grads(lambda x, *Wb: _sdf_composite(x, Wb[:9], Wb[9:], ctx.pe_w), [x, *Ws, *bs],
+                                   [g_sdf, g_feat])
+            return (res[0], None, None, None, *res[1:])
         SdfMlpTrainFunction.last_backward = "fused-tc"
         dyn, _, GP, dpe0, dpe4 = sdf_reverse_chain(g_sdf, g_feat, act, Ws, need_x)
         dx = pe_backward(x, dpe0, dpe4, ctx.pe_w, 6) if need_x else None
@@ -1127,12 +1118,8 @@ class TranslatorTrainFunction(torch.autograd.Function):
             return (dps, dconds, None, None, *([None] * (2 * n)))
         if torch.is_grad_enabled():
             TranslatorTrainFunction.last_backward = "autograd-composite (create_graph)"
-            with torch.enable_grad():
-                x0 = torch.cat([_pe_torch(ps, ctx.pe_w, 6), conds[batch_inds]], 1)
-                out = _plain_composite(x0, Ws, bs)
-                ins = [t for t in [ps, conds] + list(Ws) + list(bs) if t.requires_grad]
-                gr = iter(torch.autograd.grad([out], ins, [g_off], create_graph=True, allow_unused=True))
-            res = [next(gr) if t.requires_grad else None for t in [ps, conds] + list(Ws) + list(bs)]
+            res = _composite_grads(lambda ps, conds, *Wb: _plain_composite(
+                torch.cat([_pe_torch(ps, ctx.pe_w, 6), conds[batch_inds]], 1), Wb[:n], Wb[n:]), [ps, conds, *Ws, *bs], [g_off])
             return (res[0], res[1], None, None, *res[2:])
         TranslatorTrainFunction.last_backward = "fused-tc"
         dX0, dW, db = _plain_mlp_backward(g_off.contiguous().float(), Ws, acts, any(need[4:]), need[0] or need[1], xplanes)
@@ -1182,13 +1169,9 @@ class RenderNetTrainFunction(torch.autograd.Function):
             return (dp, dn, dv, df, None, *([None] * (2 * n)))
         if torch.is_grad_enabled():
             RenderNetTrainFunction.last_backward = "autograd-composite (create_graph)"
-            with torch.enable_grad():
-                x0 = torch.cat([points, _pe_torch(view_dirs, ctx.pe_w, 4), normals, feats], 1)
-                out = _plain_composite(x0, Ws, bs)
-                allin = [points, normals, view_dirs, feats] + list(Ws) + list(bs)
-                ins = [t for t in allin if t.requires_grad]
-                gr = iter(torch.autograd.grad([out], ins, [g_out], create_graph=True, allow_unused=True))
-            res = [next(gr) if t.requires_grad else None for t in allin]
+            res = _composite_grads(lambda p, nrm, v, f, *Wb: _plain_composite(
+                torch.cat([p, _pe_torch(v, ctx.pe_w, 4), nrm, f], 1), Wb[:n], Wb[n:]),
+                [points, normals, view_dirs, feats, *Ws, *bs], [g_out])
             return (*res[:4], None, *res[4:])
         RenderNetTrainFunction.last_backward = "fused-tc"
         dX0, dW, db = _plain_mlp_backward(g_out.contiguous().float(), Ws, acts, any(need[5:]), any(need[:4]), xplanes)
@@ -1207,28 +1190,9 @@ class RenderNetTrainFunction(torch.autograd.Function):
 TRANSLATOR_LAYER_SHAPES = [(512, 167), (512, 512), (512, 512), (512, 512), (3, 512)]
 
 
-def _aligned_blob(nbytes, dev):
-    raw = torch.empty((nbytes + 1024,), dtype=torch.uint8, device=dev)
-    off = (-raw.data_ptr()) % 1024
-    blob = raw[off:off + nbytes]
-    blob._keepalive = raw
-    return blob
-
-
 def translator_pack_weights(Ws, bs):
     """MLPTranslator weights (lin0..lin4, no weight-norm) -> packed fp16 hi/lo panels for the tensor-core engine."""
-    dev = Ws[0].device
-    for (o, i), W, b in zip(TRANSLATOR_LAYER_SHAPES, Ws, bs):
-        if tuple(W.shape) != (o, i) or tuple(b.shape) != (o,):
-            raise RuntimeError(f"unexpected translator layer shape {tuple(W.shape)} (want {(o, i)})")
-    W_all = torch.cat([W.detach().reshape(-1).float() for W in Ws]).contiguous()
-    b_all = torch.cat([b.detach().reshape(-1).float() for b in bs]).contiguous()
-    lib = _lib.load()
-    packed = _aligned_blob(lib.recmv_translator_packed_bytes(), dev)
-    with torch.cuda.device(dev):
-        check(lib.recmv_translator_pack_weights(_ptr(W_all), _ptr(b_all), _ptr(packed), _stream(W_all)),
-              "recmv_translator_pack_weights")
-    return packed
+    return _pack_weights("translator", "translator", TRANSLATOR_LAYER_SHAPES, Ws, bs)
 
 
 def deformer_forward(ps, conds, packed, pe_w, batch_inds=None, points_per_frame=0, skin=None, mode=None,
@@ -1252,18 +1216,13 @@ def deformer_forward(ps, conds, packed, pe_w, batch_inds=None, points_per_frame=
         posed = torch.empty((P, 3), dtype=torch.float32, device=dev)
     if batch_inds is not None:
         batch_inds = batch_inds.contiguous().long()
-    with torch.cuda.device(dev):
-        if want_jacobian:
-            jac = torch.empty((P, 3, 3), dtype=torch.float32, device=dev)
-            check(_lib.load().recmv_deformer_fwd_jac(_ptr(ps), _ptr(conds), _ptr(batch_inds), int(points_per_frame),
-                                                     int(conds.shape[0]), _ptr(packed), _pe_array(pe_w), _ptr(A),
-                                                     _ptr(trans), vox, _ptr(tr), _ptr(off), _ptr(posed), _ptr(jac), P,
-                                                     mode, _stream(ps)), "recmv_deformer_fwd_jac")
-            return tr, off, posed, jac
-        check(_lib.load().recmv_deformer_fwd(_ptr(ps), _ptr(conds), _ptr(batch_inds), int(points_per_frame),
-                                             int(conds.shape[0]), _ptr(packed), _pe_array(pe_w), _ptr(A), _ptr(trans),
-                                             vox, _ptr(tr), _ptr(off), _ptr(posed), P, mode, _stream(ps)),
-              "recmv_deformer_fwd")
+    args = (_ptr(ps), _ptr(conds), _ptr(batch_inds), int(points_per_frame), int(conds.shape[0]), _ptr(packed),
+            _pe_array(pe_w), _ptr(A), _ptr(trans), vox, _ptr(tr), _ptr(off), _ptr(posed))
+    if want_jacobian:
+        jac = torch.empty((P, 3, 3), dtype=torch.float32, device=dev)
+        _launch("recmv_deformer_fwd_jac", ps, *args, _ptr(jac), P, mode)
+        return tr, off, posed, jac
+    _launch("recmv_deformer_fwd", ps, *args, P, mode)
     return tr, off, posed
 
 
@@ -1272,18 +1231,7 @@ RENDERNET_LAYER_SHAPES = [(512, 289), (512, 512), (512, 512), (512, 512), (3, 51
 
 def rendernet_pack_weights(Ws, bs):
     """Effective colour-network weights (weight norm already applied) -> packed fp16 hi/lo panels."""
-    dev = Ws[0].device
-    for (o, i), W, b in zip(RENDERNET_LAYER_SHAPES, Ws, bs):
-        if tuple(W.shape) != (o, i) or tuple(b.shape) != (o,):
-            raise RuntimeError(f"unexpected colour-network layer shape {tuple(W.shape)} (want {(o, i)})")
-    W_all = torch.cat([W.detach().reshape(-1).float() for W in Ws]).contiguous()
-    b_all = torch.cat([b.detach().reshape(-1).float() for b in bs]).contiguous()
-    lib = _lib.load()
-    packed = _aligned_blob(lib.recmv_rendernet_packed_bytes(), dev)
-    with torch.cuda.device(dev):
-        check(lib.recmv_rendernet_pack_weights(_ptr(W_all), _ptr(b_all), _ptr(packed), _stream(W_all)),
-              "recmv_rendernet_pack_weights")
-    return packed
+    return _pack_weights("rendernet", "colour-network", RENDERNET_LAYER_SHAPES, Ws, bs)
 
 
 def rendernet_forward(points, normals, view_dirs, feats, packed, pe_w8, mode=None):
@@ -1297,9 +1245,7 @@ def rendernet_forward(points, normals, view_dirs, feats, packed, pe_w8, mode=Non
         raise RuntimeError("rendernet_forward: expected [P,3] x3 and [P,256]")
     out = torch.empty((P, 3), dtype=torch.float32, device=args[0].device)
     pe = (c_float * 8)(*[float(w) for w in pe_w8])
-    with torch.cuda.device(out.device):
-        check(_lib.load().recmv_rendernet_fwd(*[_ptr(a) for a in args], _ptr(packed), pe, _ptr(out), P, mode,
-                                              _stream(out)), "recmv_rendernet_fwd")
+    _launch("recmv_rendernet_fwd", out, *[_ptr(a) for a in args], _ptr(packed), pe, _ptr(out), P, mode)
     return out
 
 
@@ -1329,12 +1275,9 @@ def render_sdf(ray_dirs, cam_pos, t_near, t_far, samples, A, trans, ws_cl, cente
         frame_of_ray = frame_of_ray.contiguous().to(torch.int32)
     rm = make_raymarch(cam_pos, t_near, t_far, samples)
     vox = make_voxel(ws_cl, center, extend)
-    with torch.cuda.device(dev):
-        check(_lib.load().recmv_render_sdf(_ptr(ray_dirs), byref(rm), _ptr(A), _ptr(trans),
-                                           _ptr(frame_of_ray), int(rays_per_frame), int(A.shape[0]),
-                                           byref(vox), _ptr(packed), _pe_array(pe_w), _ptr(sdf), _ptr(xc),
-                                           _ptr(hit_idx), _ptr(hit_t), R, mode, _stream(ray_dirs)),
-              "recmv_render_sdf")
+    _launch("recmv_render_sdf", ray_dirs, _ptr(ray_dirs), byref(rm), _ptr(A), _ptr(trans), _ptr(frame_of_ray),
+            int(rays_per_frame), int(A.shape[0]), byref(vox), _ptr(packed), _pe_array(pe_w), _ptr(sdf), _ptr(xc),
+            _ptr(hit_idx), _ptr(hit_t), R, mode)
     return sdf, xc, hit_idx, hit_t
 
 
@@ -1348,10 +1291,8 @@ def interp2x_boundary3d_forward(inp, balance_value, order=0):
     N, C, D, H, W = inp.shape
     out = torch.empty((N, C, 2 * D - 1, 2 * H - 1, 2 * W - 1), dtype=torch.float32, device=inp.device)
     flag = torch.empty(out.shape, dtype=torch.uint8, device=inp.device)
-    with torch.cuda.device(inp.device):
-        check(_lib.load().recmv_interp2x_boundary3d_fwd(_ptr(inp), _ptr(out), _ptr(flag), N * C, D, H, W,
-                                                        float(balance_value), int(order), _stream(inp)),
-              "recmv_interp2x_boundary3d_fwd")
+    _launch("recmv_interp2x_boundary3d_fwd", inp, _ptr(inp), _ptr(out), _ptr(flag), N * C, D, H, W, float(balance_value),
+            int(order))
     return [out, flag.view(torch.bool)]
 
 
@@ -1363,9 +1304,7 @@ def interp2x_boundary3d_backward(grad_output):
     N, C, d, h, w = grad_output.shape
     D, H, W = (d + 1) // 2, (h + 1) // 2, (w + 1) // 2
     gi = torch.empty((N, C, D, H, W), dtype=torch.float32, device=grad_output.device)
-    with torch.cuda.device(gi.device):
-        check(_lib.load().recmv_interp2x_boundary3d_bwd(_ptr(grad_output), _ptr(gi), N * C, D, H, W, _stream(gi)),
-              "recmv_interp2x_boundary3d_bwd")
+    _launch("recmv_interp2x_boundary3d_bwd", gi, _ptr(grad_output), _ptr(gi), N * C, D, H, W)
     return gi
 
 
@@ -1375,9 +1314,8 @@ def c2f_todo_mask(is_boundary, done):
     _check_input(done, "done")
     D, H, W = is_boundary.shape
     todo = torch.empty((D, H, W), dtype=torch.uint8, device=done.device)
-    with torch.cuda.device(done.device):
-        check(_lib.load().recmv_c2f_todo_mask(_ptr(is_boundary.view(torch.uint8)), _ptr(done.view(torch.uint8)),
-                                              _ptr(todo), D, H, W, _stream(todo)), "recmv_c2f_todo_mask")
+    _launch("recmv_c2f_todo_mask", todo, _ptr(is_boundary.view(torch.uint8)), _ptr(done.view(torch.uint8)), _ptr(todo),
+            D, H, W)
     return todo.view(torch.bool)
 
 
@@ -1393,15 +1331,13 @@ def fragment_decode(pix_to_face, bary, verts, faces, mask=None, camera=None):
     verts = verts.detach().contiguous().float()
     faces = faces.contiguous().long()
     npix = N * H * W
-    for t, name in ((bary, "bary"), (verts, "verts"), (faces, "faces"), (mask, "mask")):
+    _expect("fragment_decode", "bary", bary, torch.float32, (N, H, W, K, 3), dev)
+    for t, name in ((verts, "verts"), (faces, "faces"), (mask, "mask")):
         if t is not None and t.device != dev:
             raise RuntimeError(f"fragment_decode: {name} must be on {dev}, got {t.device}")
-    if tuple(bary.shape) != (N, H, W, K, 3):
-        raise RuntimeError(f"fragment_decode: bary must have shape {(N, H, W, K, 3)}, got {tuple(bary.shape)}")
     if mask is not None and mask.numel() != npix:
         raise RuntimeError(f"fragment_decode: mask must have {npix} elements (N*H*W), got {mask.numel()}")
-    lib = _lib.load()
-    scratch = torch.empty((lib.recmv_fragment_decode_scratch_bytes(npix),), dtype=torch.uint8, device=dev)
+    scratch = torch.empty((_size("recmv_fragment_decode_scratch_bytes", npix),), dtype=torch.uint8, device=dev)
     ob, orow, ocol, ofi = (torch.empty((npix,), dtype=torch.int64, device=dev) for _ in range(4))
     opts = torch.empty((npix, 3), dtype=torch.float32, device=dev)
     orays = torch.empty((npix, 3), dtype=torch.float32, device=dev) if camera is not None else None
@@ -1412,16 +1348,12 @@ def fragment_decode(pix_to_face, bary, verts, faces, mask=None, camera=None):
     counters = torch.zeros((1,), dtype=torch.int32, device=dev)
     if mask is not None:
         mask = mask.contiguous().float()
-    with torch.cuda.device(dev):
-        check(lib.recmv_fragment_decode(_ptr(pix_to_face), _ptr(bary), N, H, W, K, _ptr(verts), _ptr(faces), int(faces.shape[0]),
-                                        _ptr(mask), cam, _ptr(scratch), _ptr(ob), _ptr(orow), _ptr(ocol), _ptr(opts), _ptr(ofi),
-                                        _ptr(orays), _ptr(counters), _stream(bary)), "recmv_fragment_decode")
+    _launch("recmv_fragment_decode", bary, _ptr(pix_to_face), _ptr(bary), N, H, W, K, _ptr(verts), _ptr(faces),
+            int(faces.shape[0]), _ptr(mask), cam, _ptr(scratch), _ptr(ob), _ptr(orow), _ptr(ocol), _ptr(opts), _ptr(ofi),
+            _ptr(orays), _ptr(counters))
     n = int(counters.item())
     out = (ob[:n], orow[:n], ocol[:n], opts[:n], ofi[:n])
     return out + (orays[:n],) if camera is not None else out
-
-
-_raster_state = {}   # per device: grow-only workspace (its pair-list capacity) + counters and their pinned host copy
 
 
 def rasterize_meshes(verts, faces, cameras, H, W, z_clip=1e-6, area_eps=1e-8, want_dists=True, capacity=None,
@@ -1437,65 +1369,44 @@ def rasterize_meshes(verts, faces, cameras, H, W, z_clip=1e-6, area_eps=1e-8, wa
     for t, name in ((verts, "verts"), (faces, "faces"), (cameras, "cameras")):
         _check_input(t, name)
     dev = verts.device
-    if faces.device != dev or cameras.device != dev:
-        raise RuntimeError(f"rasterize_meshes: faces and cameras must be on {dev}")
-    if verts.dtype != torch.float32 or verts.dim() != 3 or verts.shape[2] != 3:
-        raise RuntimeError(f"rasterize_meshes: verts must be float32 [N,V,3], got {verts.dtype} {tuple(verts.shape)}")
-    if faces.dtype != torch.int64 or faces.dim() != 2 or faces.shape[1] != 3:
-        raise RuntimeError(f"rasterize_meshes: faces must be int64 [F,3], got {faces.dtype} {tuple(faces.shape)}")
+    _expect("rasterize_meshes", "verts", verts, torch.float32, ("N", "V", 3))
+    _expect("rasterize_meshes", "faces", faces, torch.int64, ("F", 3), dev)
     N, V = int(verts.shape[0]), int(verts.shape[1])
     F = int(faces.shape[0])
-    if cameras.dtype != torch.float32 or tuple(cameras.shape) != (N, 16):
-        raise RuntimeError(f"rasterize_meshes: cameras must be float32 [{N},16], got {cameras.dtype} {tuple(cameras.shape)}")
+    _expect("rasterize_meshes", "cameras", cameras, torch.float32, (N, 16), dev)
     H, W = int(H), int(W)
-    lib = _lib.load()
-    st = _raster_state.setdefault(dev.index, {})
-    if st.get("counters") is None:
-        st["counters"] = torch.zeros((20,), dtype=torch.int32, device=dev)       # 4 counters + 16 camera floats
-        st["counters_host"] = torch.zeros((20,), dtype=torch.int32).pin_memory()
-    cap = int(capacity) if capacity is not None else max(st.get("capacity", 0), 2 * N * F + 4096)
+    ctr, host = _counters(dev, "raster_counters", 20)       # 4 counters + 16 camera floats
+    kept = (dev.index, "raster_pairs")
+    cap = int(capacity) if capacity is not None else max(_scratch_cache.get(kept, 0), 2 * N * F + 4096)
     p2f = torch.empty((N, H, W, 1), dtype=torch.int64, device=dev)
     zbuf = torch.empty((N, H, W, 1), dtype=torch.float32, device=dev)
     bary = torch.empty((N, H, W, 1, 3), dtype=torch.float32, device=dev)
     dists = torch.empty((N, H, W, 1), dtype=torch.float32, device=dev) if want_dists else None
-    ctr = st["counters"]
-    with torch.cuda.device(dev):
-        stream = _stream(verts)
-        for _ in range(2):
-            nbytes = c_size_t(0)
-            check(lib.recmv_raster_workspace_bytes(N, F, H, W, cap, byref(nbytes)), "recmv_raster_workspace_bytes")
-            if st.get("ws") is None or st["ws"].numel() < nbytes.value:
-                st["ws"] = torch.empty((nbytes.value,), dtype=torch.uint8, device=dev)
-            st["capacity"] = max(st.get("capacity", 0), cap)
-            check(lib.recmv_rasterize_meshes(_ptr(verts), V, _ptr(faces), F, N, _ptr(cameras), H, W, float(z_clip),
-                                             float(area_eps), _ptr(st["ws"]), cap, _ptr(p2f), _ptr(zbuf), _ptr(bary),
-                                             _ptr(dists), _ptr(ctr), stream), "recmv_rasterize_meshes")
-            if host_camera and N > 0:
-                ctr[4:].copy_(cameras[0].view(torch.int32))
-            st["counters_host"].copy_(ctr, non_blocking=True)
-            torch.cuda.current_stream(dev).synchronize()
-            covered, skipped, pairs, overflow = (int(v) for v in st["counters_host"][:4])
-            if not overflow:
-                break
-            if pairs >= 0x7fffffff:
-                check(_lib.RECMV_E_RANGE, "recmv_rasterize_meshes (more than 2^31 - 1 tile / face pairs)")
-            cap = pairs   # grow once to the exact size, re-run (the workspace is kept for later calls)
-        else:
-            raise _lib.RecmvError("recmv_rasterize_meshes: pair list still too small after growing")
+    for _ in range(2):
+        ws = _scratch(dev, "raster_ws", _size("recmv_raster_workspace_bytes", N, F, H, W, cap))
+        _scratch_cache[kept] = max(_scratch_cache.get(kept, 0), cap)
+        _launch("recmv_rasterize_meshes", verts, _ptr(verts), V, _ptr(faces), F, N, _ptr(cameras), H, W, float(z_clip),
+                float(area_eps), _ptr(ws), cap, _ptr(p2f), _ptr(zbuf), _ptr(bary), _ptr(dists), _ptr(ctr))
+        if host_camera and N > 0:
+            ctr[4:].copy_(cameras[0].view(torch.int32))
+        covered, skipped, pairs, overflow = (int(v) for v in _read_counters(ctr, host)[:4])
+        if not overflow:
+            break
+        if pairs >= 0x7fffffff:
+            check(_lib.RECMV_E_RANGE, "recmv_rasterize_meshes (more than 2^31 - 1 tile / face pairs)")
+        cap = pairs   # grow once to the exact size, re-run (the workspace is kept for later calls)
+    else:
+        raise _lib.RecmvError("recmv_rasterize_meshes: pair list still too small after growing")
     counts = {"covered": covered, "skipped": skipped, "pairs": pairs}
     if host_camera:
-        counts["camera"] = st["counters_host"][4:].view(torch.float32).clone()
+        counts["camera"] = host[4:].view(torch.float32).clone()
     return p2f, zbuf, bary, dists, counts
-
-
-_points_state = {}   # per device: the pair-list capacity of the first attempt + counters and their pinned host copy
 
 
 def _points_dims(points, features, K, split_size):
     """(N, P, split) of a rasterize_points call; split_size None = P (every point in the first image)."""
     _check_input(points, "points")
-    if points.dtype != torch.float32 or points.dim() != 3 or points.shape[2] != 3:
-        raise RuntimeError(f"rasterize_points: points must be float32 [N,P,3], got {points.dtype} {tuple(points.shape)}")
+    _expect("rasterize_points", "points", points, torch.float32, ("N", "P", 3))
     N, P = int(points.shape[0]), int(points.shape[1])
     if features is not None:
         _check_operand(features, points, (N, P), "features")
@@ -1521,37 +1432,25 @@ def rasterize_points(points, features, H, W, radius, K, split_size=None, want_fr
     N, P, split = _points_dims(points, features, K, split_size)
     H, W, K = int(H), int(W), int(K)
     dev = points.device
-    lib = _lib.load()
-    st = _points_state.setdefault(dev.index, {})
-    if st.get("counters") is None:
-        st["counters"] = torch.zeros((4,), dtype=torch.int32, device=dev)
-        st["counters_host"] = torch.zeros((4,), dtype=torch.int32).pin_memory()
-    cap = int(capacity) if capacity is not None else max(st.get("capacity", 0), 8 * N * P + 4096)
+    ctr, host = _counters(dev, "points_counters", 4)
+    kept = (dev.index, "points_pairs")
+    cap = int(capacity) if capacity is not None else max(_scratch_cache.get(kept, 0), 8 * N * P + 4096)
     images = torch.empty((G, N, H, W), dtype=torch.float32, device=dev)
     frags = tuple(torch.empty((N, H, W, K), dtype=dt, device=dev) for dt in (torch.int64, torch.float32, torch.float32)) \
         if want_fragments else None
-    ctr = st["counters"]
-    with torch.cuda.device(dev):
-        stream = _stream(points)
-        for _ in range(2):
-            nbytes = c_size_t(0)
-            check(lib.recmv_points_raster_workspace_bytes(N, P, H, W, cap, byref(nbytes)),
-                  "recmv_points_raster_workspace_bytes")
-            ws = torch.empty((nbytes.value,), dtype=torch.uint8, device=dev)
-            check(lib.recmv_rasterize_points(_ptr(points), _ptr(features), N, P, H, W, float(radius), K, split, G,
-                                             _ptr(ws), cap, _ptr(images), *(_ptr(t) for t in (frags or (None,) * 3)),
-                                             _ptr(ctr), stream), "recmv_rasterize_points")
-            st["counters_host"].copy_(ctr, non_blocking=True)
-            torch.cuda.current_stream(dev).synchronize()
-            covered, skipped, pairs, overflow = (int(v) for v in st["counters_host"])
-            st["capacity"] = max(st.get("capacity", 0), pairs)
-            if not overflow:
-                break
-            if pairs >= 0x7fffffff:
-                check(_lib.RECMV_E_RANGE, "recmv_rasterize_points (more than 2^31 - 1 tile / point pairs)")
-            cap = pairs   # grow once to the exact size and re-run
-        else:
-            raise _lib.RecmvError("recmv_rasterize_points: pair list still too small after growing")
+    for _ in range(2):
+        ws = torch.empty((_size("recmv_points_raster_workspace_bytes", N, P, H, W, cap),), dtype=torch.uint8, device=dev)
+        _launch("recmv_rasterize_points", points, _ptr(points), _ptr(features), N, P, H, W, float(radius), K, split, G,
+                _ptr(ws), cap, _ptr(images), *(_ptr(t) for t in (frags or (None,) * 3)), _ptr(ctr))
+        covered, skipped, pairs, overflow = (int(v) for v in _read_counters(ctr, host))
+        _scratch_cache[kept] = max(_scratch_cache.get(kept, 0), pairs)
+        if not overflow:
+            break
+        if pairs >= 0x7fffffff:
+            check(_lib.RECMV_E_RANGE, "recmv_rasterize_points (more than 2^31 - 1 tile / point pairs)")
+        cap = pairs   # grow once to the exact size and re-run
+    else:
+        raise _lib.RecmvError("recmv_rasterize_points: pair list still too small after growing")
     counts = {"covered": covered, "skipped": skipped, "pairs": pairs}
     return images, frags, counts, ws
 
@@ -1563,15 +1462,11 @@ def rasterize_points_backward(grad_images, ws, pairs, N, P, H, W, radius, K, spl
     split = P if split_size is None else int(split_size)
     dev = ws.device
     grad_images = grad_images.contiguous().float()
-    if grad_images.device != dev or tuple(grad_images.shape) != (G, N, H, W):
-        raise RuntimeError(f"rasterize_points_backward: grad_images must be [{G},{N},{H},{W}] on {dev}, got "
-                           f"{tuple(grad_images.shape)} on {grad_images.device}")
+    _expect("rasterize_points_backward", "grad_images", grad_images, torch.float32, (G, N, H, W), dev)
     grad = torch.empty((N, P, 3), dtype=torch.float32, device=dev)
     scratch = torch.empty((max(int(pairs), 1), 2), dtype=torch.float32, device=dev)
-    with torch.cuda.device(dev):
-        check(_lib.load().recmv_rasterize_points_backward(N, P, H, W, float(radius), int(K), split, G, _ptr(ws), int(pairs),
-                                                          _ptr(grad_images), _ptr(scratch), _ptr(grad),
-                                                          _stream(grad_images)), "recmv_rasterize_points_backward")
+    _launch("recmv_rasterize_points_backward", grad_images, N, P, H, W, float(radius), int(K), split, G, _ptr(ws), int(pairs),
+            _ptr(grad_images), _ptr(scratch), _ptr(grad))
     return grad
 
 
@@ -1598,8 +1493,6 @@ class RasterizePointsFunction(torch.autograd.Function):
         return g, None, None, None, None, None, None, None
 
 
-_normals_state = {}   # per device: grow-only workspace of the vertex-normal incidence sort
-
 SHADE_PARAMS = 28     # per-frame constants of recmv_shade_phong (include/recmv_b200.h)
 
 
@@ -1610,23 +1503,12 @@ def vertex_normals(verts, faces):
     for t, name in ((verts, "verts"), (faces, "faces")):
         _check_input(t, name)
     dev = verts.device
-    if faces.device != dev:
-        raise RuntimeError(f"vertex_normals: faces must be on {dev}")
-    if verts.dtype != torch.float32 or verts.dim() != 3 or verts.shape[2] != 3:
-        raise RuntimeError(f"vertex_normals: verts must be float32 [N,V,3], got {verts.dtype} {tuple(verts.shape)}")
-    if faces.dtype != torch.int64 or faces.dim() != 2 or faces.shape[1] != 3:
-        raise RuntimeError(f"vertex_normals: faces must be int64 [F,3], got {faces.dtype} {tuple(faces.shape)}")
+    _expect("vertex_normals", "verts", verts, torch.float32, ("N", "V", 3))
+    _expect("vertex_normals", "faces", faces, torch.int64, ("F", 3), dev)
     N, V, F = int(verts.shape[0]), int(verts.shape[1]), int(faces.shape[0])
     out = torch.empty((N, V, 3), dtype=torch.float32, device=dev)
-    lib = _lib.load()
-    st = _normals_state.setdefault(dev.index, {})
-    with torch.cuda.device(dev):
-        nbytes = c_size_t(0)
-        check(lib.recmv_vertex_normals_workspace_bytes(V, F, byref(nbytes)), "recmv_vertex_normals_workspace_bytes")
-        if st.get("ws") is None or st["ws"].numel() < max(nbytes.value, 1):
-            st["ws"] = torch.empty((max(nbytes.value, 1),), dtype=torch.uint8, device=dev)
-        check(lib.recmv_vertex_normals(_ptr(verts), N, V, _ptr(faces), F, _ptr(st["ws"]), _ptr(out), _stream(verts)),
-              "recmv_vertex_normals")
+    ws = _scratch(dev, "normals_ws", max(_size("recmv_vertex_normals_workspace_bytes", V, F, dev=dev), 1))
+    _launch("recmv_vertex_normals", verts, _ptr(verts), N, V, _ptr(faces), F, _ptr(ws), _ptr(out))
     return out
 
 
@@ -1641,53 +1523,27 @@ def shade_phong(frags, verts, normals, colors, faces, params):
                     (faces, "faces"), (params, "params")) + (((colors, "colors"),) if colors is not None else ()):
         _check_input(t, name)
     dev = verts.device
-    if p2f.dtype != torch.int64 or p2f.dim() != 4 or p2f.shape[3] != 1:
-        raise RuntimeError(f"shade_phong: pix_to_face must be int64 [N,H,W,1], got {p2f.dtype} {tuple(p2f.shape)}")
+    _expect("shade_phong", "pix_to_face", p2f, torch.int64, ("N", "H", "W", 1), dev)
     N, H, W = (int(s) for s in p2f.shape[:3])
-    if bary.dtype != torch.float32 or tuple(bary.shape) != (N, H, W, 1, 3):
-        raise RuntimeError(f"shade_phong: bary_coords must be float32 [{N},{H},{W},1,3], got {bary.dtype} "
-                           f"{tuple(bary.shape)}")
-    if verts.dtype != torch.float32 or verts.dim() != 3 or verts.shape[0] != N or verts.shape[2] != 3:
-        raise RuntimeError(f"shade_phong: verts must be float32 [{N},V,3], got {verts.dtype} {tuple(verts.shape)}")
+    _expect("shade_phong", "bary_coords", bary, torch.float32, (N, H, W, 1, 3), dev)
+    _expect("shade_phong", "verts", verts, torch.float32, (N, "V", 3))
     V = int(verts.shape[1])
     for t, name in ((normals, "normals"), (colors, "colors")):
-        if t is not None and (t.dtype != torch.float32 or tuple(t.shape) != (N, V, 3)):
-            raise RuntimeError(f"shade_phong: {name} must be float32 [{N},{V},3], got {t.dtype} {tuple(t.shape)}")
-    if faces.dtype != torch.int64 or faces.dim() != 2 or faces.shape[1] != 3:
-        raise RuntimeError(f"shade_phong: faces must be int64 [F,3], got {faces.dtype} {tuple(faces.shape)}")
-    if params.dtype != torch.float32 or tuple(params.shape) != (N, SHADE_PARAMS):
-        raise RuntimeError(f"shade_phong: params must be float32 [{N},{SHADE_PARAMS}], got {params.dtype} "
-                           f"{tuple(params.shape)}")
-    for t in (p2f, bary, normals, faces, params, colors):
-        if t is not None and t.device != dev:
-            raise RuntimeError(f"shade_phong: every input must be on {dev}")
+        if t is not None:
+            _expect("shade_phong", name, t, torch.float32, (N, V, 3), dev)
+    _expect("shade_phong", "faces", faces, torch.int64, ("F", 3), dev)
+    _expect("shade_phong", "params", params, torch.float32, (N, SHADE_PARAMS), dev)
     out = torch.empty((N, H, W, 4), dtype=torch.float32, device=dev)
-    with torch.cuda.device(dev):
-        check(_lib.load().recmv_shade_phong(_ptr(p2f), _ptr(bary), N, H, W, _ptr(verts), _ptr(normals), _ptr(colors), V,
-                                            _ptr(faces), int(faces.shape[0]), _ptr(params), _ptr(out), _stream(verts)),
-              "recmv_shade_phong")
+    _launch("recmv_shade_phong", verts, _ptr(p2f), _ptr(bary), N, H, W, _ptr(verts), _ptr(normals), _ptr(colors), V,
+            _ptr(faces), int(faces.shape[0]), _ptr(params), _ptr(out))
     return out
-
-
-_knn_state = {}   # per device: grow-only workspace of the nearest-neighbour split minima and the backward's sort
-
-
-def _knn_workspace(dev, N, P1, P2):
-    nbytes = c_size_t(0)
-    check(_lib.load().recmv_knn_workspace_bytes(N, P1, P2, byref(nbytes)), "recmv_knn_workspace_bytes")
-    st = _knn_state.setdefault(dev.index, {})
-    if st.get("ws") is None or st["ws"].numel() < max(nbytes.value, 1):
-        st["ws"] = torch.empty((max(nbytes.value, 1),), dtype=torch.uint8, device=dev)
-    return st["ws"]
 
 
 def _knn_lengths(lengths, N, dev, name):
     if lengths is None:
         return None
     _check_input(lengths, name)
-    if lengths.dtype != torch.int64 or tuple(lengths.shape) != (N,) or lengths.device != dev:
-        raise RuntimeError(f"knn_nearest: {name} must be int64 [{N}] on {dev}, got {lengths.dtype} "
-                           f"{tuple(lengths.shape)} on {lengths.device}")
+    _expect("knn_nearest", name, lengths, torch.int64, (N,), dev)
     return lengths
 
 
@@ -1701,16 +1557,13 @@ def knn_nearest(p1, p2, lengths1=None, lengths2=None):
             raise RuntimeError(f"knn_nearest: {name} must be float32 [N,P,2|3], got {t.dtype} {tuple(t.shape)}")
     dev = p1.device
     N, P1, D = (int(s) for s in p1.shape)
-    if p2.device != dev or p2.shape[0] != N or p2.shape[2] != D:
-        raise RuntimeError(f"knn_nearest: p2 must be [{N},P2,{D}] on {dev}, got {tuple(p2.shape)} on {p2.device}")
+    _expect("knn_nearest", "p2", p2, torch.float32, (N, "P2", D), dev)
     P2 = int(p2.shape[1])
     l1, l2 = _knn_lengths(lengths1, N, dev, "lengths1"), _knn_lengths(lengths2, N, dev, "lengths2")
     dists = torch.empty((N, P1), dtype=torch.float32, device=dev)
     idx = torch.empty((N, P1), dtype=torch.int64, device=dev)
-    with torch.cuda.device(dev):
-        ws = _knn_workspace(dev, N, P1, P2)
-        check(_lib.load().recmv_knn_nearest(_ptr(p1), _ptr(p2), _ptr(l1), _ptr(l2), N, P1, P2, D, _ptr(ws), _ptr(dists),
-                                            _ptr(idx), _stream(p1)), "recmv_knn_nearest")
+    ws = _scratch(dev, "knn_ws", max(_size("recmv_knn_workspace_bytes", N, P1, P2, dev=dev), 1))
+    _launch("recmv_knn_nearest", p1, _ptr(p1), _ptr(p2), _ptr(l1), _ptr(l2), N, P1, P2, D, _ptr(ws), _ptr(dists), _ptr(idx))
     return dists, idx
 
 
@@ -1721,16 +1574,12 @@ def knn_nearest_backward(p1, p2, idx, grad_dists, need_p2=True):
     P2 = int(p2.shape[1])
     dev = p1.device
     grad_dists = grad_dists.contiguous().float()
-    if grad_dists.device != dev or tuple(grad_dists.shape) != (N, P1):
-        raise RuntimeError(f"knn_nearest_backward: grad_dists must be [{N},{P1}] on {dev}, got "
-                           f"{tuple(grad_dists.shape)} on {grad_dists.device}")
+    _expect("knn_nearest_backward", "grad_dists", grad_dists, torch.float32, (N, P1), dev)
     g1 = torch.empty((N, P1, D), dtype=torch.float32, device=dev)
     g2 = torch.empty((N, P2, D), dtype=torch.float32, device=dev) if need_p2 else None
-    with torch.cuda.device(dev):
-        ws = _knn_workspace(dev, N, P1, P2)
-        check(_lib.load().recmv_knn_nearest_backward(_ptr(p1), _ptr(p2), _ptr(idx), _ptr(grad_dists), N, P1, P2, D,
-                                                     _ptr(ws), _ptr(g1), _ptr(g2), _stream(p1)),
-              "recmv_knn_nearest_backward")
+    ws = _scratch(dev, "knn_ws", max(_size("recmv_knn_workspace_bytes", N, P1, P2, dev=dev), 1))
+    _launch("recmv_knn_nearest_backward", p1, _ptr(p1), _ptr(p2), _ptr(idx), _ptr(grad_dists), N, P1, P2, D, _ptr(ws),
+            _ptr(g1), _ptr(g2))
     return g1, g2
 
 
@@ -1784,37 +1633,29 @@ class C2fLevel:
         occ_f = torch.empty((1, 1, self.D, self.H, self.W), dtype=torch.float32, device=self.dev)
         done_f = torch.empty((self.D, self.H, self.W), dtype=torch.uint8, device=self.dev)
         D, H, W = self.coarse
-        with torch.cuda.device(self.dev):
-            check(_lib.load().recmv_c2f_refine(_ptr(occ_coarse), _ptr(done_coarse), D, H, W, self.final, self.bmin, self.bmax,
-                                               float(balance), int(order), _ptr(self.mixed), _ptr(occ_f), _ptr(done_f),
-                                               _ptr(self.idx), _ptr(self.pts), _ptr(self.ctr), self.cap, _stream(occ_f)),
-                  "recmv_c2f_refine")
+        _launch("recmv_c2f_refine", occ_f, _ptr(occ_coarse), _ptr(done_coarse), D, H, W, self.final, self.bmin, self.bmax,
+                float(balance), int(order), _ptr(self.mixed), _ptr(occ_f), _ptr(done_f), _ptr(self.idx), _ptr(self.pts),
+                _ptr(self.ctr), self.cap)
         return occ_f, done_f
 
     def evaluate(self, packed, pe_w, mode, occ, done_u8, calculated_u8, balance):
         """SDF on the current worklist, scatter, conflicts -> the other conflict list."""
-        lib = _lib.load()
         self.cur ^= 1
         cc = self.ctr[2 + self.cur:3 + self.cur]
-        with torch.cuda.device(self.dev):
-            st = _stream(occ)
-            check(lib.recmv_sdf_mlp_fwd_counted(_ptr(self.pts), _ptr(packed), _pe_array(pe_w), _ptr(self.vals), None,
-                                                self.cap, _ptr(self.ctr), mode, st), "recmv_sdf_mlp_fwd_counted")
-            cc.zero_()
-            check(lib.recmv_c2f_scatter_list(_ptr(self.idx), _ptr(self.vals), _ptr(self.ctr), self.cap, self.level,
-                                             self.final, _ptr(occ), _ptr(done_u8), _ptr(calculated_u8), _ptr(self.claim),
-                                             float(balance), _ptr(self.clist[self.cur]), _ptr(cc), _ptr(self.ctr[4:5]), st),
-                  "recmv_c2f_scatter_list")
+        _launch("recmv_sdf_mlp_fwd_counted", occ, _ptr(self.pts), _ptr(packed), _pe_array(pe_w), _ptr(self.vals), None,
+                self.cap, _ptr(self.ctr), mode)
+        cc.zero_()
+        _launch("recmv_c2f_scatter_list", occ, _ptr(self.idx), _ptr(self.vals), _ptr(self.ctr), self.cap, self.level,
+                self.final, _ptr(occ), _ptr(done_u8), _ptr(calculated_u8), _ptr(self.claim), float(balance),
+                _ptr(self.clist[self.cur]), _ptr(cc), _ptr(self.ctr[4:5]))
 
     def next_from_conflicts(self, calculated_u8):
         """Worklist of the next round from the conflict list the last evaluate() filled."""
         cc = self.ctr[2 + self.cur:3 + self.cur]
-        with torch.cuda.device(self.dev):
-            self.ctr[0:1].zero_()
-            check(_lib.load().recmv_c2f_mark_conflicts(_ptr(self.clist[self.cur]), _ptr(cc), self.cap, _ptr(calculated_u8),
-                                                       self.level, self.final, self.bmin, self.bmax, _ptr(self.claim),
-                                                       _ptr(self.idx), _ptr(self.pts), _ptr(self.ctr), self.cap,
-                                                       _stream(calculated_u8)), "recmv_c2f_mark_conflicts")
+        self.ctr[0:1].zero_()
+        _launch("recmv_c2f_mark_conflicts", calculated_u8, _ptr(self.clist[self.cur]), _ptr(cc), self.cap,
+                _ptr(calculated_u8), self.level, self.final, self.bmin, self.bmax, _ptr(self.claim), _ptr(self.idx),
+                _ptr(self.pts), _ptr(self.ctr), self.cap)
 
     def read(self):
         """(queried so far, conflicts of the last round, overflow) -- the level's host synchronisation."""
@@ -1836,17 +1677,14 @@ def surface_solve(cam_pos, rays, seeds, batch_inds, sdf_packed, sdf_pe_w, tr_pac
     A, trans, ws_cl, center, extend = skin
     A, trans, conds = A.contiguous().float(), trans.contiguous().float(), conds.contiguous().float()
     bi = batch_inds.contiguous().long() if batch_inds is not None else None
-    lib = _lib.load()
-    wsz = lib.recmv_surface_solve_workspace(P)
+    wsz = _size("recmv_surface_solve_workspace", P)
     work = torch.empty((max(wsz, 1),), dtype=torch.uint8, device=dev)
     ok = torch.empty((P,), dtype=torch.uint8, device=dev)
     cam = (c_float * 3)(*[float(v) for v in cam_pos.view(-1).tolist()])
-    with torch.cuda.device(dev):
-        check(lib.recmv_surface_solve(cam, _ptr(rays), _ptr(ps), _ptr(bi), _ptr(sdf_packed), _pe_array(sdf_pe_w),
-                                      _ptr(tr_packed), _pe_array(tr_pe_w), _ptr(conds), int(conds.shape[0]), _ptr(A),
-                                      _ptr(trans), byref(make_voxel(ws_cl, center, extend)), float(dthreshold),
-                                      float(athreshold), float(w1), float(w2), int(times), mode, _ptr(work), wsz,
-                                      _ptr(ok), P, _stream(ps)), "recmv_surface_solve")
+    _launch("recmv_surface_solve", ps, cam, _ptr(rays), _ptr(ps), _ptr(bi), _ptr(sdf_packed), _pe_array(sdf_pe_w),
+            _ptr(tr_packed), _pe_array(tr_pe_w), _ptr(conds), int(conds.shape[0]), _ptr(A), _ptr(trans),
+            byref(make_voxel(ws_cl, center, extend)), float(dthreshold), float(athreshold), float(w1), float(w2), int(times),
+            mode, _ptr(work), wsz, _ptr(ok), P)
     return ps, ok.view(torch.bool)
 
 
@@ -1865,9 +1703,8 @@ def surface_grad_coeffs(grad_l_p, grad_f_p, jac, rays, d_minus_c=None):
     vec = torch.empty((n, 3), dtype=torch.float32, device=dev)
     rg = torch.empty((n, 3), dtype=torch.float32, device=dev) if dc is not None else None
     ok = torch.empty((n,), dtype=torch.uint8, device=dev)
-    with torch.cuda.device(dev):
-        check(_lib.load().recmv_surface_grad_coeffs(*[_ptr(a) for a in args], _ptr(dc), _ptr(coef), _ptr(vec), _ptr(rg),
-                                                    _ptr(ok), n, _stream(coef)), "recmv_surface_grad_coeffs")
+    _launch("recmv_surface_grad_coeffs", coef, *[_ptr(a) for a in args], _ptr(dc), _ptr(coef), _ptr(vec), _ptr(rg), _ptr(ok),
+            n)
     return coef, vec, rg, ok.view(torch.bool)
 
 
@@ -1886,8 +1723,7 @@ class Svd3x3Function(torch.autograd.Function):
         U = torch.empty((N, 3, 3), dtype=torch.float32, device=J.device)
         V = torch.empty((N, 3, 3), dtype=torch.float32, device=J.device)
         S = torch.empty((N, 3), dtype=torch.float32, device=J.device)
-        with torch.cuda.device(J.device):
-            check(_lib.load().recmv_svd3x3(_ptr(J), N, _ptr(U), _ptr(S), _ptr(V), _stream(J)), "recmv_svd3x3")
+        _launch("recmv_svd3x3", J, _ptr(J), N, _ptr(U), _ptr(S), _ptr(V))
         ctx.save_for_backward(U, V)
         ctx.set_materialize_grads(False)
         ctx.mark_non_differentiable(U, V)
@@ -1903,9 +1739,7 @@ class Svd3x3Function(torch.autograd.Function):
         U, V = ctx.saved_tensors
         gS = gS.contiguous().float()
         dJ = torch.empty_like(U)
-        with torch.cuda.device(U.device):
-            check(_lib.load().recmv_svd3x3_backward_s(_ptr(U), _ptr(V), _ptr(gS), U.shape[0], _ptr(dJ), _stream(U)),
-                  "recmv_svd3x3_backward_s")
+        _launch("recmv_svd3x3_backward_s", U, _ptr(U), _ptr(V), _ptr(gS), U.shape[0], _ptr(dJ))
         return dJ
 
 

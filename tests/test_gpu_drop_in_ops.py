@@ -426,7 +426,7 @@ def test_marching_cubes_dense_grid_matches_oracle():
     corners = [s[i:i + shape[0] - 1, j:j + shape[1] - 1, k:k + shape[2] - 1] for i in (0, 1) for j in (0, 1) for k in (0, 1)]
     active = np.logical_or.reduce(corners) & ~np.logical_and.reduce(corners)
     assert active.mean() > 0.99
-    ops._mc_state.clear()                                      # start from the smallest buffers: forces a regrowth
+    ops._scratch_cache.clear()                                 # start from the smallest buffers: forces a regrowth
     v, f = _mc_against_oracle(sdf)
     assert v.shape[0] > 2_500_000 and f.shape[0] > 2_500_000
 

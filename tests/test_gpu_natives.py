@@ -129,7 +129,7 @@ def _assert_mc_matches_oracle(v, f, sdf, step=(1.0, 1.0, 1.0), origin=(0.0, 0.0,
 def test_marching_cubes_buffer_growth():
     """The one-call path grows its capacity buffers when the first guess is too small, is reproducible afterwards, and
     equals the oracle before and after the growth."""
-    ops._mc_state.clear()
+    ops._scratch_cache.clear()
     big = synth.sphere_sdf_grid(97, num=6, seed=4, device=DEV)        # > 4096 vertices: forces one regrowth
     v1, f1 = ops.mc_gpu(big, 2 / 96, 2 / 96, 2 / 96, -1.0, -1.0, -1.0)
     assert v1.shape[0] > 4096

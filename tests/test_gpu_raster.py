@@ -196,7 +196,7 @@ def test_pair_list_regrows_to_the_same_result(mesh):
     d = deform(verts, 3, 7)
     cam = cameras(3, 400, 400, 7)
     big = ops.rasterize_meshes(d, faces, cam, 400, 400, capacity=10_000_000)
-    ops._raster_state.clear()                          # a fresh workspace that must grow inside the call
+    ops._scratch_cache.clear()                         # a fresh workspace that must grow inside the call
     small = ops.rasterize_meshes(d, faces, cam, 400, 400, capacity=16)
     assert small[4] == big[4] and small[4]["pairs"] > 16
     for a, b in zip(big[:4], small[:4]):
