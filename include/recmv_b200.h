@@ -447,6 +447,44 @@ RECMV_API int recmv_knn_nearest_backward(const float* p1, const float* p2, const
                           int N, int64_t P1, int64_t P2, int D, void* workspace, float* grad_p1, float* grad_p2,
                           recmv_stream_t stream);
 
+/* ---- template registration: the inner step of NRICP_Optimizer_AdamW (DESIGN section 1f) ---------------------------
+ * replaces the per-iteration torch graph of nricp_optimizer.py:382-423 (Local_Affine warp, edge stiffness, pytorch3d's
+ * uniform mesh_laplacian_smoothing, autograd and AdamW(amsgrad=True)).
+ * Adjacency: faces [F,3] int64 over V vertices (a face with an index outside [0, V) is skipped).  E = the unique
+ * sorted pairs of the 3F face sides; row_ptr [V+1] int32 and col [6F] int32 are the symmetric CSR of E (both
+ * directions of every edge, so a self edge (a, a) appears twice in row a), neighbours ascending within a row; only
+ * col[0, row_ptr[V]) is used, the rest is -1.  deg [V] int32 = row length; boundary [V] u8 = 1 where one of the
+ * vertex's sides occurs exactly once among the 3F sides.  No host synchronisation.
+ * workspace: recmv_mesh_adjacency_workspace_bytes(V, F).
+ * Warp: X [V,3,4] f32 = [A | b] per vertex, x [V,3] source points -> out_v = A x + b; out_n = inv(A)^T n and out_ok
+ * (|det A| >= 1e-4, else n' = 0) when not NULL (they need normals [V,3]).
+ * Step, one AdamW-AMSGrad iteration in two launches, in place on X and its moments exp_avg / exp_avg_sq /
+ * max_exp_avg_sq [V,3,4] (prm->step == 1 starts them from zero and does not read them): with c_i = target_v[corr_idx
+ * [i]], m_i = target_n[corr_idx[i]] (corr_idx [V] int64, an index outside [0, T) gates the vertex out) and
+ * w_i = !boundary_i & ok_i & (cos(m_i, n'_i) > threshold), loss = sqrt(S) + lw / V sum_i |Lv_i| with
+ * S = sum_i w_i |v_i - c_i|^2 + sw sum_{(i,j) in E} ||(X_i - X_j) diag(1,1,1,gamma)||^2 and Lv_i = mean_{j in N(i)} v_j
+ * - v_i (-v_i when deg_i = 0).  stats DEVICE float[8] = {data sum, sw * stiffness sum, Laplacian term, loss, gate
+ * count, S, 0, 0} of the state before the update.  Every reduction runs in a fixed order that depends on V alone: the
+ * results are bit-identical from run to run and on any GPU.  No float atomics, no host synchronisation.
+ * workspace: recmv_nricp_workspace_bytes(V).                                                                        */
+typedef struct {
+  float stiffness_weight, laplacian_weight, gamma, threshold;
+  float lr, beta1, beta2, eps, weight_decay;   /* torch.optim.AdamW: 1e-4, 0.9, 0.999, 1e-8, 1e-2 in the reference */
+  int step;                                    /* 1-based step count since the moments were last reset */
+} recmv_nricp_params_t;
+
+RECMV_API int recmv_mesh_adjacency_workspace_bytes(int64_t V, int64_t F, size_t* bytes);
+RECMV_API int recmv_mesh_adjacency(const int64_t* faces, int64_t F, int64_t V, void* workspace, int32_t* row_ptr,
+                          int32_t* col, int32_t* deg, uint8_t* boundary, recmv_stream_t stream);
+RECMV_API int recmv_nricp_warp(const float* X, const float* x, const float* normals, int64_t V, float* out_v,
+                          float* out_n, uint8_t* out_ok, recmv_stream_t stream);
+RECMV_API int recmv_nricp_workspace_bytes(int64_t V, size_t* bytes);
+RECMV_API int recmv_nricp_step(const float* x, const float* normals, const float* target_v, const float* target_n,
+                          int64_t T, const int64_t* corr_idx, const int32_t* row_ptr, const int32_t* col,
+                          const uint8_t* boundary, int64_t V, const recmv_nricp_params_t* prm /*host*/, float* X,
+                          float* exp_avg, float* exp_avg_sq, float* max_exp_avg_sq, void* workspace,
+                          float* stats /*device[8]*/, recmv_stream_t stream);
+
 /* ---- A11 / (f2): the sweep of one pyramid level as a DEVICE WORKLIST (SURVEY 8b `recmv_c2f_sweep`) -----------------
  * replaces the coordinate-list bookkeeping of MCAcc/seg3d_lossless.py:306-428 (nonzero / unique / index scatter, a
  * host sync per step).  level / final_res are (W, H, D) = (x, y, z) lattice sizes (host).  A worklist is idx_out[i]

@@ -34,6 +34,12 @@ class RayMarch(Structure):
                 ("samples_per_ray", c_int)]
 
 
+class NricpParams(Structure):
+    _fields_ = [("stiffness_weight", c_float), ("laplacian_weight", c_float), ("gamma", c_float),
+                ("threshold", c_float), ("lr", c_float), ("beta1", c_float), ("beta2", c_float), ("eps", c_float),
+                ("weight_decay", c_float), ("step", c_int)]
+
+
 # name -> (restype, argtypes); must list every symbol of include/recmv_b200.h
 SIGNATURES = {
     "recmv_version": (c_int, []),
@@ -131,6 +137,14 @@ SIGNATURES = {
                                   c_void_p, c_void_p, c_void_p]),
     "recmv_knn_nearest_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int64, c_int64, c_int,
                                            c_void_p, c_void_p, c_void_p, c_void_p]),
+    "recmv_mesh_adjacency_workspace_bytes": (c_int, [c_int64, c_int64, POINTER(c_size_t)]),
+    "recmv_mesh_adjacency": (c_int, [c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                     c_void_p]),
+    "recmv_nricp_warp": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "recmv_nricp_workspace_bytes": (c_int, [c_int64, POINTER(c_size_t)]),
+    "recmv_nricp_step": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p,
+                                 c_int64, POINTER(NricpParams), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                 c_void_p, c_void_p]),
     "recmv_c2f_refine":(c_int, [c_void_p, c_void_p, c_int, c_int, c_int, POINTER(c_int), POINTER(c_float), POINTER(c_float),
                                  c_float, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
     "recmv_c2f_scatter_list": (c_int, [c_void_p, c_void_p, c_void_p, c_int, POINTER(c_int), POINTER(c_int), c_void_p,

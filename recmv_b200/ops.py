@@ -1604,6 +1604,90 @@ class KnnNearestFunction(torch.autograd.Function):
         return (g1 if ctx.needs_input_grad[0] else None), g2, None, None
 
 
+NRICP_STATS = 8   # stats record of recmv_nricp_step (include/recmv_b200.h)
+
+
+def mesh_adjacency(faces, V):
+    """Edges and boundary of a triangle mesh (recmv_mesh_adjacency): faces [F,3] int64, CUDA and contiguous, over V
+    vertices -> (row_ptr [V+1] int32, col [6F] int32, deg [V] int32, boundary [V] bool).  row_ptr / col is the symmetric
+    CSR of the unique sorted face sides, neighbours ascending; col[row_ptr[V]:] is -1.  A vertex is on the boundary when
+    one of its sides occurs once among the 3F sides; faces with an index outside [0, V) are skipped.  No host
+    synchronisation."""
+    _check_input(faces, "faces")
+    dev = faces.device
+    _expect("mesh_adjacency", "faces", faces, torch.int64, ("F", 3))
+    F, V = int(faces.shape[0]), int(V)
+    row_ptr = torch.empty((V + 1,), dtype=torch.int32, device=dev)
+    col = torch.empty((6 * F,), dtype=torch.int32, device=dev)
+    deg = torch.empty((V,), dtype=torch.int32, device=dev)
+    boundary = torch.empty((V,), dtype=torch.bool, device=dev)
+    ws = _scratch(dev, "adjacency_ws", max(_size("recmv_mesh_adjacency_workspace_bytes", V, F, dev=dev), 1))
+    _launch("recmv_mesh_adjacency", faces, _ptr(faces), F, V, _ptr(ws), _ptr(row_ptr), _ptr(col), _ptr(deg),
+            _ptr(boundary))
+    return row_ptr, col, deg, boundary
+
+
+def nricp_warp(X, x, normals=None):
+    """Local affine warp (recmv_nricp_warp): X [V,3,4] f32 = [A | b] per vertex, x [V,3] f32 -> v = A x + b [V,3]; with
+    normals [V,3] also (n' = inv(A)^T n [V,3], ok [V] bool), n' = 0 where |det A| < 1e-4.  All CUDA and contiguous."""
+    for t, name in ((X, "X"), (x, "x")) + (((normals, "normals"),) if normals is not None else ()):
+        _check_input(t, name)
+    dev = x.device
+    _expect("nricp_warp", "x", x, torch.float32, ("V", 3))
+    V = int(x.shape[0])
+    _expect("nricp_warp", "X", X, torch.float32, (V, 3, 4), dev)
+    v = torch.empty((V, 3), dtype=torch.float32, device=dev)
+    n_out = ok = None
+    if normals is not None:
+        _expect("nricp_warp", "normals", normals, torch.float32, (V, 3), dev)
+        n_out = torch.empty((V, 3), dtype=torch.float32, device=dev)
+        ok = torch.empty((V,), dtype=torch.bool, device=dev)
+    _launch("recmv_nricp_warp", x, _ptr(X), _ptr(x), _ptr(normals), V, _ptr(v), _ptr(n_out), _ptr(ok))
+    return v if normals is None else (v, n_out, ok)
+
+
+def nricp_step(x, normals, target_v, target_n, corr_idx, adjacency, X, moments, step, stiffness_weight,
+               laplacian_weight, gamma=1.0, threshold=0.5, lr=1e-4, betas=(0.9, 0.999), eps=1e-8, weight_decay=1e-2,
+               stats=None):
+    """One NRICP inner iteration (recmv_nricp_step, DESIGN section 1f), in place on X [V,3,4] and moments = (exp_avg,
+    exp_avg_sq, max_exp_avg_sq), each [V,3,4] f32: gate, loss, closed-form gradient and torch.optim.AdamW(amsgrad=True)
+    with the given hyper-parameters at 1-based `step` (step 1 starts the moments from zero).  x, normals [V,3] f32 are
+    the source points and normals; target_v, target_n [T,3] f32; corr_idx [V] int64 the target index of every vertex;
+    adjacency = mesh_adjacency(faces, V).  Returns stats [8] f32 on the device (written into `stats` when given):
+    {data sum, stiffness term, Laplacian term, loss, gate count, S, 0, 0} before the update.  Two launches, no host
+    synchronisation, bit-identical from run to run."""
+    row_ptr, col, _deg, boundary = adjacency
+    for t, name in ((x, "x"), (normals, "normals"), (target_v, "target_v"), (target_n, "target_n"),
+                    (corr_idx, "corr_idx"), (row_ptr, "row_ptr"), (col, "col"), (boundary, "boundary"), (X, "X"),
+                    (moments[0], "exp_avg"), (moments[1], "exp_avg_sq"), (moments[2], "max_exp_avg_sq")):
+        _check_input(t, name)
+    dev = x.device
+    _expect("nricp_step", "x", x, torch.float32, ("V", 3))
+    V = int(x.shape[0])
+    _expect("nricp_step", "normals", normals, torch.float32, (V, 3), dev)
+    _expect("nricp_step", "target_v", target_v, torch.float32, ("T", 3), dev)
+    T = int(target_v.shape[0])
+    _expect("nricp_step", "target_n", target_n, torch.float32, (T, 3), dev)
+    _expect("nricp_step", "corr_idx", corr_idx, torch.int64, (V,), dev)
+    _expect("nricp_step", "row_ptr", row_ptr, torch.int32, (V + 1,), dev)
+    _expect("nricp_step", "col", col, torch.int32, ("E",), dev)
+    _expect("nricp_step", "boundary", boundary, torch.bool, (V,), dev)
+    for t, name in ((X, "X"), (moments[0], "exp_avg"), (moments[1], "exp_avg_sq"), (moments[2], "max_exp_avg_sq")):
+        _expect("nricp_step", name, t, torch.float32, (V, 3, 4), dev)
+    if stats is None:
+        stats = torch.empty((NRICP_STATS,), dtype=torch.float32, device=dev)
+    else:
+        _check_input(stats, "stats")
+        _expect("nricp_step", "stats", stats, torch.float32, (NRICP_STATS,), dev)
+    prm = _lib.NricpParams(stiffness_weight, laplacian_weight, gamma, threshold, lr, betas[0], betas[1], eps,
+                           weight_decay, int(step))
+    ws = _scratch(dev, "nricp_ws", max(_size("recmv_nricp_workspace_bytes", V), 1))
+    _launch("recmv_nricp_step", x, _ptr(x), _ptr(normals), _ptr(target_v), _ptr(target_n), T, _ptr(corr_idx),
+            _ptr(row_ptr), _ptr(col), _ptr(boundary), V, byref(prm), _ptr(X), _ptr(moments[0]), _ptr(moments[1]),
+            _ptr(moments[2]), _ptr(ws), _ptr(stats))
+    return stats
+
+
 class C2fLevel:
     """Device worklist of one pyramid level (recmv_c2f_refine / recmv_sdf_mlp_fwd_counted / recmv_c2f_scatter_list /
     recmv_c2f_mark_conflicts): one fused full-grid pass builds the level and its worklist, conflict rounds are driven by
