@@ -485,6 +485,25 @@ RECMV_API int recmv_nricp_step(const float* x, const float* normals, const float
                           float* exp_avg, float* exp_avg_sq, float* max_exp_avg_sq, void* workspace,
                           float* stats /*device[8]*/, recmv_stream_t stream);
 
+/* ---- template fitting: the Laplacian-editing solve of Laplacian_Optimizer (DESIGN section 1g) ----------------------
+ * replaces the dense inv(L^T W L) L^T W t of lap_deform_optimizer.py:144-183.  verts [V,3] f32 = x; (row_ptr, col, deg)
+ * = recmv_mesh_adjacency of the template's faces; L = D^-1 Adj - I (-I on a row with deg 0).  Constraints: cidx [M]
+ * int64 SORTED ascending (duplicates allowed, each its own row of P; an index outside [0, V) is skipped) with targets
+ * ctgt [M,3] f32 in the same order.  Solves A y = b, A = L^T L + c P^T P, b = L^T L x + c P^T u (c = constrain_weight
+ * >= 0), for the three columns independently by Jacobi-preconditioned CG in float64 from y0 = x: a column stops when
+ * |r| <= tol |b|, when r.r is not finite, or after max_iter iterations.  A component with no constraint keeps y = x
+ * exactly.  smooth != 0 then stores y'_i = (1/deg_i) sum_{j in N(i), j != i} y_j (0 at deg_i = 0), else y; out [V,3]
+ * f32.  stats DEVICE float[8] = {iterations of x, y, z; |r| / |b| of x, y, z (|r| where |b| = 0); 1 = every column
+ * met tol, 0 = one stopped at max_iter, -1 = one had a non-finite residual; constraints skipped}.  Three launches, the
+ * second cooperative; max_blocks = 0 runs every co-resident block, > 0 caps the grid (the result does not depend on
+ * it).  Reductions run in a fixed order over 256-vertex chunks: bit-identical from run to run and for any grid.  No
+ * atomics, no host synchronisation.  workspace: recmv_lap_edit_workspace_bytes(V, M).                            */
+RECMV_API int recmv_lap_edit_workspace_bytes(int64_t V, int64_t M, size_t* bytes);
+RECMV_API int recmv_lap_edit_solve(const float* verts, int64_t V, const int32_t* row_ptr, const int32_t* col,
+                          const int32_t* deg, const int64_t* cidx, const float* ctgt, int64_t M, double constrain_weight,
+                          double tol, int max_iter, int smooth, int max_blocks, void* workspace, float* out,
+                          float* stats /*device[8]*/, recmv_stream_t stream);
+
 /* ---- A11 / (f2): the sweep of one pyramid level as a DEVICE WORKLIST (SURVEY 8b `recmv_c2f_sweep`) -----------------
  * replaces the coordinate-list bookkeeping of MCAcc/seg3d_lossless.py:306-428 (nonzero / unique / index scatter, a
  * host sync per step).  level / final_res are (W, H, D) = (x, y, z) lattice sizes (host).  A worklist is idx_out[i]

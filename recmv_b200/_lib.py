@@ -6,7 +6,7 @@ FastMinv/M3x3Inv.cpp:4-6).
 """
 import ctypes
 import os
-from ctypes import (POINTER, Structure, c_char_p, c_float, c_int, c_int64, c_size_t,
+from ctypes import (POINTER, Structure, c_char_p, c_double, c_float, c_int, c_int64, c_size_t,
                     c_void_p)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -145,6 +145,9 @@ SIGNATURES = {
     "recmv_nricp_step": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p,
                                  c_int64, POINTER(NricpParams), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                  c_void_p, c_void_p]),
+    "recmv_lap_edit_workspace_bytes": (c_int, [c_int64, c_int64, POINTER(c_size_t)]),
+    "recmv_lap_edit_solve": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64,
+                                     c_double, c_double, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "recmv_c2f_refine":(c_int, [c_void_p, c_void_p, c_int, c_int, c_int, POINTER(c_int), POINTER(c_float), POINTER(c_float),
                                  c_float, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
     "recmv_c2f_scatter_list": (c_int, [c_void_p, c_void_p, c_void_p, c_int, POINTER(c_int), POINTER(c_int), c_void_p,

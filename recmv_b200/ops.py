@@ -1688,6 +1688,48 @@ def nricp_step(x, normals, target_v, target_n, corr_idx, adjacency, X, moments, 
     return stats
 
 
+LAP_EDIT_STATS = 8   # stats record of recmv_lap_edit_solve (include/recmv_b200.h)
+
+
+def laplacian_edit(verts, adjacency, cidx, ctgt, constrain_weight=1.0, smooth=True, tol=1e-10, max_iter=50000,
+                   stats=None, max_blocks=0):
+    """Laplacian editing of a template (recmv_lap_edit_solve, DESIGN section 1g): y = argmin |L y - L x|^2 +
+    c |P y - u|^2 with x = verts [V,3] f32, adjacency = mesh_adjacency(faces, V), constraints cidx [M] int64 (any order,
+    duplicates allowed, indices outside [0, V) skipped and counted) with targets ctgt [M,3] f32 and c =
+    constrain_weight, solved in float64 by Jacobi-preconditioned CG from y0 = x; smooth applies the reference's
+    zero-diagonal Laplacian afterwards.  Returns (new_verts [V,3] f32, stats [8] f32 on the device, written into `stats`
+    when given): {iterations of x, y, z; relative residuals of x, y, z; 1 converged / 0 max_iter reached / -1 non-finite;
+    constraints skipped}.  Three launches, no host synchronisation.  max_blocks caps the solver's grid (0: every
+    co-resident block); the result does not depend on it."""
+    row_ptr, col, deg, _boundary = adjacency
+    for t, name in ((verts, "verts"), (row_ptr, "row_ptr"), (col, "col"), (deg, "deg"), (cidx, "cidx"),
+                    (ctgt, "ctgt")):
+        _check_input(t, name)
+    dev = verts.device
+    _expect("laplacian_edit", "verts", verts, torch.float32, ("V", 3))
+    V = int(verts.shape[0])
+    _expect("laplacian_edit", "row_ptr", row_ptr, torch.int32, (V + 1,), dev)
+    _expect("laplacian_edit", "col", col, torch.int32, ("E",), dev)
+    _expect("laplacian_edit", "deg", deg, torch.int32, (V,), dev)
+    _expect("laplacian_edit", "cidx", cidx, torch.int64, ("M",), dev)
+    M = int(cidx.shape[0])
+    _expect("laplacian_edit", "ctgt", ctgt, torch.float32, (M, 3), dev)
+    if stats is None:
+        stats = torch.empty((LAP_EDIT_STATS,), dtype=torch.float32, device=dev)
+    else:
+        _check_input(stats, "stats")
+        _expect("laplacian_edit", "stats", stats, torch.float32, (LAP_EDIT_STATS,), dev)
+    # the kernel finds each vertex's constraints by binary search: sort them by vertex, keeping duplicates in order
+    cidx, order = torch.sort(cidx, stable=True)
+    ctgt = ctgt.index_select(0, order)
+    out = torch.empty((V, 3), dtype=torch.float32, device=dev)
+    ws = _scratch(dev, "lap_edit_ws", _size("recmv_lap_edit_workspace_bytes", V, M))
+    _launch("recmv_lap_edit_solve", verts, _ptr(verts), V, _ptr(row_ptr), _ptr(col), _ptr(deg), _ptr(cidx), _ptr(ctgt),
+            M, float(constrain_weight), float(tol), int(max_iter), int(bool(smooth)), int(max_blocks), _ptr(ws),
+            _ptr(out), _ptr(stats))
+    return out, stats
+
+
 class C2fLevel:
     """Device worklist of one pyramid level (recmv_c2f_refine / recmv_sdf_mlp_fwd_counted / recmv_c2f_scatter_list /
     recmv_c2f_mark_conflicts): one fused full-grid pass builds the level and its worklist, conflict rounds are driven by

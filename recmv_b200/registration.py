@@ -1,4 +1,7 @@
-"""Drop-in `NRICP_Optimizer_AdamW` (engineer/optimizer/nricp_optimizer.py:321-448): the template registration of
+"""Drop-in `Laplacian_Optimizer` (engineer/optimizer/lap_deform_optimizer.py:25-186): the feature-curve fit of the
+garment templates, solved by the matrix-free PCG of csrc/lap_edit.cu (DESIGN section 1g).
+
+Drop-in `NRICP_Optimizer_AdamW` (engineer/optimizer/nricp_optimizer.py:321-448): the template registration of
 `registration` (OptimGarmentNetwork.py:2415-2425) with its inner loop on the fused step of csrc/nricp.cu.
 
 Same constructor, same `__call__(**inputs) -> fitting(inputs) -> (loss, smpl_slice)`, same per-epoch line and the same
@@ -7,7 +10,9 @@ steps, with one host read for the epoch's line.  The rules are DESIGN section 1f
 because the reference builds a new optimizer per epoch.  Not supported (no live caller passes them):
 `use_normal=False` and non-empty `static_pts_type`."""
 import os
+import warnings
 
+import numpy as np
 import torch
 
 from . import ops
@@ -19,6 +24,73 @@ def _write_obj(path, verts, faces):
             f.write("v {:.6f} {:.6f} {:.6f}\n".format(*v))
         for t in (faces + 1).tolist():
             f.write("f {:d} {:d} {:d}\n".format(*t))
+
+
+def _write_ply(path, verts):
+    """A vertex-only binary PLY, the form pytorch3d's save_ply(path, verts) writes."""
+    v = np.ascontiguousarray(verts.detach().cpu().numpy(), dtype="<f4").reshape(-1, 3)
+    with open(path, "wb") as f:
+        f.write("ply\nformat binary_little_endian 1.0\nelement vertex {:d}\nproperty float x\nproperty float y\n"
+                "property float z\nend_header\n".format(len(v)).encode("ascii"))
+        f.write(v.tobytes())
+
+
+class Laplacian_Optimizer:
+    """Laplacian editing of the garment templates onto the feature curves: per epoch and template, the constraints from
+    the template's own best_match (and static points), then y = argmin |L y - L x|^2 + c |P y - u|^2 and, with smooth,
+    the reference's zero-diagonal Laplacian smoothing.  `stats` keeps the device stats of the last solve."""
+
+    def __init__(self, epoch=3, constrain_weight=1., optimizer_setting=None, smooth=True):
+        self.name = "Laplacian_Deform_Optimzier"
+        self.optimizier_setting = optimizer_setting
+        self.epoch = epoch
+        self.constrain_weights = constrain_weight
+        self.smooth = smooth
+        self.stats = None
+
+    def __call__(self, **inputs):
+        return self.fitting(inputs)
+
+    def _collect_data(self, inputs):
+        """[(source_idx, target)] per template, the reference's merge_source_target_map of best_match and static points."""
+        target_packed = {name: mesh.verts_packed() for mesh, name in zip(inputs["target_meshes"],
+                                                                          inputs["target_fl_type"])}
+        maps = []
+        for template in inputs["source_fl_meshes"]:
+            idx, tgt = template.best_match(target_packed, template.device, inputs["outlayer"])
+            static = template.static_pts_match()
+            if static is not None:
+                idx, tgt = torch.cat([idx, static[0]], dim=0), torch.cat([tgt, static[1]], dim=0)
+            maps.append((idx, tgt))
+        return maps
+
+    @torch.no_grad()
+    def fitting(self, inputs):
+        templates = inputs["source_fl_meshes"]
+        for _ in range(self.epoch):
+            maps = self._collect_data(inputs)
+            vertices = [template.vertices for template in templates]
+            os.makedirs("./debug/register/", exist_ok=True)
+            for i, ((idx, tgt), v) in enumerate(zip(maps, vertices)):
+                _write_ply("./debug/register/source_{}.ply".format(i), v[idx])
+                _write_ply("./debug/register/target_{}.ply".format(i), tgt)
+            for template, (idx, tgt), v in zip(templates, maps, vertices):
+                dev = v.device
+                x = v.to(torch.float32).contiguous()
+                faces = template.faces.reshape(-1, 3).to(dev, torch.int64).contiguous()
+                adjacency = ops.mesh_adjacency(faces, x.shape[0])
+                new_v, stats = ops.laplacian_edit(x, adjacency, idx.to(dev, torch.int64).contiguous(),
+                                                  tgt.to(dev, torch.float32).contiguous(), self.constrain_weights,
+                                                  self.smooth)
+                self.stats = stats
+                st = stats.tolist()   # the solve's one host read
+                if st[6] != 1.0:
+                    warnings.warn("Laplacian_Optimizer: the solve did not converge ({}): iterations {}, relative "
+                                  "residuals {}, {} constraints skipped".format(
+                                      "non-finite residual" if st[6] < 0 else "max_iter reached",
+                                      [int(k) for k in st[:3]], st[3:6], int(st[7])), RuntimeWarning)
+                template.update_vertices(new_v)
+        return inputs
 
 
 class NRICP_Optimizer_AdamW:
