@@ -255,14 +255,13 @@ def tube(nt, nz, radius=0.3, height=1.5, jitter=0.0, seed=0):
         Z = Z + jitter * (height / nz) * g.uniform(-1, 1, Z.shape) * ((np.arange(nz) > 0) & (np.arange(nz) < nz - 1))
     rad = radius * (1.0 + 0.5 * (1.0 - Z / height))   # wider at the hem: skirt-like
     v = np.stack([(rad * np.cos(T)).ravel(), (rad * np.sin(T)).ravel(), Z.ravel()], 1)
-    f = []
-    for i in range(nt):
-        for j in range(nz - 1):
-            a, b, cc, d = i * nz + j, ((i + 1) % nt) * nz + j, ((i + 1) % nt) * nz + j + 1, i * nz + j + 1
-            f += [[a, b, cc], [a, cc, d]]
+    # quad (i, j) gives faces (a, b, c) and (a, c, d), in i-major then j order
+    I, J = np.meshgrid(np.arange(nt), np.arange(nz - 1), indexing="ij")
+    a, b = I * nz + J, ((I + 1) % nt) * nz + J
+    f = np.stack([np.stack([a, b, b + 1], -1), np.stack([a, b + 1, a + 1], -1)], axis=2).reshape(-1, 3)
     hem = np.arange(nt) * nz
     waist = np.arange(nt) * nz + nz - 1
-    return v, np.array(f, dtype=np.int64), dict(waist=waist, hem=hem)
+    return v, f.astype(np.int64), dict(waist=waist, hem=hem)
 
 
 def loop_targets(v, loops):

@@ -58,12 +58,17 @@ def identity_affine(V):
 
 
 def inv3x3(A):
-    """FastMinv's rule in float64: inverse by cofactors, zeros and ok = False where |det| < 1e-4."""
-    det = np.linalg.det(A)
-    ok = np.abs(det) >= 1e-4
+    """FastMinv's rule in float64: inverse by cofactors, zeros and ok = False where |det| < 1e-4.  A NaN det is not
+    below 1e-4, so a NaN (or inf) matrix gives ok = True and the non-finite cofactor quotients, as the kernel does."""
+    A = np.asarray(A, dtype=np.float64)
+    # cof[..., i, j] = the (i, j) cofactor; the inverse is its transpose over det
+    r0, r1, r2 = A[..., 0, :], A[..., 1, :], A[..., 2, :]
+    cof = np.stack([np.cross(r1, r2), np.cross(r2, r0), np.cross(r0, r1)], axis=-2)
+    det = (r0 * cof[..., 0, :]).sum(-1)
+    ok = ~(np.abs(det) < 1e-4)
     inv = np.zeros_like(A)
-    if ok.any():
-        inv[ok] = np.linalg.inv(A[ok])
+    with np.errstate(divide="ignore", invalid="ignore"):
+        inv[ok] = np.swapaxes(cof[ok], -1, -2) / det[ok][:, None, None]
     return inv, ok
 
 
@@ -216,7 +221,7 @@ def torch_loss(X, x, n, c, m, faces, boundary, sw, lw, gamma, threshold):
     v = (A @ x[:, :, None])[:, :, 0] + b
     with torch.no_grad():
         Ai = torch.linalg.inv(A)
-        ok = torch.linalg.det(A).abs() >= 1e-4
+        ok = ~(torch.linalg.det(A).abs() < 1e-4)
         n2 = torch.where(ok[:, None], (Ai.transpose(1, 2) @ n[:, :, None])[:, :, 0], torch.zeros_like(n))
         cos = (m * n2).sum(-1) / torch.sqrt(torch.clamp_min((m * m).sum(-1) * (n2 * n2).sum(-1), 1e-16))
         w = ~boundary & ok & (cos > threshold)

@@ -40,7 +40,10 @@ def _check_adjacency(faces, V):
 
 @pytest.mark.parametrize("faces,V", [([[0, 1, 2]], 3), ([[0, 1, 2], [2, 1, 3]], 5), ([[0, 0, 1]], 2),
                                      ([[0, 1, 2], [1, 2, 5], [-1, 0, 1]], 4), ([[3, 3, 3]], 4),
-                                     (np.zeros((0, 3), dtype=np.int64), 3)])
+                                     (np.zeros((0, 3), dtype=np.int64), 3),
+                                     # a side in three faces (non-manifold), and a face repeated as is and reversed
+                                     ([[0, 1, 2], [1, 0, 3], [0, 4, 1]], 5),
+                                     ([[0, 1, 2], [0, 1, 2], [2, 1, 0], [1, 3, 2]], 4)])
 def test_adjacency_hand_meshes(faces, V):
     _check_adjacency(faces, V)
 

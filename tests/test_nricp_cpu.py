@@ -133,3 +133,25 @@ def test_fitting_loop_matches_the_reference(golden, case):
     # the printed terms are rounded to 4-5 decimals
     np.testing.assert_allclose(r["stats"], z[f"stats_{case}"], rtol=0, atol=6e-5)
     assert np.array_equal(r["stats"][:, 1], z[f"stats_{case}"][:, 1])
+
+
+def test_inverse_rule_matches_fastminv_on_non_finite_and_gate_matrices():
+    # FastMinv's test is |det| < 1e-4, so a NaN det passes the gate: ok = True and a non-finite inverse
+    from oracle import oracle_torch as ot
+    g = np.random.default_rng(3)
+    A = g.standard_normal((12, 3, 3))
+    A[0, 1, 2] = np.nan
+    A[1, 0, 0] = np.inf
+    A[2, 2, 1] = -np.inf
+    A[3] = np.diag([1e-2, 1e-2, 0.99])      # det 9.9e-5: below the gate
+    A[4] = np.diag([1e-2, 1e-2, 1.01])      # det 1.01e-4: above it
+    A[5, 2] = A[5, 0]                       # exactly singular
+    inv, ok = no.inv3x3(A)
+    ref_inv, ref_ok = ot.minv3x3_fwd(torch.as_tensor(A))
+    assert ok.tolist() == ref_ok.tolist()
+    assert ok[0] and ok[1] and ok[2] and not ok[3] and ok[4] and not ok[5]
+    assert np.isnan(inv[0]).any() and (inv[3] == 0).all() and (inv[5] == 0).all()
+    np.testing.assert_array_equal(np.isnan(inv), torch.isnan(ref_inv).numpy())
+    fin = np.isfinite(inv)
+    np.testing.assert_allclose(inv[fin], ref_inv.numpy()[fin], rtol=1e-12, atol=0)
+    np.testing.assert_allclose(inv[6:], np.linalg.inv(A[6:]), rtol=1e-12, atol=1e-12)
