@@ -428,6 +428,22 @@ RECMV_API int recmv_shade_phong(const int64_t* pix_to_face, const float* bary, i
                           const float* normals, const float* colors, int V, const int64_t* faces, int64_t F,
                           const float* params /*device[N][28]*/, float* out_rgba, recmv_stream_t stream);
 
+/* ---- area-weighted surface sampling: the fans of `curve_aware_loss` (DESIGN section 1h) ---------------------------
+ * replaces trimesh's `sample_surface` (OptimGarmentNetwork.py:808-809,832-833) with a pinned stream.  verts [M,V,3]
+ * f32, faces [F,3] int64 shared by the M meshes -> out [M,S,3] f32.  Sample s of mesh m depends only on (seed, offset,
+ * m, s): Philox4x32-10 with key {seed low word, seed high word} and counter {low, high word of offset + m*S + s
+ * (mod 2^64), 0, 0} gives x0..x3; u = ((x0 << 21) | (x1 >> 11)) 2^-53, a = x2 2^-32, b = x3 2^-32, and (a, b) ->
+ * (1 - a, 1 - b) when a + b > 1.  Areas in fp64 from the fp32 corners, e1 = v1 - v0, e2 = v2 - v0, c = e1 x e2,
+ * area = 0.5 sqrt((cx^2 + cy^2) + cz^2); a face with an index outside [0, V) or a non-finite area counts 0.  C[f]
+ * fp64 inclusive, summed sequentially inside each 256-face chunk, the chunk totals summed sequentially, C = chunk prefix
+ * + local (np.cumsum for F <= 256).  Face = first f with C[f] >= u C[F-1] (face 0 when the total is 0); point =
+ * (a e1 + b e2) + v0 in fp64, rounded once to f32; NaN when the face has an invalid index.  Every fp64 operation is
+ * rounded on its own (no FMA).  Three launches, no atomics (bit-identical from run to run and on any GPU), no host
+ * synchronisation.  F = 0 with M*S > 0 is RECMV_E_SHAPE.  workspace: recmv_surface_sample_workspace_bytes(M, F).     */
+RECMV_API int recmv_surface_sample_workspace_bytes(int M, int64_t F, size_t* bytes);
+RECMV_API int recmv_surface_sample(const float* verts, int M, int V, const int64_t* faces, int64_t F, int64_t S,
+                          uint64_t seed, uint64_t offset, void* workspace, float* out, recmv_stream_t stream);
+
 /* ---- nearest neighbour (K = 1 knn_points): the feature-curve chamfer loss and template registration --------------
  * replaces pytorch3d's KNN extension behind `knn_points` / `chamfer_distance` (DESIGN section 1e).
  * p1 [N,P1,D] queries, p2 [N,P2,D] candidates, f32, D = 2 or 3; lengths1 / lengths2 DEVICE int64[N] or NULL (= P1, P2),

@@ -7,7 +7,7 @@ FastMinv/M3x3Inv.cpp:4-6).
 import ctypes
 import os
 from ctypes import (POINTER, Structure, c_char_p, c_double, c_float, c_int, c_int64, c_size_t,
-                    c_void_p)
+                    c_uint64, c_void_p)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "librecmv_b200.so")
@@ -132,7 +132,10 @@ SIGNATURES = {
     "recmv_vertex_normals": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int64, c_void_p, c_void_p, c_void_p]),
     "recmv_shade_phong": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p,
                                   c_int64, c_void_p, c_void_p, c_void_p]),
-    "recmv_knn_workspace_bytes": (c_int, [c_int, c_int64, c_int64, POINTER(c_size_t)]),
+    "recmv_surface_sample_workspace_bytes": (c_int, [c_int, c_int64, POINTER(c_size_t)]),
+    "recmv_surface_sample": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int64, c_int64, c_uint64, c_uint64, c_void_p,
+                                     c_void_p, c_void_p]),
+    "recmv_knn_workspace_bytes":(c_int, [c_int, c_int64, c_int64, POINTER(c_size_t)]),
     "recmv_knn_nearest": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int64, c_int64, c_int, c_void_p,
                                   c_void_p, c_void_p, c_void_p]),
     "recmv_knn_nearest_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int64, c_int64, c_int,

@@ -1512,6 +1512,28 @@ def vertex_normals(verts, faces):
     return out
 
 
+def surface_sample(verts, faces, count, seed, offset=0):
+    """Area-weighted surface samples (recmv_surface_sample, DESIGN section 1h): verts [M,V,3] f32, faces [F,3] int64
+    shared by the M meshes, CUDA and contiguous -> [M,count,3] f32.  Sample s of mesh m is a pure function of (seed,
+    offset, m, s) (Philox4x32-10 counter offset + m*count + s), so one call over M meshes equals M calls at offsets
+    offset, offset + count, ...  Three launches, bit-identical from run to run, no host synchronisation."""
+    for t, name in ((verts, "verts"), (faces, "faces")):
+        _check_input(t, name)
+    dev = verts.device
+    _expect("surface_sample", "verts", verts, torch.float32, ("M", "V", 3))
+    _expect("surface_sample", "faces", faces, torch.int64, ("F", 3), dev)
+    M, V, F, S = int(verts.shape[0]), int(verts.shape[1]), int(faces.shape[0]), int(count)
+    if S < 0:
+        raise RuntimeError(f"surface_sample: count must be >= 0, got {S}")
+    if F == 0 and M * S > 0:
+        raise RuntimeError("surface_sample: faces is empty, there is no surface to sample")
+    out = torch.empty((M, S, 3), dtype=torch.float32, device=dev)
+    ws = _scratch(dev, "surface_sample_ws", max(_size("recmv_surface_sample_workspace_bytes", M, F), 1))
+    _launch("recmv_surface_sample", verts, _ptr(verts), M, V, _ptr(faces), F, S, int(seed) % (1 << 64),
+            int(offset) % (1 << 64), _ptr(ws), _ptr(out))
+    return out
+
+
 def shade_phong(frags, verts, normals, colors, faces, params):
     """Hard Phong shading of K = 1 mesh fragments (recmv_shade_phong).  frags: an object with pix_to_face [N,H,W,1]
     int64 and bary_coords [N,H,W,1,3] f32 (raster.Fragments), or the tuple of rasterize_meshes; verts, normals [N,V,3]

@@ -56,6 +56,17 @@ def vertex_normals(verts, faces):
     return ops.vertex_normals(verts.detach().float().contiguous(), faces.detach().long().contiguous())
 
 
+def sample_surface(verts, faces, count, seed=0, offset=0):
+    """Area-weighted surface samples of N meshes with one face list (trimesh's `sample_surface` with a pinned stream):
+    verts [N,V,3], faces [F,3] -> [N,count,3] f32.  Sample s of mesh n is a pure function of (seed, offset, n, s), so
+    advancing `offset` by N*count per call continues the stream (csrc/surface_sample.cu, DESIGN section 1h).  Faces
+    with an index outside [0, V) have area 0.  Forward only; the inputs are used detached."""
+    if not verts.is_cuda:
+        raise RuntimeError("sample_surface runs on CUDA tensors only (no CPU path)")
+    return ops.surface_sample(verts.detach().float().contiguous(), faces.detach().long().contiguous(), count, seed,
+                              offset)
+
+
 # pytorch3d's PointLights and Materials defaults
 DEFAULT_LIGHTS = {"location": (0.0, 1.0, 0.0), "ambient_color": (0.5,) * 3, "diffuse_color": (0.3,) * 3,
                   "specular_color": (0.2,) * 3}

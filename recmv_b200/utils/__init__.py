@@ -44,6 +44,61 @@ def fl_proj_loss(fl_pts_list, gt_fl_pts_list, fl_masks, proj_fl_weights=None):
     return (w * S / V.clamp_min(1) / Q.clamp_min(1)).sum() / C
 
 
+def _curve_index(fl_names, target):
+    """The reference's `for fl_idx, name in enumerate(fl_names): if name == target: break`: a missing name falls
+    through to the last curve."""
+    return next((i for i, n in enumerate(fl_names) if n == target), len(fl_names) - 1)
+
+
+def make_curve_aware_loss(curve_aware, samples=50000):
+    """`OptimGarmentNetwork.curve_aware_loss(self, ratio)` (OptimGarmentNetwork.py:787-839) with the fans sampled on the
+    GPU; bind it as `OptimGarmentNetwork.curve_aware_loss = make_curve_aware_loss(CURVE_AWARE)`.
+    As the reference: 0. when `pc_weight.curve_aware_weight` is 0; the `upper_bottom` curve's term whenever that curve
+    exists, the `curve_aware[garment_type]` curve's term when `isfine` (a missing name falls through to the last
+    curve); each term mean |sdf(p) + sdfShrinkRadius| through `garment_nets[-1]` over `samples` area-weighted points of
+    the fan (the curve, its centroid, faces (i, i+1, P) and (P-1, 0, P)), times the weight (60 without `pc_weight`).
+    The samples are detached, as the reference's host copy is.  Unlike the reference, all fans of a call are sampled
+    in one launch (csrc/surface_sample.cu) and evaluated in one SDF forward, `info['pc_<name>_circle_loss_sdf']` holds
+    a detached 0-d tensor, and nothing is read back to the host.  The stream's seed is drawn from torch's CPU
+    generator at the first call (so `torch.manual_seed` makes a run reproducible) and its offset advances by
+    curves * samples per call; both are in the returned function's `stream` dict."""
+    stream = {"seed": None, "offset": 0}
+
+    def curve_aware_loss(self, ratio):
+        ca_loss = 0.
+        if self.conf.get_float('pc_weight.curve_aware_weight') == 0.:
+            return ca_loss
+        terms = []
+        if 'upper_bottom' in self.fl_names:
+            terms.append(('upper_bottom', _curve_index(self.fl_names, 'upper_bottom')))
+        if self.garment_type in curve_aware and self.isfine:
+            target = curve_aware[self.garment_type]
+            terms.append((target, _curve_index(self.fl_names, target)))
+        if not terms:
+            return ca_loss
+        curves = self.inter_free_curve.forward()
+        pts = torch.stack([curves[i] for _, i in terms]).detach().float()
+        if not pts.is_cuda:
+            raise RuntimeError("curve_aware_loss runs on CUDA tensors only (no CPU path)")
+        M, P = int(pts.shape[0]), int(pts.shape[1])
+        verts = torch.cat([pts, pts.mean(1, keepdim=True)], 1).contiguous()
+        i = torch.arange(P, device=pts.device)
+        faces = torch.stack([i, (i + 1) % P, torch.full_like(i, P)], 1)
+        if stream["seed"] is None:
+            stream["seed"] = int(torch.empty((), dtype=torch.int64).random_())
+        surface_pts = _ops.surface_sample(verts, faces, samples, stream["seed"], stream["offset"])
+        stream["offset"] += M * samples
+        mnfld_pred = self.garment_nets[-1](surface_pts.view(-1, 3), ratio).view(M, samples)
+        circle_sdf_loss = (mnfld_pred + self.sdfShrinkRadius).abs().mean(1)
+        for (name, _), v in zip(terms, circle_sdf_loss.detach().unbind(0)):
+            self.info['pc_{}_circle_loss_sdf'.format(name)] = v
+        weight = self.conf.get_float('pc_weight.curve_aware_weight') if 'pc_weight' in self.conf else 60.
+        return (circle_sdf_loss * weight).sum()
+
+    curve_aware_loss.stream = stream
+    return curve_aware_loss
+
+
 def compute_Jacobian(ps, ds, retain_graph, create_graph, allow_unused=False):
     """J = dD/dp by three autograd passes (utils/utils.py:133-156) -> [N,3,3], row i = grad of D_i."""
     rows = []
