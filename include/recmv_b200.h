@@ -384,6 +384,23 @@ RECMV_API int recmv_rasterize_meshes(const float* verts, int V, const int64_t* f
                           void* workspace, int64_t capacity, int64_t* out_pix_to_face, float* out_zbuf, float* out_bary,
                           float* out_dists, int32_t* counters /*device*/, recmv_stream_t stream);
 
+/* ---- sparse z-buffer probe: the visibility test of fl_visible_by_body_zbuff / check_zbuf_body (DESIGN section 1i) --
+ * the value the reference's `grid_sample(zbuf filled, uv, align_corners=True)` returns at a set of query points, with
+ * zbuf the recmv_rasterize_meshes zbuf of the same verts, faces, camera, H, W, z_clip, area_eps -- without rasterizing
+ * the frame.  screen_pts [N,Q,D] f32 (D >= 2; x, y read), norm_size DEVICE float[N][2] = (w, h), fill DEVICE float[N].
+ * u = 2 sx / w - 1, v = 2 sy / h - 1, ix = ((u + 1) / 2) (W - 1), iy = ((v + 1) / 2) (H - 1); ATen's bilinear taps nw,
+ * ne, sw, se and weights, zeros padding; a tap's value is the rasterizer's zbuf there, or fill[n] where that zbuf is
+ * -1 (background); out [N,Q] = the weighted taps accumulated in that order with fused multiply-adds; 0 when ix or iy
+ * is not finite.  out_tap_zbuf [N,Q,4] f32 / out_tap_face [N,Q,4] int64 (both NULL or both set): the rasterizer's
+ * (zbuf, packed face) at each tap, (-1, -1) on background and outside the image.  A face with an index outside [0, V)
+ * is skipped.  Five launches, no host synchronisation, deterministic.  workspace: recmv_zbuf_probe_workspace_bytes.  */
+RECMV_API int recmv_zbuf_probe_workspace_bytes(int N, int64_t Q, int H, int W, size_t* bytes);
+RECMV_API int recmv_zbuf_probe(const float* verts, int V, const int64_t* faces, int64_t F, int N,
+                          const float* camera /*device[N][16]*/, int H, int W, float z_clip, float area_eps,
+                          const float* screen_pts, int64_t Q, int D, const float* norm_size, const float* fill,
+                          void* workspace, float* out, float* out_tap_zbuf, int64_t* out_tap_face,
+                          recmv_stream_t stream);
+
 /* ---- point rasterizer + alpha compositor: the silhouettes of `pcRender` ------------------------------------------
  * replaces pytorch3d's PointsRasterizer + AlphaCompositor (model/CameraMine.py:347-415, weights 1 - d / r^2).
  * points [N,P,3] f32 already projected: (NDC x, NDC y, view z); pixel (row, col) has its centre at NDC

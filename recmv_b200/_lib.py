@@ -123,6 +123,10 @@ SIGNATURES = {
     "recmv_raster_workspace_bytes": (c_int, [c_int, c_int64, c_int, c_int, c_int64, POINTER(c_size_t)]),
     "recmv_rasterize_meshes": (c_int, [c_void_p, c_int, c_void_p, c_int64, c_int, c_void_p, c_int, c_int, c_float, c_float,
                                        c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "recmv_zbuf_probe_workspace_bytes": (c_int, [c_int, c_int64, c_int, c_int, POINTER(c_size_t)]),
+    "recmv_zbuf_probe": (c_int, [c_void_p, c_int, c_void_p, c_int64, c_int, c_void_p, c_int, c_int, c_float, c_float,
+                                 c_void_p, c_int64, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                 c_void_p]),
     "recmv_points_raster_workspace_bytes": (c_int, [c_int, c_int64, c_int, c_int, c_int64, POINTER(c_size_t)]),
     "recmv_rasterize_points": (c_int, [c_void_p, c_void_p, c_int, c_int64, c_int, c_int, c_float, c_int, c_int64, c_int,
                                        c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),

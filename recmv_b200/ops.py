@@ -1403,6 +1403,38 @@ def rasterize_meshes(verts, faces, cameras, H, W, z_clip=1e-6, area_eps=1e-8, wa
     return p2f, zbuf, bary, dists, counts
 
 
+def zbuf_probe(verts, faces, cameras, H, W, screen_pts, norm_size, fill, z_clip=1e-6, area_eps=1e-8, return_taps=False):
+    """Sparse z-buffer probe (recmv_zbuf_probe, DESIGN section 1i): what grid_sample(align_corners=True) of the filled
+    zbuf of rasterize_meshes(verts, faces, cameras, H, W, z_clip, area_eps) returns at the query points, without
+    rasterizing the frame.  verts [N,V,3] f32, faces [F,3] int64, cameras [N,16] f32, screen_pts [N,Q,D] f32 (D >= 2;
+    x, y read), norm_size [N,2] f32 (w, h) and fill [N] f32, all CUDA and contiguous.  Returns out [N,Q] f32, and with
+    return_taps also (tap_zbuf [N,Q,4] f32, tap_face [N,Q,4] int64): the rasterizer's zbuf and packed face at the taps
+    nw, ne, sw, se, (-1, -1) on background and outside the image.  Five launches, no host synchronisation."""
+    for t, name in ((verts, "verts"), (faces, "faces"), (cameras, "cameras"), (screen_pts, "screen_pts"),
+                    (norm_size, "norm_size"), (fill, "fill")):
+        _check_input(t, name)
+    dev = verts.device
+    _expect("zbuf_probe", "verts", verts, torch.float32, ("N", "V", 3))
+    _expect("zbuf_probe", "faces", faces, torch.int64, ("F", 3), dev)
+    N, V, F = int(verts.shape[0]), int(verts.shape[1]), int(faces.shape[0])
+    _expect("zbuf_probe", "cameras", cameras, torch.float32, (N, 16), dev)
+    _expect("zbuf_probe", "screen_pts", screen_pts, torch.float32, (N, "Q", "D"), dev)
+    Q, D = int(screen_pts.shape[1]), int(screen_pts.shape[2])
+    if D < 2:
+        raise RuntimeError(f"zbuf_probe: screen_pts must have at least 2 coordinates, got {D}")
+    _expect("zbuf_probe", "norm_size", norm_size, torch.float32, (N, 2), dev)
+    _expect("zbuf_probe", "fill", fill, torch.float32, (N,), dev)
+    H, W = int(H), int(W)
+    out = torch.empty((N, Q), dtype=torch.float32, device=dev)
+    tz = torch.empty((N, Q, 4), dtype=torch.float32, device=dev) if return_taps else None
+    tf = torch.empty((N, Q, 4), dtype=torch.int64, device=dev) if return_taps else None
+    ws = _scratch(dev, "zbuf_probe_ws", max(_size("recmv_zbuf_probe_workspace_bytes", N, Q, H, W), 1))
+    _launch("recmv_zbuf_probe", verts, _ptr(verts), V, _ptr(faces), F, N, _ptr(cameras), H, W, float(z_clip),
+            float(area_eps), _ptr(screen_pts), Q, D, _ptr(norm_size), _ptr(fill), _ptr(ws), _ptr(out), _ptr(tz),
+            _ptr(tf))
+    return (out, tz, tf) if return_taps else out
+
+
 def _points_dims(points, features, K, split_size):
     """(N, P, split) of a rasterize_points call; split_size None = P (every point in the first image)."""
     _check_input(points, "points")

@@ -47,6 +47,44 @@ def rasterize_meshes(verts, faces, cameras, image_size, z_clip=1e-6, area_eps=1e
     return Fragments(p2f, zbuf, bary, dists)
 
 
+def screen_points(points, cameras):
+    """[N,P,3] world points -> [N,P,3] (sx, sy, view z): the rasterizer's projection (view X R + T, screen (px - fx X/Z,
+    py - fy Y/Z)) as element-wise torch ops on the points' device, with no host read.  It is the screen position of
+    the reference camera's `transform_points_screen` computed without the NDC round trip, so x and y can differ from
+    it in the last bits; the third coordinate is the view depth, not pytorch3d's NDC z."""
+    N = int(points.shape[0])
+    cam = camera_rows(cameras, N, points.device)
+    p = points.float()
+    v = [p[..., 0:1] * cam[:, None, 4 + j:5 + j] + p[..., 1:2] * cam[:, None, 7 + j:8 + j]
+         + p[..., 2:3] * cam[:, None, 10 + j:11 + j] + cam[:, None, 13 + j:14 + j] for j in range(3)]
+    sx = cam[:, None, 2:3] - cam[:, None, 0:1] * v[0] / v[2]
+    sy = cam[:, None, 3:4] - cam[:, None, 1:2] * v[1] / v[2]
+    return torch.cat([sx, sy, v[2]], -1)
+
+
+def zbuf_probe(verts, faces, cameras, image_size, screen_pts, norm_size, fill, z_clip=1e-6, area_eps=1e-8,
+               return_taps=False):
+    """The reference's z-buffer visibility sample without the full frame (csrc/zbuf_probe.cu, DESIGN section 1i):
+    grid_sample(zbuf, uv, align_corners=True)[:, 0, :, 0] with zbuf the rasterize_meshes zbuf of (verts [N,V,3],
+    faces [F,3], cameras, image_size (H, W)), its background (zbuf == -1) replaced by fill [N], and uv = 2 screen_pts
+    [..., :2] / norm_size - 1 per frame (screen_pts [N,Q,D], D >= 2; norm_size [N,2] = (w, h), the reference's
+    `proj_size`).  Returns [N,Q] f32; with return_taps also the rasterizer's (zbuf [N,Q,4], packed face [N,Q,4]) at the
+    taps nw, ne, sw, se, (-1, -1) on background and outside the image.  A non-finite sample position gives 0.
+    Deterministic, no host read; forward only, the inputs are used detached."""
+    H, W = (int(s) for s in image_size)
+    for t, name in ((verts, "verts"), (screen_pts, "screen_pts"), (norm_size, "norm_size"), (fill, "fill")):
+        if not torch.is_tensor(t) or not t.is_cuda:
+            raise RuntimeError(f"zbuf_probe: {name} must be a CUDA tensor (no CPU path)")
+    dev = verts.device
+    N = int(verts.shape[0])
+    cam = camera_rows(cameras, N, dev)
+    return ops.zbuf_probe(verts.detach().float().contiguous(), faces.detach().long().contiguous(), cam, H, W,
+                          screen_pts.detach().float().contiguous(),
+                          norm_size.detach().to(dev, torch.float32).expand(N, 2).contiguous(),
+                          fill.detach().to(dev, torch.float32).reshape(-1).expand(N).contiguous(), z_clip, area_eps,
+                          return_taps)
+
+
 def vertex_normals(verts, faces):
     """Per-vertex normals of N meshes with one face list (pytorch3d's `Meshes.verts_normals_padded` for meshes of equal
     size): verts [N,V,3], faces [F,3] -> [N,V,3] f32, area-weighted, unit length (0 for an unreferenced vertex).

@@ -3,6 +3,7 @@
 import torch
 
 from .. import ops as _ops
+from .. import raster as _raster
 from ..knn import chamfer_distance
 from ..model.Embedder import annealing_weights  # noqa: F401  (utils/utils.py:40-46)
 from ..ops import FastDiff3x3MinvFunction  # noqa: F401    (utils/utils.py:8-18)
@@ -97,6 +98,70 @@ def make_curve_aware_loss(curve_aware, samples=50000):
 
     curve_aware_loss.stream = stream
     return curve_aware_loss
+
+
+def _probe_settings(mask_render):
+    """(cameras, (H, W), z_clip, area_eps) of a `maskRender`: its rasterizer's cameras and settings, the image size an
+    int or (H, W) as in pytorch3d's RasterizationSettings."""
+    r = mask_render.rasterizer
+    s = r.raster_settings
+    size = s.image_size
+    H, W = (int(size), int(size)) if isinstance(size, int) else (int(size[0]), int(size[1]))
+    return r.cameras, (H, W), float(getattr(s, "z_clip", 1e-6)), float(getattr(s, "area_eps", 1e-8))
+
+
+def _cam_z(cameras):
+    """cam_pos()[2] of camera 0 (CameraMine.cam_pos, -R T) as a device 0-d tensor."""
+    if hasattr(cameras, "cam_pos"):
+        return cameras.cam_pos()[2]
+    R, T = (torch.as_tensor(x, dtype=torch.float32) for x in (cameras[2], cameras[3]))
+    return -R.reshape(-1, 3, 3)[0].matmul(T.reshape(-1, 3)[0].view(-1, 1)).view(-1)[2]
+
+
+def fl_visible_by_body_zbuff(self, cameras, d_cond_list, poses, ratio, fl_vs_dict, def_fl_vs, cano_smpl_verts_list,
+                             fl_names, g_i, garment_name, proj_size, N):
+    """`OptimGarmentNetwork.fl_visible_by_body_zbuff` (OptimGarmentNetwork.py:1374-1465) on the sparse z-buffer probe;
+    bind it as `OptimGarmentNetwork.fl_visible_by_body_zbuff = fl_visible_by_body_zbuff` (the Large-Pose class inherits
+    it).  Returns [N,P,2] = (garment check, body check) for the P curve points, with the reference's formulas: c_z =
+    cam_pos()[2] of the renderer's camera 0; garment column z - (s + c_z), s the bilinear sample of the deformed
+    garment's zbuf with background filled by max_v(Z - c_z) over the deformed garment vertices; body column the same
+    for the skinned canonical-SMPL curve points against the skinned `tmpBodyVs` / `tmpBodyFs`.  The zbuf is the one
+    `self.maskRender` would rasterize (its cameras, image size and clip settings); the screen points come from the
+    `cameras` argument and are normalised by `proj_size`.  Only the pixels the samples read are rasterized
+    (raster.zbuf_probe), nothing is read back to the host, and the deformers run without a graph: the result is
+    detached, as the reference's outputs feed only `<` comparisons."""
+    rcams, size, z_clip, area_eps = _probe_settings(self.maskRender)
+    with torch.no_grad():
+        c_z = _cam_z(rcams).detach()
+        def_garment_vs = self.deformer(self.garment_vs[g_i][None, :, :].expand(N, -1, 3), [d_cond_list[g_i + 1], poses],
+                                       ratio=ratio, offset_type=garment_name)
+        fl = torch.cat(def_fl_vs, dim=1).detach()
+        fill = (def_garment_vs[..., -1] - c_z).max(-1)[0]
+        s = _raster.zbuf_probe(def_garment_vs, self.garment_fs[g_i], rcams, size, _raster.screen_points(fl, cameras),
+                               proj_size, fill, z_clip, area_eps)
+        garment_check = fl[..., -1] - (s + c_z)
+        smpl_fl = torch.cat([self.deformer.defs[1](v.expand(N, -1, 3), poses)
+                             for v, _ in zip(cano_smpl_verts_list, fl_names)], dim=1)
+        body = self.deformer.defs[1](self.tmpBodyVs.view(1, -1, 3).expand(N, -1, 3), poses)
+        fill = (body[..., -1] - c_z).max(-1)[0]
+        s = _raster.zbuf_probe(body, self.tmpBodyFs, rcams, size, _raster.screen_points(smpl_fl, cameras), proj_size,
+                               fill, z_clip, area_eps)
+        smpl_check = smpl_fl[..., -1] - (s + c_z)
+    return torch.stack([garment_check, smpl_check], -1)
+
+
+def check_zbuf_body(smpl_mesh, N, deform_lbs, poses, trans, cameras, mask_render, img_size, screen_pts):
+    """`engineer.core.fl_optimizer.check_zbuf_body` (fl_optimizer.py:30-59) on the sparse z-buffer probe; bind it as
+    `fl_optimizer.check_zbuf_body = check_zbuf_body`.  Returns [N,Q]: the bilinear sample, at the caller's screen
+    points normalised by img_size [N,2] = (w, h), of the skinned body's zbuf with background filled by the raw maximum
+    vertex z.  Sets `mask_render.rasterizer.cameras = cameras` as the reference does.  No host read; detached."""
+    mask_render.rasterizer.cameras = cameras
+    _, size, z_clip, area_eps = _probe_settings(mask_render)
+    with torch.no_grad():
+        verts = deform_lbs(smpl_mesh.verts_packed()[None].expand(N, -1, 3), [poses, trans])
+        fill = verts[..., -1].max(-1)[0]
+        return _raster.zbuf_probe(verts, smpl_mesh.faces_packed(), cameras, size, screen_pts, img_size, fill, z_clip,
+                                  area_eps)
 
 
 def compute_Jacobian(ps, ds, retain_graph, create_graph, allow_unused=False):
