@@ -3,7 +3,9 @@ not from any rasterizer's code: every face is tested against every pixel centre 
 
 Camera (model/CameraMine.py): view X_v = X R + T (:169-173), screen (sx, sy) = (px - fx X_v/Z_v, py - fy Y_v/Z_v)
 (:104-142, :273-287), pixel (row, col) centred at (col, row).  A face is skipped when a vertex has Z_v <= z_clip or its
-doubled screen area |A| <= area_eps; it covers a pixel when its three barycentrics (edge functions over A) are >= 0;
+doubled screen area |A| <= area_eps; it covers a pixel when its three barycentrics (edge functions over A) are >= 0
+and the perspective denominator sum_j b_j / Z_j is > 0 (the interpolated point lies in front of the camera plane; only
+a face with a vertex at Z <= 0, which needs z_clip < 0, can fail this);
 b'_i = (b_i/Z_i) / sum_j (b_j/Z_j), zbuf = sum_i b'_i Z_i; the smallest zbuf wins, ties to the lower packed index
 n*F + f; dists = -(squared distance to the nearest edge) in NDC x = 1 - (2 sx + 1)/W, y = 1 - (2 sy + 1)/H.
 
@@ -96,7 +98,8 @@ def _frame(verts, faces, cam, H, W, z_clip, area_eps, margin_px, ztol, face_base
             d[:, i] = b[:, i] * np.abs(A[f]) / np.hypot(X[:, bb] - X[:, a], Y[:, bb] - Y[:, a])   # signed px distance
         pix = row * W + col
         inb = (col >= lo_x[f]) & (col <= hi_x[f]) & (row >= lo_y[f]) & (row <= hi_y[f])
-        covered = (b >= 0).all(1) & inb
+        with np.errstate(divide="ignore", invalid="ignore"):
+            covered = (b >= 0).all(1) & inb & ((b / zz[f]).sum(1) > 0)
         dmin = d.min(1)
         amb[pix[(d > -margin_px).all(1) & (dmin < margin_px)]] = True   # coverage could flip
         f, pix, b = f[covered], pix[covered], b[covered]

@@ -1475,11 +1475,13 @@ def rasterize_points(points, features, H, W, radius, K, split_size=None, want_fr
         _launch("recmv_rasterize_points", points, _ptr(points), _ptr(features), N, P, H, W, float(radius), K, split, G,
                 _ptr(ws), cap, _ptr(images), *(_ptr(t) for t in (frags or (None,) * 3)), _ptr(ctr))
         covered, skipped, pairs, overflow = (int(v) for v in _read_counters(ctr, host))
+        if overflow and pairs >= 0x7fffffff:
+            # before the pair count is kept as the next call's list size: a saturated count would size every later
+            # call's workspace at 8 GiB
+            check(_lib.RECMV_E_RANGE, "recmv_rasterize_points (more than 2^31 - 1 tile / point pairs)")
         _scratch_cache[kept] = max(_scratch_cache.get(kept, 0), pairs)
         if not overflow:
             break
-        if pairs >= 0x7fffffff:
-            check(_lib.RECMV_E_RANGE, "recmv_rasterize_points (more than 2^31 - 1 tile / point pairs)")
         cap = pairs   # grow once to the exact size and re-run
     else:
         raise _lib.RecmvError("recmv_rasterize_points: pair list still too small after growing")
