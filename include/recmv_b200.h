@@ -461,6 +461,27 @@ RECMV_API int recmv_surface_sample_workspace_bytes(int M, int64_t F, size_t* byt
 RECMV_API int recmv_surface_sample(const float* verts, int M, int V, const int64_t* faces, int64_t F, int64_t S,
                           uint64_t seed, uint64_t offset, void* workspace, float* out, recmv_stream_t stream);
 
+/* ---- training-ray sub-sampling: sample_train_ray's mask selection, random draw and view rays -----------------------
+ * replaces engineer/networks/OptimGarmentNetwork.py:983-1055 after `find_surface_ps` (DESIGN section 1j).
+ * G lists (garments); the pointer arguments ending in [G] are HOST arrays of G device pointers.  List g has
+ * lengths[g] (host) rows: batch / row / col int64 [P_g] and init_pts f32 [P_g,3], against masks[g] f32 [N,H,W].
+ * Candidates are the rows with mask[b, r, c] > 0 (NaN fails; an index outside the mask is not a candidate), in input
+ * order; pnum_g is their count.  pnum_g <= target keeps every candidate; otherwise candidate j is kept iff u_j < thr,
+ * thr = (float)((double)target / (double)pnum_g), u_j = (x0 >> 8) * 2^-24 with x0 the first word of Philox4x32-10 under
+ * key (seed lo, seed hi) at counter (lo, hi, 0, 0) of offset + P_0 + ... + P_{g-1} + j.  Kept rows go, in candidate
+ * order, to the capacity outputs out_* [P_g] / [P_g,3]: batch, row, col and init point copied bit for bit, and the view
+ * ray of camera 0 (camera: DEVICE f32 >= 13 = {fx, fy, px, py, R row-major}, raster.camera_rows' layout) by the formula
+ * of recmv_fragment_decode.  counts: DEVICE int32[G] <- kept rows per list.  Five launches per 8 lists, no atomics
+ * (bit-identical from run to run), no host synchronisation.  P_g > 2^31 - 1 is RECMV_E_RANGE.
+ * workspace: recmv_train_rays_workspace_bytes(G, lengths).                                                            */
+RECMV_API int recmv_train_rays_workspace_bytes(int G, const int64_t* lengths, size_t* bytes);
+RECMV_API int recmv_train_rays_sample(int G, const int64_t* const* batch, const int64_t* const* row,
+                             const int64_t* const* col, const float* const* init_pts, const int64_t* lengths,
+                             const float* const* masks, int N, int H, int W, const float* camera, int64_t target,
+                             uint64_t seed, uint64_t offset, void* workspace, int64_t* const* out_batch,
+                             int64_t* const* out_row, int64_t* const* out_col, float* const* out_pts,
+                             float* const* out_rays, int32_t* counts, recmv_stream_t stream);
+
 /* ---- nearest neighbour (K = 1 knn_points): the feature-curve chamfer loss and template registration --------------
  * replaces pytorch3d's KNN extension behind `knn_points` / `chamfer_distance` (DESIGN section 1e).
  * p1 [N,P1,D] queries, p2 [N,P2,D] candidates, f32, D = 2 or 3; lengths1 / lengths2 DEVICE int64[N] or NULL (= P1, P2),

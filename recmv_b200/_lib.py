@@ -139,6 +139,10 @@ SIGNATURES = {
     "recmv_surface_sample_workspace_bytes": (c_int, [c_int, c_int64, POINTER(c_size_t)]),
     "recmv_surface_sample": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int64, c_int64, c_uint64, c_uint64, c_void_p,
                                      c_void_p, c_void_p]),
+    "recmv_train_rays_workspace_bytes": (c_int, [c_int, POINTER(c_int64), POINTER(c_size_t)]),
+    "recmv_train_rays_sample": (c_int, [c_int] + [POINTER(c_void_p)] * 4 + [POINTER(c_int64), POINTER(c_void_p), c_int,
+                                        c_int, c_int, c_void_p, c_int64, c_uint64, c_uint64, c_void_p]
+                                + [POINTER(c_void_p)] * 5 + [c_void_p, c_void_p]),
     "recmv_knn_workspace_bytes":(c_int, [c_int, c_int64, c_int64, POINTER(c_size_t)]),
     "recmv_knn_nearest": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int64, c_int64, c_int, c_void_p,
                                   c_void_p, c_void_p, c_void_p]),

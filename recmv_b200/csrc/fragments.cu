@@ -2,8 +2,7 @@
 // Replaces utils/FindSurfacePs.py:7-60 (FindSurfacePs: `nonzero`, torch_scatter `scatter(min)`, three gathers, an
 // index_select of the mesh, several host syncs) and the ray construction that follows it in the training step
 // (model/CameraMine.py:146-167 view_rays, called from OptimGarmentNetwork.py:1046-1050 sample_train_ray), plus the
-// ground-truth mask filter of sample_train_ray (:1006-1011).  The random sub-sampling of sample_train_ray stays on the
-// host (its RNG is a CPU torch.rand over the compacted list).
+// ground-truth mask filter of sample_train_ray (:1006-1011).
 //
 // Per pixel (n, r, c) with K fragments: first k with pix_to_face >= 0 and all three barycentrics > 0; covered pixels are
 // emitted in (n, r, c) order -- the order `nonzero` gives the reference -- with
@@ -12,6 +11,7 @@
 //   ray   = normalize(-c / fx + px / fx, -r / fy + py / fy, 1) @ R^T        (optional)
 // HBM-bound: 8 K + 12 K bytes read per pixel, 64 bytes written per covered pixel.
 #include "common.cuh"
+#include "compact.cuh"
 
 namespace recmv {
 namespace {
@@ -48,34 +48,7 @@ __global__ void __launch_bounds__(kFragThreads) frag_count_kernel(const long lon
 
 // exclusive scan of the block counts (one CTA; nb <= a few thousand for a 1024^2 x 4 batch), total -> counters[0]
 __global__ void __launch_bounds__(1024) frag_scan_kernel(int* __restrict__ block_counts, int nb, int* __restrict__ counters) {
-  __shared__ int warp_sums[32];
-  __shared__ int carry_s;
-  if (threadIdx.x == 0) carry_s = 0;
-  __syncthreads();
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  for (int base = 0; base < nb; base += 1024) {
-    const int b = base + threadIdx.x;
-    const int v = b < nb ? block_counts[b] : 0;
-    int inc = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const int t = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += t; }
-    if (lane == 31) warp_sums[wid] = inc;
-    __syncthreads();
-    if (wid == 0) {
-      const int w = warp_sums[lane];
-      int wi = w;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) { const int t = __shfl_up_sync(0xffffffffu, wi, o); if (lane >= o) wi += t; }
-      warp_sums[lane] = wi - w;
-    }
-    __syncthreads();
-    const int carry = carry_s;
-    if (b < nb) block_counts[b] = carry + warp_sums[wid] + inc - v;
-    __syncthreads();
-    if (threadIdx.x == 1023) carry_s = carry + warp_sums[31] + inc;
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) counters[0] = carry_s;
+  scan_block_counts(block_counts, nb, counters);
 }
 
 __global__ void __launch_bounds__(kFragThreads) frag_emit_kernel(
@@ -107,17 +80,10 @@ __global__ void __launch_bounds__(kFragThreads) frag_emit_kernel(
     out_pts[3 * (size_t)slot + a] = __fadd_rn(__fadd_rn(t0, t1), t2);
   }
   if (cam.enabled && out_rays) {
-    // CameraMine.view_rays with ps = (col, row, 1): every operation rounded separately, as the torch expression does
-    const float x = (float)c, y = (float)r;
-    float v0 = __fadd_rn(__fdiv_rn(-x, cam.fx), __fdiv_rn(cam.px, cam.fx));
-    float v1 = __fadd_rn(__fdiv_rn(-y, cam.fy), __fdiv_rn(cam.py, cam.fy));
-    float v2 = 1.f;
-    const float nrm = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(v0, v0), __fmul_rn(v1, v1)), __fmul_rn(v2, v2)));
-    v0 = __fdiv_rn(v0, nrm); v1 = __fdiv_rn(v1, nrm); v2 = __fdiv_rn(v2, nrm);
+    float ray[3];
+    view_ray(cam.fx, cam.fy, cam.px, cam.py, cam.R, (float)c, (float)r, ray);
 #pragma unroll
-    for (int i = 0; i < 3; ++i)
-      out_rays[3 * (size_t)slot + i] = __fadd_rn(__fadd_rn(__fmul_rn(v0, cam.R[3 * i]), __fmul_rn(v1, cam.R[3 * i + 1])),
-                                                 __fmul_rn(v2, cam.R[3 * i + 2]));
+    for (int i = 0; i < 3; ++i) out_rays[3 * (size_t)slot + i] = ray[i];
   }
 }
 

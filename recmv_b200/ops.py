@@ -1568,6 +1568,51 @@ def surface_sample(verts, faces, count, seed, offset=0):
     return out
 
 
+def train_rays_sample(batch, row, col, init_pts, masks, camera, target, seed, offset=0):
+    """sample_train_ray's selection for G garments (recmv_train_rays_sample, DESIGN section 1j).  batch, row, col: G
+    int64 [P_g] tensors, init_pts: G f32 [P_g,3], masks: G f32 [N,H,W], camera: f32 [>= 13] or [M,16] (row 0 used,
+    raster.camera_rows' layout), all CUDA and on one device.  Rows with mask > 0 are candidates; a garment with more
+    than `target` of them keeps candidate j iff its uniform (Philox4x32-10 counter offset + P_0 + ... + P_{g-1} + j)
+    is below fp32(target / pnum).  Returns G tuples (batch, row, col, init points, view rays) of the kept rows in input
+    order; the stream advances by P_0 + ... + P_{G-1}.  Five launches per 8 garments and one host synchronisation:
+    the read of the G kept counts."""
+    G = len(batch)
+    if not (len(row) == len(col) == len(init_pts) == len(masks) == G):
+        raise RuntimeError("train_rays_sample: batch, row, col, init_pts and masks must have one entry per garment")
+    if G == 0:
+        return []
+    _check_input(masks[0], "masks")
+    dev = masks[0].device
+    shape = tuple(masks[0].shape)
+    if len(shape) != 3:
+        raise RuntimeError(f"train_rays_sample: masks must be [N,H,W], got {shape}")
+    lists = []
+    for g in range(G):
+        for t, name in ((batch[g], "batch"), (row[g], "row"), (col[g], "col"), (init_pts[g], "init_pts"),
+                        (masks[g], "masks")):
+            _check_input(t, name)
+        P = int(batch[g].shape[0])
+        _expect("train_rays_sample", "masks", masks[g], torch.float32, shape, dev)
+        for t, name in ((batch[g], "batch"), (row[g], "row"), (col[g], "col")):
+            _expect("train_rays_sample", name, t, torch.int64, (P,), dev)
+        _expect("train_rays_sample", "init_pts", init_pts[g], torch.float32, (P, 3), dev)
+        lists.append((P, tuple(torch.empty((P,), dtype=torch.int64, device=dev) for _ in range(3))
+                      + tuple(torch.empty((P, 3), dtype=torch.float32, device=dev) for _ in range(2))))
+    _check_input(camera, "camera")
+    if camera.device != dev or camera.dtype != torch.float32 or camera.numel() < 13:
+        raise RuntimeError(f"train_rays_sample: camera must be f32 with >= 13 values on {dev}")
+    lengths = (ctypes.c_int64 * G)(*[P for P, _ in lists])
+    ptrs = lambda ts: (ctypes.c_void_p * G)(*[t.data_ptr() for t in ts])  # noqa: E731
+    ws = _scratch(dev, "train_rays_ws", max(_size("recmv_train_rays_workspace_bytes", G, lengths), 1))
+    ctr, host = _counters(dev, f"train_rays_counts_{G}", G)
+    N, H, W = shape
+    _launch("recmv_train_rays_sample", masks[0], G, ptrs(batch), ptrs(row), ptrs(col), ptrs(init_pts), lengths,
+            ptrs(masks), N, H, W, _ptr(camera), int(target), int(seed) % (1 << 64), int(offset) % (1 << 64), _ptr(ws),
+            *[ptrs([o[k] for _, o in lists]) for k in range(5)], _ptr(ctr))
+    n = _read_counters(ctr, host).tolist()
+    return [tuple(t[:n[g]] for t in o) for g, (_, o) in enumerate(lists)]
+
+
 def shade_phong(frags, verts, normals, colors, faces, params):
     """Hard Phong shading of K = 1 mesh fragments (recmv_shade_phong).  frags: an object with pix_to_face [N,H,W,1]
     int64 and bary_coords [N,H,W,1,3] f32 (raster.Fragments), or the tuple of rasterize_meshes; verts, normals [N,V,3]

@@ -1,5 +1,7 @@
 """Mirror of the hot-path helpers of the reference's `utils` package (utils/utils.py:8-18,40-46,133-156,
 198-264).  Same names, arguments and return values; the native calls go to librecmv_b200.so."""
+import sys
+
 import torch
 
 from .. import ops as _ops
@@ -98,6 +100,55 @@ def make_curve_aware_loss(curve_aware, samples=50000):
 
     curve_aware_loss.stream = stream
     return curve_aware_loss
+
+
+def make_sample_train_ray():
+    """`OptimGarmentNetwork.sample_train_ray` (OptimGarmentNetwork.py:983-1055) with the selection on the GPU; bind it
+    as `OptimGarmentNetwork.sample_train_ray = make_sample_train_ray()` (the Large-Pose class inherits it).
+    As the reference: `sample_pix_num` from `self.conf` when present, // `self.garment_size`; per garment the rows whose
+    ground-truth mask is > 0 and, when more than T = sample_pix * N of them remain, a Bernoulli draw at fp32(T / pnum);
+    a `RectifiedPerspectiveCameras` (looked up in the bound class's module) from `self.dataset.get_camera_parameters`,
+    assigned to `self.maskRender.rasterizer.cameras` and to `self.pcRender.rasterizer.cameras` when `pcRender` is set;
+    returns (batch, row, col, init points, rays) lists and the cameras.  Unlike the reference, all garments go through
+    one launch sequence (csrc/train_rays.cu) with one host read, the G kept counts, and the uniforms come from a
+    Philox4x32-10 stream whose seed is drawn from torch's CPU generator at the first call and whose offset advances by
+    the garments' input rows per call; both are in the returned function's `stream` dict.  When the camera's
+    focal_length, principal_point or R requires grad, the rays are the camera's own `view_rays` of the kept (col, row),
+    so the graph is the reference's; otherwise they come from the kernel.  The init points are returned detached (the
+    fragment decode that produces them has no graph)."""
+    stream = {"seed": None, "offset": 0}
+
+    def sample_train_ray(self, N, sample_pix, gt_garment_masks_list, batch_garment_inds_list, batch_garment_row_list,
+                         batch_garment_col_list, batch_garment_init_pts_list, frame_ids, device):
+        sample_pix = self.conf.get_int('sample_pix_num') if 'sample_pix_num' in self.conf else sample_pix
+        sample_pix = sample_pix // self.garment_size
+        for t in list(gt_garment_masks_list) + list(batch_garment_inds_list):
+            if not t.is_cuda:
+                raise RuntimeError("sample_train_ray runs on CUDA tensors only (no CPU path)")
+        focals, princeple_ps, Rs, Ts, H, W = self.dataset.get_camera_parameters(frame_ids.numel(), device)
+        cameras_cls = sys.modules[type(self).__module__].RectifiedPerspectiveCameras
+        cameras = cameras_cls(focals, princeple_ps, Rs, Ts, image_size=[(W, H)]).to(device)
+        self.maskRender.rasterizer.cameras = cameras
+        if self.pcRender:
+            self.pcRender.rasterizer.cameras = cameras
+        if stream["seed"] is None:
+            stream["seed"] = int(torch.empty((), dtype=torch.int64).random_())
+        masks = [m.float().contiguous() for m in gt_garment_masks_list]
+        cam = _raster.camera_rows(cameras, int(cameras.R.reshape(-1, 9).shape[0]), device)[0].detach()
+        kept = _ops.train_rays_sample([b.long().contiguous() for b in batch_garment_inds_list],
+                                      [r.long().contiguous() for r in batch_garment_row_list],
+                                      [c.long().contiguous() for c in batch_garment_col_list],
+                                      [p.detach().float().contiguous() for p in batch_garment_init_pts_list], masks,
+                                      cam, sample_pix * N, stream["seed"], stream["offset"])
+        stream["offset"] += sum(int(b.shape[0]) for b in batch_garment_inds_list)
+        out = [list(x) for x in zip(*kept)] if kept else [[] for _ in range(5)]
+        if any(t.requires_grad for t in (cameras.focal_length, cameras.principal_point, cameras.R)):
+            out[4] = [cameras.view_rays(torch.cat([c.view(-1, 1), r.view(-1, 1), torch.ones_like(c.view(-1, 1))],
+                                                  dim=-1).float()) for r, c in zip(out[1], out[2])]
+        return out[0], out[1], out[2], out[3], out[4], cameras
+
+    sample_train_ray.stream = stream
+    return sample_train_ray
 
 
 def _probe_settings(mask_render):
