@@ -482,6 +482,63 @@ RECMV_API int recmv_train_rays_sample(int G, const int64_t* const* batch, const 
                              int64_t* const* out_row, int64_t* const* out_col, float* const* out_pts,
                              float* const* out_rays, int32_t* counts, recmv_stream_t stream);
 
+/* ---- surface-render loss points: surface_render_loss's eikonal / regulariser samples and the `check` compaction -----
+ * replaces engineer/networks/OptimGarmentNetwork.py:1103-1167's CPU draws and boolean indexing (DESIGN section 1k).
+ * G garments; the pointer arguments ending in [G] are HOST arrays of G device pointers; M[g] (surface-solve points)
+ * and V[g] (MC vertices, >= 1) are host int64.  Garment g: init_pts f32 [M_g,3], verts f32 [V_g,3], check uint8 [M_g],
+ * batch / row / col int64 [M_g], rays f32 [M_g,3].  S = 4096 // G; thr_g = (float)((double)S / (double)V_g).
+ * Counter of row i of lane l (0 E-draw, 1 D-draw, 2 E-local, 3 E-global, 4 D-local) of garment g:
+ * offset + 5 (C_0 + ... + C_{g-1}) + l C_g + i, C_g = M_g + V_g; Philox4x32-10 under key (seed lo, seed hi) at counter
+ * (lo, hi, 0, 0).  Vertex v is kept in lane E / D iff (x0 >> 8) 2^-24 < thr_g (E-draw / D-draw row v).
+ * recmv_loss_points_count: DEVICE counts int32[3G] <- (kept E, kept D, checked) per garment; two launches per 8
+ * garments, no host synchronisation.  The caller reads the counts and passes them (HOST int32[3G]) to
+ * recmv_loss_points_emit, which writes, with B_L = cat(init_pts, kept_L vertices in index order):
+ *   out_eikonal[g] f32 [|B_E| + |B_E| / 6, 3] = cat(B_E + 0.01 z (E-local row), global rows fp32(fp32(u 3.6f) - 1.8f)
+ *                  with u = (x_k >> 8) 2^-24, k = coordinate (E-global row));
+ *   out_regular[g] f32 [2 |B_D|, 3] = cat(B_D, B_D + 0.01 z (D-local row));
+ *   out_pts / out_rays [checked, 3], out_batch / out_row / out_col / out_index int64 [checked]: the rows whose check is
+ *   non-zero, in order, copied bit for bit, and their input indices.
+ * z = (r0 cos 2 pi ub, r0 sin 2 pi ub, r1 cos 2 pi ud) in double, r = sqrt(-2 ln ((x >> 8) + 1) 2^-24) of x0 / x2,
+ * ub / ud = (x >> 8) 2^-24 of x1 / x3, rounded to f32; a local point is x + fp32(z 0.01f).  The workspace
+ * (recmv_loss_points_workspace_bytes(G, M, V)) carries the draws from count to emit.  No atomics (bit-identical from
+ * run to run).  V_g = 0 is RECMV_E_SHAPE; C_g > 2^31 - 1 is RECMV_E_RANGE.                                           */
+RECMV_API int recmv_loss_points_workspace_bytes(int G, const int64_t* M, const int64_t* V, size_t* bytes);
+RECMV_API int recmv_loss_points_count(int G, const int64_t* M, const int64_t* V, const uint8_t* const* check, int S,
+                             uint64_t seed, uint64_t offset, void* workspace, int32_t* counts, recmv_stream_t stream);
+RECMV_API int recmv_loss_points_emit(int G, const float* const* init_pts, const int64_t* M, const float* const* verts,
+                            const int64_t* V, const int64_t* const* batch, const int64_t* const* row,
+                            const int64_t* const* col, const float* const* rays, const int32_t* counts, int S,
+                            uint64_t seed, uint64_t offset, void* workspace, float* const* out_eikonal,
+                            float* const* out_regular, float* const* out_pts, float* const* out_rays,
+                            int64_t* const* out_batch, int64_t* const* out_row, int64_t* const* out_col,
+                            int64_t* const* out_index, recmv_stream_t stream);
+
+/* ---- per-frame means of the photometric terms: torch_scatter's scatter(e, batch, reduce='mean', dim_size=N).mean() --
+ * L = (1/N) sum_b [sum_{i in b} e_i / max(1, n_b)] (an empty frame gives 0; a row whose frame lies outside [0, N) is
+ * not counted), with f64 partials over fixed 1024-row chunks combined in chunk order: no float atomics, bit-identical
+ * from run to run (DESIGN section 1k).  loss: DEVICE f32[1]; counts: DEVICE int32[N] <- n_b, kept for the backward;
+ * grad_loss: DEVICE f32[1].  workspace: recmv_frame_loss_workspace_bytes(M, N).  N <= 0 is RECMV_E_SHAPE.
+ * colour: e_i = sum_ch |gt[b, r, c, ch] - colors[i, ch]| (f32, channels in order), gt f32 [N,H,W,3]; an index outside
+ *   gt is not counted.  Backward dcolors [M,3] = -sign(gt - colors) g / (N max(1, n_b)), sign(0) = 0.
+ * normal: gtn [M,3], J [M,3,3] (row a = grad of D_a), nx [M,3], w [M] f32; nn = |gtn| (double), valid iff nn > 1e-4,
+ *   n = gtn / nn, d = J^T n - nx, e_i = |d| w_i over the valid rows.  Backward to gtn, J and nx (w is constant; 0 at
+ *   |d| = 0 and for invalid rows).                                                                                   */
+RECMV_API int recmv_frame_loss_workspace_bytes(int64_t M, int N, size_t* bytes);
+RECMV_API int recmv_color_frame_mean(const float* gt, int N, int H, int W, const int64_t* batch, const int64_t* row,
+                            const int64_t* col, const float* colors, int64_t M, void* workspace, float* loss,
+                            int32_t* counts, recmv_stream_t stream);
+RECMV_API int recmv_color_frame_mean_backward(const float* gt, int N, int H, int W, const int64_t* batch,
+                                     const int64_t* row, const int64_t* col, const float* colors, int64_t M,
+                                     const int32_t* counts, const float* grad_loss, float* dcolors,
+                                     recmv_stream_t stream);
+RECMV_API int recmv_normal_frame_mean(const float* gtn, const float* J, const float* nx, const float* w,
+                             const int64_t* batch, int64_t M, int N, void* workspace, float* loss, int32_t* counts,
+                             recmv_stream_t stream);
+RECMV_API int recmv_normal_frame_mean_backward(const float* gtn, const float* J, const float* nx, const float* w,
+                                      const int64_t* batch, int64_t M, int N, const int32_t* counts,
+                                      const float* grad_loss, float* dgtn, float* dJ, float* dnx,
+                                      recmv_stream_t stream);
+
 /* ---- nearest neighbour (K = 1 knn_points): the feature-curve chamfer loss and template registration --------------
  * replaces pytorch3d's KNN extension behind `knn_points` / `chamfer_distance` (DESIGN section 1e).
  * p1 [N,P1,D] queries, p2 [N,P2,D] candidates, f32, D = 2 or 3; lengths1 / lengths2 DEVICE int64[N] or NULL (= P1, P2),

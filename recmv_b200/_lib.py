@@ -6,7 +6,7 @@ FastMinv/M3x3Inv.cpp:4-6).
 """
 import ctypes
 import os
-from ctypes import (POINTER, Structure, c_char_p, c_double, c_float, c_int, c_int64, c_size_t,
+from ctypes import (POINTER, Structure, c_char_p, c_double, c_float, c_int, c_int32, c_int64, c_size_t,
                     c_uint64, c_void_p)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -143,6 +143,18 @@ SIGNATURES = {
     "recmv_train_rays_sample": (c_int, [c_int] + [POINTER(c_void_p)] * 4 + [POINTER(c_int64), POINTER(c_void_p), c_int,
                                         c_int, c_int, c_void_p, c_int64, c_uint64, c_uint64, c_void_p]
                                 + [POINTER(c_void_p)] * 5 + [c_void_p, c_void_p]),
+    "recmv_loss_points_workspace_bytes": (c_int, [c_int, POINTER(c_int64), POINTER(c_int64), POINTER(c_size_t)]),
+    "recmv_loss_points_count": (c_int, [c_int, POINTER(c_int64), POINTER(c_int64), POINTER(c_void_p), c_int, c_uint64,
+                                        c_uint64, c_void_p, c_void_p, c_void_p]),
+    "recmv_loss_points_emit": (c_int, [c_int, POINTER(c_void_p), POINTER(c_int64), POINTER(c_void_p), POINTER(c_int64)]
+                               + [POINTER(c_void_p)] * 4 + [POINTER(c_int32), c_int, c_uint64, c_uint64, c_void_p]
+                               + [POINTER(c_void_p)] * 8 + [c_void_p]),
+    "recmv_frame_loss_workspace_bytes": (c_int, [c_int64, c_int, POINTER(c_size_t)]),
+    "recmv_color_frame_mean": (c_int, [c_void_p, c_int, c_int, c_int] + [c_void_p] * 4 + [c_int64] + [c_void_p] * 4),
+    "recmv_color_frame_mean_backward": (c_int, [c_void_p, c_int, c_int, c_int] + [c_void_p] * 4 + [c_int64]
+                                        + [c_void_p] * 4),
+    "recmv_normal_frame_mean": (c_int, [c_void_p] * 5 + [c_int64, c_int] + [c_void_p] * 4),
+    "recmv_normal_frame_mean_backward": (c_int, [c_void_p] * 5 + [c_int64, c_int] + [c_void_p] * 6),
     "recmv_knn_workspace_bytes":(c_int, [c_int, c_int64, c_int64, POINTER(c_size_t)]),
     "recmv_knn_nearest": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int64, c_int64, c_int, c_void_p,
                                   c_void_p, c_void_p, c_void_p]),

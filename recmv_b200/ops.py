@@ -1613,6 +1613,141 @@ def train_rays_sample(batch, row, col, init_pts, masks, camera, target, seed, of
     return [tuple(t[:n[g]] for t in o) for g, (_, o) in enumerate(lists)]
 
 
+def loss_points_sample(init_pts, verts, check, batch, row, col, rays, S, seed, offset=0):
+    """surface_render_loss's sample points and check compaction for G garments (recmv_loss_points_count / _emit, DESIGN
+    section 1k).  Per garment: init_pts f32 [M,3], verts f32 [V,3] (V >= 1), check bool [M], batch / row / col int64
+    [M], rays f32 [M,3], all CUDA and on one device; S = 4096 // G.  Returns G tuples (X_E [|B_E| + |B_E|//6, 3],
+    X_D [2|B_D|, 3], points, rays, batch, row, col, index) with B_L = cat(init_pts, the vertices kept by lane L's draw
+    at fp32(S / V)); the last six are the rows whose check is true, in order, and their input indices.  The stream
+    advances by 5 (C_0 + ... + C_{G-1}), C_g = M_g + V_g.  Three launches per 8 garments and one host
+    synchronisation: the read of the 3G counts that size the outputs."""
+    G = len(init_pts)
+    if not all(len(x) == G for x in (verts, check, batch, row, col, rays)):
+        raise RuntimeError("loss_points_sample: every input list must have one entry per garment")
+    if G == 0:
+        return []
+    _check_input(verts[0], "verts")
+    dev = verts[0].device
+    Ms, Vs = [], []
+    for g in range(G):
+        for t, name in ((init_pts[g], "init_pts"), (verts[g], "verts"), (check[g], "check"), (batch[g], "batch"),
+                        (row[g], "row"), (col[g], "col"), (rays[g], "rays")):
+            _check_input(t, name)
+        M, V = int(init_pts[g].shape[0]), int(verts[g].shape[0])
+        _expect("loss_points_sample", "init_pts", init_pts[g], torch.float32, (M, 3), dev)
+        _expect("loss_points_sample", "verts", verts[g], torch.float32, (V, 3), dev)
+        _expect("loss_points_sample", "check", check[g], torch.bool, (M,), dev)
+        _expect("loss_points_sample", "rays", rays[g], torch.float32, (M, 3), dev)
+        for t, name in ((batch[g], "batch"), (row[g], "row"), (col[g], "col")):
+            _expect("loss_points_sample", name, t, torch.int64, (M,), dev)
+        if V == 0:
+            raise RuntimeError("loss_points_sample: a garment has no vertices (the draw's rate S / V is undefined)")
+        Ms.append(M)
+        Vs.append(V)
+    Mc, Vc = (ctypes.c_int64 * G)(*Ms), (ctypes.c_int64 * G)(*Vs)
+    ptrs = lambda ts: (ctypes.c_void_p * G)(*[t.data_ptr() if t is not None else None for t in ts])  # noqa: E731
+    seed, offset = int(seed) % (1 << 64), int(offset) % (1 << 64)
+    ws = _scratch(dev, "loss_points_ws", max(_size("recmv_loss_points_workspace_bytes", G, Mc, Vc), 1))
+    ctr, host = _counters(dev, f"loss_points_counts_{G}", 3 * G)
+    _launch("recmv_loss_points_count", verts[0], G, Mc, Vc, ptrs(check), int(S), seed, offset, _ptr(ws), _ptr(ctr))
+    n = _read_counters(ctr, host).tolist()
+    outs = []
+    for g in range(G):
+        nE, nD, nc = Ms[g] + n[3 * g], Ms[g] + n[3 * g + 1], n[3 * g + 2]
+        f32 = lambda *s: torch.empty(s, dtype=torch.float32, device=dev)  # noqa: E731
+        i64 = lambda k: torch.empty((k,), dtype=torch.int64, device=dev)  # noqa: E731
+        outs.append((f32(nE + nE // 6, 3), f32(2 * nD, 3), f32(nc, 3), f32(nc, 3), i64(nc), i64(nc), i64(nc), i64(nc)))
+    _launch("recmv_loss_points_emit", verts[0], G, ptrs(init_pts), Mc, ptrs(verts), Vc, ptrs(batch), ptrs(row),
+            ptrs(col), ptrs(rays), (ctypes.c_int32 * (3 * G))(*n), int(S), seed, offset, _ptr(ws),
+            *[ptrs([o[k] for o in outs]) for k in range(8)])
+    return outs
+
+
+def _frame_mean_ws(dev, M, N):
+    return _scratch(dev, "frame_loss_ws", max(_size("recmv_frame_loss_workspace_bytes", int(M), int(N)), 1))
+
+
+class ColorFrameMeanFunction(torch.autograd.Function):
+    """The colour term of surface_render_loss (OptimGarmentNetwork.py:1186-1188) for one garment:
+    apply(colors [M,3] f32, gtCs [N,H,W,3] f32, batch, row, col int64 [M], N) -> 0-d f32
+    (1/N) sum_b mean_{i in b} sum_ch |gtCs[b, r, c, ch] - colors[i, ch]|, an empty frame giving 0 (recmv_color_frame_mean,
+    DESIGN section 1k).  Deterministic; no host synchronisation.  Differentiable in colors (first order)."""
+
+    @staticmethod
+    def forward(ctx, colors, gtCs, batch, row, col, N):
+        colors, gtCs = colors.contiguous(), gtCs.contiguous()
+        for t, name in ((colors, "colors"), (gtCs, "gtCs"), (batch, "batch"), (row, "row"), (col, "col")):
+            _check_input(t, name)
+        dev = colors.device
+        M, N = int(colors.shape[0]), int(N)
+        _expect("color_frame_mean", "gtCs", gtCs, torch.float32, (N, "H", "W", 3), dev)   # the kernel bounds b by N
+        _expect("color_frame_mean", "colors", colors, torch.float32, (M, 3), dev)
+        for t, name in ((batch, "batch"), (row, "row"), (col, "col")):
+            _expect("color_frame_mean", name, t, torch.int64, (M,), dev)
+        H, W = int(gtCs.shape[1]), int(gtCs.shape[2])
+        loss = torch.empty((), dtype=torch.float32, device=dev)
+        counts = torch.empty((N,), dtype=torch.int32, device=dev)
+        _launch("recmv_color_frame_mean", colors, _ptr(gtCs), N, H, W, _ptr(batch), _ptr(row), _ptr(col), _ptr(colors),
+                M, _ptr(_frame_mean_ws(dev, M, N)), _ptr(loss), _ptr(counts))
+        ctx.save_for_backward(colors, gtCs, batch, row, col, counts)
+        ctx.shape = (N, H, W)
+        return loss
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g):
+        if not ctx.needs_input_grad[0]:
+            return None, None, None, None, None, None
+        colors, gtCs, batch, row, col, counts = ctx.saved_tensors
+        N, H, W = ctx.shape
+        g = g.contiguous().float()
+        dcol = torch.empty_like(colors)
+        _launch("recmv_color_frame_mean_backward", colors, _ptr(gtCs), N, H, W, _ptr(batch), _ptr(row), _ptr(col),
+                _ptr(colors), int(colors.shape[0]), _ptr(counts), _ptr(g), _ptr(dcol))
+        return dcol, None, None, None, None, None
+
+
+class NormalFrameMeanFunction(torch.autograd.Function):
+    """The normal term of surface_render_loss (OptimGarmentNetwork.py:1206-1215) for one garment:
+    apply(gtn [M,3], J [M,3,3], nx [M,3], w [M] f32, batch int64 [M], N) -> 0-d f32: rows with nn = |gtn| > 1e-4 are
+    valid, d = J^T (gtn / nn) - nx, and the value is (1/N) sum_b mean_{valid i in b} |d_i| w_i, an empty frame giving 0
+    (recmv_normal_frame_mean, computed in double, DESIGN section 1k).  Deterministic; no host synchronisation.
+    Differentiable (first order) in gtn, J and nx; w is a constant."""
+
+    @staticmethod
+    def forward(ctx, gtn, J, nx, w, batch, N):
+        gtn, J, nx, w = (t.contiguous() for t in (gtn, J, nx, w))
+        for t, name in ((gtn, "gtn"), (J, "J"), (nx, "nx"), (w, "w"), (batch, "batch")):
+            _check_input(t, name)
+        dev = gtn.device
+        M, N = int(gtn.shape[0]), int(N)
+        _expect("normal_frame_mean", "gtn", gtn, torch.float32, (M, 3), dev)
+        _expect("normal_frame_mean", "J", J, torch.float32, (M, 3, 3), dev)
+        _expect("normal_frame_mean", "nx", nx, torch.float32, (M, 3), dev)
+        _expect("normal_frame_mean", "w", w, torch.float32, (M,), dev)
+        _expect("normal_frame_mean", "batch", batch, torch.int64, (M,), dev)
+        loss = torch.empty((), dtype=torch.float32, device=dev)
+        counts = torch.empty((N,), dtype=torch.int32, device=dev)
+        _launch("recmv_normal_frame_mean", gtn, _ptr(gtn), _ptr(J), _ptr(nx), _ptr(w), _ptr(batch), M, N,
+                _ptr(_frame_mean_ws(dev, M, N)), _ptr(loss), _ptr(counts))
+        ctx.save_for_backward(gtn, J, nx, w, batch, counts)
+        ctx.N = N
+        return loss
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g):
+        need = ctx.needs_input_grad
+        if not (need[0] or need[1] or need[2]):
+            return None, None, None, None, None, None
+        gtn, J, nx, w, batch, counts = ctx.saved_tensors
+        g = g.contiguous().float()
+        dgtn, dJ, dnx = torch.empty_like(gtn), torch.empty_like(J), torch.empty_like(nx)
+        _launch("recmv_normal_frame_mean_backward", gtn, _ptr(gtn), _ptr(J), _ptr(nx), _ptr(w), _ptr(batch),
+                int(gtn.shape[0]), ctx.N, _ptr(counts), _ptr(g), _ptr(dgtn), _ptr(dJ), _ptr(dnx))
+        return (dgtn if need[0] else None), (dJ if need[1] else None), (dnx if need[2] else None), None, None, None
+
+
 def shade_phong(frags, verts, normals, colors, faces, params):
     """Hard Phong shading of K = 1 mesh fragments (recmv_shade_phong).  frags: an object with pix_to_face [N,H,W,1]
     int64 and bary_coords [N,H,W,1,3] f32 (raster.Fragments), or the tuple of rasterize_meshes; verts, normals [N,V,3]

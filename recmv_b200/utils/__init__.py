@@ -151,6 +151,123 @@ def make_sample_train_ray():
     return sample_train_ray
 
 
+def make_surface_render_loss():
+    """`OptimGarmentNetwork.surface_render_loss` (OptimGarmentNetwork.py:1083-1219) with its sampling, compaction and
+    per-frame means on the GPU; bind it as `OptimGarmentNetwork.surface_render_loss = make_surface_render_loss()` (the
+    Large-Pose class inherits it).  As the reference: the conf lookups and weights, the branch order, per garment the
+    eikonal term on cat(init points, vertices kept at rate 4096 // G / V) plus local and global samples, the info-only
+    translator forward when `offset_weight` is 0, the regulariser on cat(init points, an independent draw of vertices)
+    and their local samples expanded over the N frames, and, when `info['<name>_rayInfo'][1] > 0`, the colour and
+    normal terms on the checked rows; `self.TmpPs` (fresh leaves with requires_grad), `self.rays`, `self.batch_inds`,
+    `self.row_inds` and `self.col_inds` are set as the reference sets them, for `propagateTmpPsGrad`.
+    Unlike the reference: all garments are sampled and compacted in one launch sequence (ops.loss_points_sample,
+    csrc/loss_points.cu) with the call's one host read; the draws come from a Philox4x32-10 stream whose seed is drawn
+    from torch's CPU generator at the first call and whose offset advances by 5 (M_g + V_g) summed over the garments
+    (both in the returned function's `stream` dict); the frame means are ops.ColorFrameMeanFunction and
+    ops.NormalFrameMeanFunction, so torch_scatter is not needed; the singular-Jacobian fallbacks are selected with
+    `torch.where`, without the reference's host test and print; the info values are detached 0-d tensors (the colour
+    default stays -1.0).  `offset_weight > 0` raises NotImplementedError; CPU tensors raise."""
+    stream = {"seed": None, "offset": 0}
+
+    def surface_render_loss(self, datas, N, cameras, frame_ids, ratio, check_list, gtCs, init_garment_ps_list,
+                            sample_batch_garment_row_list, sample_batch_garment_col_list,
+                            sample_batch_garment_inds_list, sample_rays_list, device):
+        G = self.garment_size
+        self.TmpPs = [None for _ in range(G)]
+        self.rays = [None for _ in range(G)]
+        self.batch_inds = [None for _ in range(G)]
+        self.row_inds = [None for _ in range(G)]
+        self.col_inds = [None for _ in range(G)]
+        conf = self.conf
+        if 'offset_weight' in conf and conf.get_float('offset_weight') > 0.:
+            raise NotImplementedError("surface_render_loss: offset_weight > 0 is not supported")
+        total_loss = 0.
+        d_cond_list, poses, trans, rendcond = self.get_grad_parameters(frame_ids, device)
+        inputs = (list(init_garment_ps_list), [self.garment_vs[g] for g in range(len(init_garment_ps_list))],
+                  list(check_list), list(sample_batch_garment_inds_list), list(sample_batch_garment_row_list),
+                  list(sample_batch_garment_col_list), list(sample_rays_list))
+        for t in [t for ts in inputs for t in ts] + [gtCs]:
+            if not t.is_cuda:
+                raise RuntimeError("surface_render_loss runs on CUDA tensors only (no CPU path)")
+        if stream["seed"] is None:
+            stream["seed"] = int(torch.empty((), dtype=torch.int64).random_())
+        P, V, chk, bi, ri, ci, rays_in = inputs
+        samples = _ops.loss_points_sample([p.detach().float().contiguous() for p in P],
+                                          [v.detach().float().contiguous() for v in V],
+                                          [c.bool().contiguous() for c in chk], [b.long().contiguous() for b in bi],
+                                          [r.long().contiguous() for r in ri], [c.long().contiguous() for c in ci],
+                                          [r.detach().float().contiguous() for r in rays_in], 4096 // G,
+                                          stream["seed"], stream["offset"])
+        stream["offset"] += 5 * sum(int(p.shape[0]) + int(v.shape[0]) for p, v in zip(P, V))
+        for garment_idx, (X_E, X_D, ps, rays_c, batch_c, row_c, col_c, index) in enumerate(samples):
+            garment_name = self.garment_names[garment_idx]
+            net = self.garment_nets[garment_idx]
+            nonmnfld_pnts = X_E.requires_grad_()
+            nonmnfld_grad = net.gradient(nonmnfld_pnts, net(nonmnfld_pnts, ratio))
+            grad_loss = ((nonmnfld_grad.norm(2, dim=-1) - 1) ** 2).mean()
+            self.info['{}_grad_loss'.format(garment_name)] = grad_loss.detach()
+            total_loss += grad_loss * conf.get_float('grad_weight')
+
+            d_cond = d_cond_list[garment_idx + 1]
+            if 'offset_weight' in conf and conf.get_float('offset_weight') == 0.:
+                with torch.no_grad():
+                    self.deformer.defs[0](nonmnfld_pnts.view(1, -1, 3).expand(N, -1, 3), d_cond, ratio=ratio,
+                                          offset_type=garment_name)
+                    def_offloss = self.deformer.defs[0].offset[garment_name].view(-1, 3).norm(p=2, dim=-1).mean()
+                    self.info['{}_offset_loss'.format(garment_name)] = def_offloss.detach()
+            nonmnfld_pnts = None
+            if 'def_regu' in conf and conf.get_float('def_regu.weight') > 0.:
+                def_loss = deformation_regulariser(self.deformer.defs[0], X_D.view(1, -1, 3).expand(N, -1, 3), d_cond,
+                                                   ratio, conf.get_float('def_regu.c'), offset_type=garment_name)
+                self.info['def_{}_loss'.format(garment_name)] = def_loss.detach()
+                total_loss += def_loss * conf.get_float('def_regu.weight')
+
+            self.info['{}_color_loss'.format(garment_name)] = -1.0
+            if self.info['{}_rayInfo'.format(garment_name)][1] > 0:
+                TmpPs = ps
+                TmpPs.requires_grad = True
+                self.TmpPs[garment_idx] = TmpPs
+                rays = sample_rays_list[garment_idx]
+                self.rays[garment_idx] = rays.index_select(0, index) if rays.requires_grad else rays_c
+                self.batch_inds[garment_idx] = batch_c
+                self.col_inds[garment_idx] = col_c
+                self.row_inds[garment_idx] = row_c
+                sdfs = net(TmpPs, ratio)
+                nx = torch.autograd.grad(sdfs, TmpPs, torch.ones_like(sdfs), retain_graph=True, create_graph=True)[0]
+                nx = nx / nx.norm(dim=1, keepdim=True)
+                defconds = [d_cond, [poses, trans]]
+                crays, defVs = _cardinal_rays_where(self.deformer, TmpPs, self.rays[garment_idx], defconds, batch_c,
+                                                    ratio, 'train', offset_type=garment_name)
+                if conf.get_float('color_weight') > 0.:
+                    colors = compute_netRender_color(self.netRender, TmpPs, defVs, nx, crays, net.rendcond,
+                                                     rendcond[batch_c], ratio)
+                    color_loss = _ops.ColorFrameMeanFunction.apply(colors, gtCs.float(), batch_c, row_c, col_c, N)
+                    self.info['{}_color_loss'.format(garment_name)] = color_loss.detach()
+                    total_loss += conf.get_float('color_weight') * color_loss
+                if 'normal' in datas and 'normal_weight' in conf and conf.get_float('normal_weight') > 0.:
+                    if 'weighted_normal' in conf and conf.get_bool('weighted_normal'):
+                        cnx, _ = _deformed_normals_where(net, self.deformer, TmpPs, defconds, batch_c, ratio, 'test',
+                                                         garment_name)
+                        weights = torch.clamp((-self.rays[garment_idx] * cnx.detach()).sum(1).detach(), max=1.,
+                                              min=0.) ** 2
+                    else:
+                        weights = torch.ones(nx.shape[0], device=device)
+                    gtnormals = datas['normal'].to(device)[batch_c, row_c, col_c, :]
+                    R0 = cameras.R[0]     # R[0] @ diag(-1, 1, -1), built without a host-to-device copy
+                    flipped = torch.stack([-R0[:, 0], R0[:, 1], -R0[:, 2]], 1)
+                    gtnormals = (flipped @ gtnormals.view(-1, 3, 1)).view(-1, 3)
+                    ds = self.deformer(TmpPs, defconds, batch_c, ratio=ratio, offset_type=garment_name)
+                    grad_d_p = compute_Jacobian(TmpPs, ds, True, True)
+                    normal_loss = _ops.NormalFrameMeanFunction.apply(gtnormals.float(), grad_d_p.float(), nx.float(),
+                                                                     weights.detach().float(), batch_c, N)
+                    self.info['{}_normal_loss'.format(garment_name)] = normal_loss.detach()
+                    total_loss += conf.get_float('normal_weight') * normal_loss
+        return total_loss
+
+    surface_render_loss.stream = stream
+    return surface_render_loss
+
+
 def _probe_settings(mask_render):
     """(cameras, (H, W), z_clip, area_eps) of a `maskRender`: its rasterizer's cameras and settings, the image size an
     int or (H, W) as in pytorch3d's RasterizationSettings."""
@@ -244,12 +361,24 @@ def _value_and_jacobian(deformer, ps, defconds, batch_inds, ratio, offset_type, 
     return ds, compute_Jacobian(ps, ds, check, check)
 
 
-def compute_cardinal_rays(deformer, ps, rays, defconds, batch_inds, ratio, phase, offset_type=None):
-    """crays = normalize(J^-1 v) with the FastMinv singularity fallback (utils/utils.py:232-250)."""
+def _cardinal_rays(deformer, ps, rays, defconds, batch_inds, ratio, phase, offset_type):
+    """(J^-1 v, FastMinv's ok flags, D(p)): the formula compute_cardinal_rays shares with the drop-ins."""
     check = phase in ('train', 'Train')
     ds, J = _value_and_jacobian(deformer, ps, defconds, batch_inds, ratio, offset_type, check)
     Jinv, ok = FastDiff3x3MinvFunction.apply(J)
-    crays = Jinv.matmul(rays.view(-1, 3, 1)).view(-1, 3)
+    return Jinv.matmul(rays.view(-1, 3, 1)).view(-1, 3), ok, ds
+
+
+def _cardinal_rays_where(deformer, ps, rays, defconds, batch_inds, ratio, phase, offset_type=None):
+    """compute_cardinal_rays with the singular rows' fallback (the view ray) selected on the device: no host read."""
+    crays, ok, ds = _cardinal_rays(deformer, ps, rays, defconds, batch_inds, ratio, phase, offset_type)
+    crays = torch.where(ok[:, None], crays, rays.detach())
+    return crays / crays.norm(dim=1, keepdim=True), ds
+
+
+def compute_cardinal_rays(deformer, ps, rays, defconds, batch_inds, ratio, phase, offset_type=None):
+    """crays = normalize(J^-1 v) with the FastMinv singularity fallback (utils/utils.py:232-250)."""
+    crays, ok, ds = _cardinal_rays(deformer, ps, rays, defconds, batch_inds, ratio, phase, offset_type)
     bad = ~ok
     if bad.sum().item() > 0:
         print('unwished error n_inv_mask:(%d:%d)' % (bad.sum().item(), bad.numel()))
@@ -261,15 +390,28 @@ def compute_cardinal_rays(deformer, ps, rays, defconds, batch_inds, ratio, phase
     return crays, ds
 
 
-def compute_deformed_normals(sdf, deformer, ps, defconds, batch_inds, ratio, phase, offset_type):
-    """n = normalize(J^-T grad sdf) (utils/utils.py:198-230)."""
+def _deformed_normals(sdf, deformer, ps, defconds, batch_inds, ratio, phase, offset_type):
+    """(J^-T grad sdf, FastMinv's ok flags, J, grad sdf, D(p)): the formula compute_deformed_normals shares with the
+    drop-ins."""
     sdfs = sdf(ps, ratio)
     check = phase in ('train', 'Train')
     with _ops.input_grad_only():
         onx = torch.autograd.grad(sdfs, ps, torch.ones_like(sdfs), retain_graph=check, create_graph=check)[0]
     ds, J = _value_and_jacobian(deformer, ps, defconds, batch_inds, ratio, offset_type, check)
     Jinv, ok = FastDiff3x3MinvFunction.apply(J)
-    nx = Jinv.transpose(-2, -1).matmul(onx.view(-1, 3, 1)).view(-1, 3)
+    return Jinv.transpose(-2, -1).matmul(onx.view(-1, 3, 1)).view(-1, 3), ok, J, onx, ds
+
+
+def _deformed_normals_where(sdf, deformer, ps, defconds, batch_inds, ratio, phase, offset_type):
+    """compute_deformed_normals with the singular rows' fallback (J grad sdf) selected on the device: no host read."""
+    nx, ok, J, onx, ds = _deformed_normals(sdf, deformer, ps, defconds, batch_inds, ratio, phase, offset_type)
+    nx = torch.where(ok[:, None], nx, J.matmul(onx.unsqueeze(-1)).view(-1, 3))
+    return nx / nx.norm(dim=1, keepdim=True), ds
+
+
+def compute_deformed_normals(sdf, deformer, ps, defconds, batch_inds, ratio, phase, offset_type):
+    """n = normalize(J^-T grad sdf) (utils/utils.py:198-230)."""
+    nx, ok, J, onx, ds = _deformed_normals(sdf, deformer, ps, defconds, batch_inds, ratio, phase, offset_type)
     bad = ~ok
     if bad.sum().item() > 0:
         print('unwished error n_inv_mask:(%d:%d)' % (bad.sum().item(), bad.numel()))
