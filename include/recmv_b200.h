@@ -672,6 +672,23 @@ RECMV_API int recmv_surface_grad_coeffs(const float* grad_l_p, const float* grad
                               float* def_vec, float* ray_grad /*may be NULL*/, uint8_t* ok, int64_t n,
                               recmv_stream_t stream);
 
+/* ---- implicit-surface gradient of every garment of a call (DESIGN section 1l; OptimGarmentNetwork.py:2159-2313) ----
+ * The per-row algebra of recmv_surface_grad_coeffs (bit-identical per row) over n rows, garment g's rows at
+ * [offsets[g], offsets[g+1]) (offsets: HOST int64[G+1], offsets[0] = 0, non-decreasing, offsets[G] = n).
+ * Per row: sdf_coef [n] = -r0, def_vec [n,3] = r[1:4] (-[v]x), ok [n]; ray_grad [n,3] = r[1:4] [d - c]x when not NULL
+ * (needs d [n,3] and cam_pos = c, DEVICE f32[3]; d - c is formed in the kernel).
+ * Per garment: ok_count int32[G] = its ok rows; cam_grad [G,3] = -sum of its def_vec rows (may be NULL); a garment
+ * without rows gives 0 and 0.  The sums are f64 partials over fixed 1024-row chunks combined in chunk order, the
+ * counts block counts combined in block order: no atomics, bit-identical from run to run and for any grid.
+ * Two launches per 8 garments, no host synchronisation.  workspace: recmv_implicit_grad_workspace_bytes(n, G) bytes
+ * of device memory.  n > 2^31 - 1 is RECMV_E_RANGE.                                                                  */
+RECMV_API int recmv_implicit_grad_workspace_bytes(int64_t n, int G, size_t* bytes);
+RECMV_API int recmv_implicit_grad(const float* grad_l_p, const float* grad_f_p, const float* jac, const float* rays,
+                        const float* d /*may be NULL*/, const float* cam_pos /*[3] or NULL*/,
+                        const int64_t* offsets /*host, G+1*/, int G, float* sdf_coef, float* def_vec,
+                        float* ray_grad /*NULL unless wanted*/, uint8_t* ok, int32_t* ok_count /*[G]*/,
+                        float* cam_grad /*[G,3] or NULL*/, void* workspace, int64_t n, recmv_stream_t stream);
+
 /* Calibration knob of the tensor-core modes.  The tensor core accumulates in fp32 with truncation: each of the K/16
  * MMAs that adds into the full-size accumulator loses on average ~2^-24 of it, a systematic bias towards zero.  The
  * epilogue therefore scales a layer's raw accumulators by (1 + gain_per_kblock * K/64); the default gain is

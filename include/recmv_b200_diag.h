@@ -3,6 +3,8 @@
  *   recmv_sdf_mlp_tc_debug is exported by librecmv_b200.so (it launches the product kernel with its raw-accumulator
  *                          hook enabled) but is declared only here: no reference interface maps to it.
  * Used by tools/tc_bringup.py and tools/tc_stall_profile.py.
+ *   recmv_implicit_grad_grid runs recmv_implicit_grad on a capped grid; tests/test_gpu_propagate.py checks with it
+ *                          that the per-garment reductions do not depend on the launch configuration.
  */
 #ifndef RECMV_B200_DIAG_H_
 #define RECMV_B200_DIAG_H_
@@ -25,6 +27,14 @@ RECMV_API int recmv_sdf_mlp_tc_debug(const float* x, const void* packed, const f
  * producer waits on EMPTY, producer tile loop total (the producer lane of each ring).  n >= 8; reset != 0 clears them.
  * Synchronises the device.                                                                                      */
 RECMV_API int recmv_tc_stall_profile(unsigned long long* counters /*host*/, int n, int reset);
+
+/* recmv_implicit_grad with its row kernel's grid capped at max_ctas CTAs (max_ctas <= 0: the product's grid).  The
+ * results do not depend on the grid; the tests check that with this entry.                                       */
+RECMV_API int recmv_implicit_grad_grid(const float* grad_l_p, const float* grad_f_p, const float* jac,
+                                       const float* rays, const float* d, const float* cam_pos,
+                                       const int64_t* offsets /*host, G+1*/, int G, float* sdf_coef, float* def_vec,
+                                       float* ray_grad, uint8_t* ok, int32_t* ok_count, float* cam_grad,
+                                       void* workspace, int64_t n, int max_ctas, recmv_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -185,6 +185,8 @@ SIGNATURES = {
                                     POINTER(c_float), c_void_p, c_int, c_void_p, c_void_p, POINTER(Voxel), c_float, c_float,
                                     c_float, c_float, c_int, c_int, c_void_p, c_size_t, c_void_p, c_int64, c_void_p]),
     "recmv_surface_grad_coeffs": (c_int, [c_void_p] * 9 + [c_int64, c_void_p]),
+    "recmv_implicit_grad_workspace_bytes": (c_int, [c_int64, c_int, POINTER(c_size_t)]),
+    "recmv_implicit_grad": (c_int, [c_void_p] * 6 + [POINTER(c_int64), c_int] + [c_void_p] * 7 + [c_int64, c_void_p]),
     "recmv_tc_set_acc_gain": (c_int, [c_int, c_float]),
     "recmv_check_async_errors": (c_int, [POINTER(c_int), c_int]),
     "recmv_render_sdf": (c_int, [c_void_p, POINTER(RayMarch), c_void_p, c_void_p, c_void_p, c_int64,
@@ -198,6 +200,8 @@ SIGNATURES = {
 DIAG_SIGNATURES = {
     "recmv_sdf_mlp_tc_debug": (c_int, [c_void_p, c_void_p, POINTER(c_float), c_void_p, c_void_p, c_int64,
                                        c_int, c_int, c_void_p, POINTER(c_int), c_void_p]),
+    "recmv_implicit_grad_grid": (c_int, [c_void_p] * 6 + [POINTER(c_int64), c_int] + [c_void_p] * 7
+                                 + [c_int64, c_int, c_void_p]),
 }
 
 _lib = None

@@ -2070,6 +2070,54 @@ def surface_grad_coeffs(grad_l_p, grad_f_p, jac, rays, d_minus_c=None):
     return coef, vec, rg, ok.view(torch.bool)
 
 
+def implicit_surface_grad(grad_l_p, grad_f_p, jac, rays, d, offsets, cam_pos=None, want_ray_grad=False, _max_ctas=None):
+    """The per-row algebra of propagateTmpPsGrad (OptimGarmentNetwork.py:2213-2311) for every garment of a call, and
+    its per-garment reductions (recmv_implicit_grad, DESIGN section 1l).  grad_l_p, grad_f_p, rays, d f32 [n,3], jac
+    f32 [n,3,3], all CUDA and on one device; offsets: G + 1 host ints, garment g's rows at [offsets[g], offsets[g+1]);
+    cam_pos: the camera centre, f32 [3] on the device, or None.  Returns (sdf_coef [n], def_vec [n,3], ray_grad [n,3]
+    or None, ok [n] bool, ok_count [G] int32, cam_grad [G,3] or None): ray_grad = r[1:4] [d - c]x when want_ray_grad
+    (needs d and cam_pos), cam_grad = -sum of each garment's def_vec rows when cam_pos is given.  Deterministic; no
+    host synchronisation (a CUDA `offsets` tensor raises, as reading it would be one)."""
+    if torch.is_tensor(offsets):
+        if offsets.is_cuda:
+            raise RuntimeError("implicit_surface_grad: offsets must be host integers")
+        offsets = offsets.tolist()
+    offs = [int(o) for o in offsets]
+    G = len(offs) - 1
+    if G < 0:
+        raise RuntimeError("implicit_surface_grad: offsets needs G + 1 >= 1 entries")
+    names = ("grad_l_p", "grad_f_p", "jac", "rays")
+    for t, name in zip((grad_l_p, grad_f_p, jac, rays), names):
+        _check_input(t, name)
+    dev = grad_l_p.device
+    n = int(grad_l_p.shape[0])
+    for t, name, shape in zip((grad_l_p, grad_f_p, jac, rays), names, ((n, 3), (n, 3), (n, 3, 3), (n, 3))):
+        _expect("implicit_surface_grad", name, t, torch.float32, shape, dev)
+    if offs[0] != 0 or offs[-1] != n or any(b < a for a, b in zip(offs, offs[1:])):
+        raise RuntimeError(f"implicit_surface_grad: offsets must run from 0 to n = {n} without decreasing, got {offs}")
+    if want_ray_grad and (d is None or cam_pos is None):
+        raise RuntimeError("implicit_surface_grad: the ray gradient needs d and cam_pos")
+    if d is not None:
+        _check_input(d, "d")
+        _expect("implicit_surface_grad", "d", d, torch.float32, (n, 3), dev)
+    if cam_pos is not None:
+        _check_input(cam_pos, "cam_pos")
+        _expect("implicit_surface_grad", "cam_pos", cam_pos, torch.float32, (3,), dev)
+    f32 = lambda *s: torch.empty(s, dtype=torch.float32, device=dev)  # noqa: E731
+    coef, vec, ok = f32(n), f32(n, 3), torch.empty((n,), dtype=torch.uint8, device=dev)
+    rg = f32(n, 3) if want_ray_grad else None
+    cnt = torch.empty((G,), dtype=torch.int32, device=dev)
+    camg = f32(G, 3) if cam_pos is not None else None
+    ws = _scratch(dev, "implicit_grad_ws", _size("recmv_implicit_grad_workspace_bytes", n, G))
+    args = [_ptr(t) for t in (grad_l_p, grad_f_p, jac, rays, d, cam_pos)]
+    args += [(ctypes.c_int64 * (G + 1))(*offs), G] + [_ptr(t) for t in (coef, vec, rg, ok, cnt, camg, ws)] + [n]
+    if _max_ctas is None:
+        _launch("recmv_implicit_grad", coef, *args)
+    else:   # the same kernels on a capped grid (include/recmv_b200_diag.h): the results must not change
+        _launch("recmv_implicit_grad_grid", coef, *args, int(_max_ctas))
+    return coef, vec, rg, ok.view(torch.bool), cnt, camg
+
+
 class Svd3x3Function(torch.autograd.Function):
     """(U, S, V) = svd(J), J [N,3,3] float32 CUDA, J = U diag(S) V^T with S descending -- torch.svd's contract, computed
     per matrix in registers (csrc/svd3.cu) instead of the reference's round trip through the host

@@ -268,6 +268,115 @@ def make_surface_render_loss():
     return surface_render_loss
 
 
+def _repeat_rows(t, G):
+    return t.repeat(G, *([1] * (t.dim() - 1)))
+
+
+def make_propagate_tmp_ps_grad():
+    """`propagateTmpPsGrad(self, frame_ids, ratio)` of OptimGarmentNetwork (OptimGarmentNetwork.py:2159-2313) and of
+    OptimGarmentNetwork_LargePose (OptimGarmentNetwork_Large_Pose.py:327-473, which drops the SDF term) with the
+    implicit-surface algebra on the GPU; bind the returned function on both classes, as the Large-Pose class overrides
+    the method.  As the reference: the garments before the first one whose `TmpPs` or `TmpPs.grad` is missing are
+    processed and that one gets `info['<name>_invInfo'] = (-1, -1)` (the reference returns there); the cameras are
+    rebuilt from `self.dataset.get_camera_parameters` with the bound class's module's `RectifiedPerspectiveCameras` and
+    assigned to `self.maskRender.rasterizer.cameras`; v is the camera's `view_rays` of (col, row, 1) when
+    `self.rays[g]` requires grad, else `self.rays[g]` detached, c = `cam_pos()`; b = [grad f ; [v]x J] and
+    r = TmpPs.grad (b^T b)^-1 b^T with FastMinv's rule; -r0 goes back through the garment's SDF (when it has a
+    parameter that requires grad), r[1:4] (-[v]x) through the deformer to its parameters, the garment conditions, the
+    poses and the translations, r[1:4] [d - c]x to v when v requires grad and the sum of -r[1:4] (-[v]x) to c when c
+    requires grad; gradients accumulate into `.grad`; `deformer.defs[0].offset[<name>]` holds the garment's rows.
+    Unlike the reference: grad f comes from each garment net's `value_and_grad`, d and J of all garments from ONE
+    forward-mode deformer launch (conditions stacked [G N, 128], poses and translations repeated G times, row frame
+    g N + b), the algebra and the per-garment reductions from ONE kernel (ops.implicit_surface_grad), and all VJPs from
+    ONE `torch.autograd.backward` (one training forward of the deformer over all rows) instead of the surrogate-loss
+    chain: the sums are the same, the floating-point accumulation order differs.  `info['<name>_invInfo']` is
+    (rows, ok count) with the count a detached 0-d device tensor; the fixed-camera branch reads `self.rays[g]` (the
+    reference's `self.rays.detach()` calls .detach() on the list).  `TmpPs.grad` is left untouched.  No host
+    synchronisation; CPU tensors raise."""
+
+    def propagateTmpPsGrad(self, frame_ids, ratio):
+        names = self.garment_names
+        active = 0
+        while active < self.garment_size and self.TmpPs[active] is not None and self.TmpPs[active].grad is not None:
+            active += 1
+        missing = active < self.garment_size
+        if active > 0:
+            _propagate(self, frame_ids, ratio, active)
+        if missing:
+            self.info['{}_invInfo'.format(names[active])] = (-1, -1)
+
+    return propagateTmpPsGrad
+
+
+def _propagate(self, frame_ids, ratio, G):
+    """propagateTmpPsGrad for garments 0 .. G-1, all of which have TmpPs and TmpPs.grad."""
+    names = self.garment_names
+    ps = [self.TmpPs[g].detach() for g in range(G)]
+    device = ps[0].device
+    for t in ps + [self.TmpPs[g].grad for g in range(G)] + [self.batch_inds[g] for g in range(G)]:
+        if not t.is_cuda:
+            raise RuntimeError("propagateTmpPsGrad runs on CUDA tensors only (no CPU path)")
+    d_cond_list, poses, trans, _ = self.get_grad_parameters(frame_ids, device)
+    focals, princeple_ps, Rs, Ts, H, W = self.dataset.get_camera_parameters(frame_ids.numel(), device)
+    cameras_cls = sys.modules[type(self).__module__].RectifiedPerspectiveCameras
+    cameras = cameras_cls(focals, princeple_ps, Rs, Ts, image_size=[(W, H)]).to(device)
+    self.maskRender.rasterizer.cameras = cameras
+    vs = []
+    for g in range(G):
+        if self.rays[g].requires_grad:
+            col, row = self.col_inds[g].view(-1, 1), self.row_inds[g].view(-1, 1)
+            vs.append(cameras.view_rays(torch.cat([col, row, torch.ones_like(col)], dim=-1).float()))
+        else:
+            vs.append(self.rays[g].detach())
+    c = cameras.cam_pos()
+    offsets = [0]
+    for p in ps:
+        offsets.append(offsets[-1] + int(p.shape[0]))
+    P = torch.cat(ps).float().contiguous()
+    gf = torch.cat([self.garment_nets[g].value_and_grad(ps[g], ratio)[1].reshape(-1, 3) for g in range(G)])
+    # one deformer over all garments: frame g N + b reads garment g's condition row b and pose / translation b
+    N = int(poses.shape[0])
+    conds = torch.cat([d_cond_list[1 + g] for g in range(G)])
+    defconds = [conds, [_repeat_rows(poses, G), _repeat_rows(trans, G)]]
+    binds = torch.cat([self.batch_inds[g].long() + g * N for g in range(G)])
+    fixed = [conds.detach(), [t.detach() for t in defconds[1]]]
+    d, J = _value_and_jacobian(self.deformer, P.requires_grad_(), fixed, binds, ratio, names[0], False)
+    P = P.detach()
+    want_ray_grad = any(v.requires_grad for v in vs)
+    coef, vec, ray_grad, _, ok_count, cam_grad = _ops.implicit_surface_grad(
+        torch.cat([self.TmpPs[g].grad for g in range(G)]).float().contiguous(), gf.float().contiguous(),
+        J.detach().float().contiguous(), torch.cat([v.detach() for v in vs]).float().contiguous(),
+        d.detach().float().contiguous(), offsets, c.detach().float().reshape(3).contiguous(), want_ray_grad)
+    outs, cots = [], []
+    for g in range(G):
+        net = self.garment_nets[g]
+        if any(p.requires_grad for p in net.parameters()):
+            f = net(ps[g], ratio)
+            outs.append(f)
+            cots.append(coef[offsets[g]:offsets[g + 1]].view_as(f).to(f.dtype))
+    dtrain = self.deformer(P, defconds, binds, ratio=ratio, offset_type=names[0])
+    if dtrain.requires_grad:
+        outs.append(dtrain)
+        cots.append(vec.to(dtrain.dtype))
+    for g, v in enumerate(vs):
+        if v.requires_grad:
+            outs.append(v)
+            cots.append(ray_grad[offsets[g]:offsets[g + 1]].to(v.dtype))
+    if c.requires_grad:
+        outs.append(c)
+        cots.append(cam_grad.sum(0).view_as(c).to(c.dtype))
+    if outs:
+        torch.autograd.backward(outs, cots)
+    tr = self.deformer.defs[0]
+    off = getattr(tr, 'offset', {}).get(names[0])
+    if off is not None and off.shape[0] == offsets[-1]:
+        off = off.detach()
+        for g in range(G):
+            tr.offset[names[g]] = off[offsets[g]:offsets[g + 1]]
+    for g in range(G):
+        self.info['{}_invInfo'.format(names[g])] = (offsets[g + 1] - offsets[g], ok_count[g])
+
+
 def _probe_settings(mask_render):
     """(cameras, (H, W), z_clip, area_eps) of a `maskRender`: its rasterizer's cameras and settings, the image size an
     int or (H, W) as in pytorch3d's RasterizationSettings."""
