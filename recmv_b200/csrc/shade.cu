@@ -39,6 +39,12 @@ __global__ void __launch_bounds__(kNormThreads) normals_keys_kernel(const long l
   vals[e] = (unsigned)e;
 }
 
+// |(x, y, z)|^2 in the order the sm_90a compiler contracts the plain x * x + y * y + z * z to, written out so that the
+// float32 restatement in tests/shade_f32.py is exact: y * y rounded, then x and z fused.
+__device__ __forceinline__ float norm2(float x, float y, float z) {
+  return __fmaf_rn(z, z, __fmaf_rn(x, x, __fmul_rn(y, y)));
+}
+
 __global__ void __launch_bounds__(kNormThreads) normals_sum_kernel(const float* __restrict__ verts, int V,
                                                                     const long long* __restrict__ faces,
                                                                     const unsigned* __restrict__ vals,
@@ -67,14 +73,22 @@ __global__ void __launch_bounds__(kNormThreads) normals_sum_kernel(const float* 
     sy += __fsub_rn(__fmul_rn(uz, wx), __fmul_rn(ux, wz));
     sz += __fsub_rn(__fmul_rn(ux, wy), __fmul_rn(uy, wx));
   }
-  const float inv = 1.f / fmaxf(sqrtf(sx * sx + sy * sy + sz * sz), 1e-6f);
+  const float inv = 1.f / fmaxf(sqrtf(norm2(sx, sy, sz)), 1e-6f);
   float* o = out + 3 * gid;
   o[0] = sx * inv; o[1] = sy * inv; o[2] = sz * inv;
 }
 
 __device__ __forceinline__ void normalize3(float& x, float& y, float& z) {
-  const float inv = 1.f / fmaxf(sqrtf(x * x + y * y + z * z), 1e-6f);
+  const float inv = 1.f / fmaxf(sqrtf(norm2(x, y, z)), 1e-6f);
   x *= inv; y *= inv; z *= inv;
+}
+
+// A correctly rounded a * b + c.  The interpolation uses the PTX instruction rather than __fmaf_rn: the two round alike,
+// but the intrinsic leads ptxas to a different schedule than the one the plain, contracted expression compiled to.
+__device__ __forceinline__ float fma_rn(float a, float b, float c) {
+  float d;
+  asm("fma.rn.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));
+  return d;
 }
 
 __global__ void __launch_bounds__(kShadeThreads) shade_phong_kernel(
@@ -96,14 +110,17 @@ __global__ void __launch_bounds__(kShadeThreads) shade_phong_kernel(
     vi[k] += m * V;
   }
   const float b[3] = {bary[3 * pix], bary[3 * pix + 1], bary[3 * pix + 2]};
+  // Every contraction is written out, in the order the compiler chose for the plain expressions, so that the float32
+  // restatement in tests/shade_f32.py is exact; powf is the one operation it does not restate.  The interpolation is
+  // a fused chain over the corners from +0: fma(b2, a2, fma(b1, a1, fma(b0, a0, 0))).
   float P[3] = {0.f, 0.f, 0.f}, Nr[3] = {0.f, 0.f, 0.f}, C[3] = {0.f, 0.f, 0.f};
 #pragma unroll
   for (int k = 0; k < 3; ++k)
 #pragma unroll
     for (int j = 0; j < 3; ++j) {
-      P[j] += b[k] * __ldg(verts + 3 * vi[k] + j);
-      Nr[j] += b[k] * __ldg(normals + 3 * vi[k] + j);
-      C[j] += b[k] * (colors ? __ldg(colors + 3 * vi[k] + j) : 1.f);
+      P[j] = fma_rn(b[k], __ldg(verts + 3 * vi[k] + j), P[j]);
+      Nr[j] = fma_rn(b[k], __ldg(normals + 3 * vi[k] + j), Nr[j]);
+      C[j] = fma_rn(b[k], colors ? __ldg(colors + 3 * vi[k] + j) : 1.f, C[j]);
     }
   float nx = Nr[0], ny = Nr[1], nz = Nr[2];
   normalize3(nx, ny, nz);
@@ -111,18 +128,21 @@ __global__ void __launch_bounds__(kShadeThreads) shade_phong_kernel(
   normalize3(lx, ly, lz);
   float vx = __ldg(prm + 0) - P[0], vy = __ldg(prm + 1) - P[1], vz = __ldg(prm + 2) - P[2];
   normalize3(vx, vy, vz);
-  const float cosl = nx * lx + ny * ly + nz * lz;
-  const float rx = -lx + 2.f * cosl * nx, ry = -ly + 2.f * cosl * ny, rz = -lz + 2.f * cosl * nz;
-  const float sa = cosl > 0.f ? fmaxf(vx * rx + vy * ry + vz * rz, 0.f) : 0.f;
+  // dot products in norm2's order; R = 2 cos N - L with 2 cos exact and each product fused with -L
+  const float cosl = __fmaf_rn(nz, lz, __fmaf_rn(nx, lx, __fmul_rn(ny, ly)));
+  const float c2 = 2.f * cosl;
+  const float rx = __fmaf_rn(nx, c2, -lx), ry = __fmaf_rn(ny, c2, -ly), rz = __fmaf_rn(nz, c2, -lz);
+  const float sa = cosl > 0.f ? fmaxf(__fmaf_rn(vz, rz, __fmaf_rn(vx, rx, __fmul_rn(vy, ry))), 0.f) : 0.f;
   const float spec = powf(sa, __ldg(prm + 24));
   const float dif = fmaxf(cosl, 0.f);
   float rgb[3];
 #pragma unroll
   for (int j = 0; j < 3; ++j) {
-    const float amb = __ldg(prm + 15 + j) * __ldg(prm + 6 + j);
-    const float d = __ldg(prm + 18 + j) * __ldg(prm + 9 + j) * dif;
-    const float s = __ldg(prm + 21 + j) * __ldg(prm + 12 + j) * spec;
-    rgb[j] = (amb + d) * C[j] + s;
+    // (ambient + diffuse) colour + specular: the ambient product fused into the sum, that sum fused with the colour
+    const float ma = __ldg(prm + 15 + j), la = __ldg(prm + 6 + j);
+    const float d = __fmul_rn(__fmul_rn(__ldg(prm + 18 + j), __ldg(prm + 9 + j)), dif);
+    const float s = __fmul_rn(__fmul_rn(__ldg(prm + 21 + j), __ldg(prm + 12 + j)), spec);
+    rgb[j] = __fmaf_rn(__fmaf_rn(ma, la, d), C[j], s);
   }
   out[pix] = make_float4(rgb[0], rgb[1], rgb[2], 1.f);
 }
