@@ -12,6 +12,7 @@
 // HBM-bound: 8 K + 12 K bytes read per pixel, 64 bytes written per covered pixel.
 #include "common.cuh"
 #include "compact.cuh"
+#include "workspace.cuh"
 
 namespace recmv {
 namespace {
@@ -87,14 +88,23 @@ __global__ void __launch_bounds__(kFragThreads) frag_emit_kernel(
   }
 }
 
+struct FragWs { signed char* first; int* block_counts; };
+
+// The block counts follow the first layers with 4-byte alignment.  No kernel reads the 256 bytes after them and
+// nothing records what they were for; they stay so that the size does not change.
+FragWs frag_layout(Carve& c, int64_t npix, int64_t nb) {
+  const FragWs w{c.take<signed char>(npix), c.take<int>(nb, 4)};
+  c.take<char>(256, 4);
+  return w;
+}
+
 }  // namespace
 }  // namespace recmv
 
 using namespace recmv;
 
 extern "C" size_t recmv_fragment_decode_scratch_bytes(int64_t npix) {
-  const int64_t nb = (npix + kFragThreads - 1) / kFragThreads;
-  return (size_t)((npix + 255) & ~(int64_t)255) + (size_t)nb * 4 + 256;
+  return layout_bytes(frag_layout, npix, (npix + kFragThreads - 1) / kFragThreads);
 }
 
 // camera: host float[13] = {fx, fy, px, py, R[9] row-major} or NULL (no rays).  counters: device int32[1] <- count.
@@ -114,21 +124,21 @@ extern "C" int recmv_fragment_decode(const int64_t* pix_to_face, const float* ba
     return RECMV_E_NULL;
   if (camera && !out_rays) return RECMV_E_NULL;
   const int nb = (int)((npix + kFragThreads - 1) / kFragThreads);
-  signed char* first = (signed char*)scratch;
-  int* block_counts = (int*)((char*)scratch + ((npix + 255) & ~(int64_t)255));
+  const FragWs w = carve(scratch, frag_layout, npix, nb);
   FragCamera cam = {};
   if (camera) {
     cam.fx = camera[0]; cam.fy = camera[1]; cam.px = camera[2]; cam.py = camera[3];
     for (int i = 0; i < 9; ++i) cam.R[i] = camera[4 + i];
     cam.enabled = 1;
   }
-  frag_count_kernel<<<nb, kFragThreads, 0, st>>>((const long long*)pix_to_face, bary, mask, npix, K, first, block_counts);
+  frag_count_kernel<<<nb, kFragThreads, 0, st>>>((const long long*)pix_to_face, bary, mask, npix, K, w.first,
+                                                 w.block_counts);
   int s = launch_status();
   if (s) return s;
-  frag_scan_kernel<<<1, 1024, 0, st>>>(block_counts, nb, counters);
+  frag_scan_kernel<<<1, 1024, 0, st>>>(w.block_counts, nb, counters);
   s = launch_status();
   if (s) return s;
-  frag_emit_kernel<<<nb, kFragThreads, 0, st>>>((const long long*)pix_to_face, bary, first, block_counts, verts,
+  frag_emit_kernel<<<nb, kFragThreads, 0, st>>>((const long long*)pix_to_face, bary, w.first, w.block_counts, verts,
                                                 (const long long*)faces, num_faces, npix, H, W, K, cam,
                                                 (long long*)out_batch, (long long*)out_row, (long long*)out_col, out_pts,
                                                 (long long*)out_finds, out_rays);

@@ -10,6 +10,7 @@
 // Forward: one CTA per 1024-row chunk, then one CTA for the frames; backward: one thread per row.  No atomics.
 #include "common.cuh"
 #include "frame_mean.cuh"
+#include "workspace.cuh"
 
 namespace recmv {
 namespace {
@@ -147,8 +148,6 @@ __global__ void __launch_bounds__(kMeanThreads) normal_backward_kernel(const Nor
   }
 }
 
-size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
-
 long long chunks_of(long long M) { return (M + kChunkRows - 1) / kChunkRows; }
 
 int mean_sizes(int64_t M, int N, long long* chunks) {
@@ -158,19 +157,22 @@ int mean_sizes(int64_t M, int N, long long* chunks) {
   return RECMV_OK;
 }
 
+struct MeanWs { double* part_sum; int* part_cnt; };
+
+MeanWs mean_layout(Carve& c, long long chunks, int N) { return {c.take<double>(chunks * N), c.take<int>(chunks * N)}; }
+
 template <class Row>
 int frame_mean(const Row& row, int64_t M, int N, void* workspace, float* loss, int32_t* counts, cudaStream_t st) {
   long long chunks;
   int s = mean_sizes(M, N, &chunks);
   if (s) return s;
   if (!loss || !counts || (chunks > 0 && !workspace)) return RECMV_E_NULL;
-  double* part_sum = (double*)workspace;
-  int* part_cnt = (int*)((char*)workspace + align256((size_t)chunks * N * 8));
+  const MeanWs w = carve(workspace, mean_layout, chunks, N);
   if (chunks > 0) {
-    frame_partials_kernel<<<(unsigned)chunks, kMeanThreads, 0, st>>>(row, (long long)M, N, part_sum, part_cnt);
+    frame_partials_kernel<<<(unsigned)chunks, kMeanThreads, 0, st>>>(row, (long long)M, N, w.part_sum, w.part_cnt);
     if ((s = launch_status())) return s;
   }
-  frame_finish_kernel<<<1, kMeanThreads, 0, st>>>(part_sum, part_cnt, (int)chunks, N, loss, (int*)counts);
+  frame_finish_kernel<<<1, kMeanThreads, 0, st>>>(w.part_sum, w.part_cnt, (int)chunks, N, loss, (int*)counts);
   return launch_status();
 }
 
@@ -186,7 +188,7 @@ extern "C" int recmv_frame_loss_workspace_bytes(int64_t M, int N, size_t* bytes)
   long long chunks;
   const int s = mean_sizes(M, N, &chunks);
   if (s) return s;
-  *bytes = align256((size_t)chunks * N * 8) + align256((size_t)chunks * N * 4);
+  *bytes = layout_bytes(mean_layout, chunks, N);
   return RECMV_OK;
 }
 

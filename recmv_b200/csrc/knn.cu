@@ -194,23 +194,9 @@ int check_shape(int N, long long P1, long long P2) {
   return RECMV_OK;
 }
 
-struct BackwardWs {
-  unsigned *keys_in, *keys_out, *vals_in, *vals_out;
-  int *beg, *end;
-  void* temp;
-};
-
-BackwardWs carve(void* ws, long long M, long long NP2) {
-  BackwardWs w;
-  char* p = (char*)ws;
-  w.keys_in = (unsigned*)p; p += align256((size_t)M * 4);
-  w.keys_out = (unsigned*)p; p += align256((size_t)M * 4);
-  w.vals_in = (unsigned*)p; p += align256((size_t)M * 4);
-  w.vals_out = (unsigned*)p; p += align256((size_t)M * 4);
-  w.beg = (int*)p; p += align256((size_t)NP2 * 4);
-  w.end = (int*)p; p += align256((size_t)NP2 * 4);
-  w.temp = p;
-  return w;
+// the forward's workspace: S keys per query, unpadded
+unsigned long long* forward_layout(Carve& c, int S, long long M) {
+  return c.take<unsigned long long>((size_t)S * M, 8);
 }
 
 template <int D>
@@ -220,7 +206,7 @@ int nearest(const float* p1, const float* p2, const long long* l1, const long lo
   plan(N, P1, P2, &S, &chunk);
   const int qb = (P1 + kKnnThreads - 1) / kKnnThreads;
   const long long NP1 = (long long)N * P1;
-  unsigned long long* keys = (unsigned long long*)ws;
+  unsigned long long* keys = carve(ws, forward_layout, S, NP1);
   knn_scan_kernel<D><<<dim3((unsigned)((long long)N * qb), (unsigned)S), kKnnThreads, 0, st>>>(
       p1, p2, l1, l2, P1, P2, qb, chunk, NP1, keys);
   int s = launch_status();
@@ -234,7 +220,7 @@ template <int D>
 int nearest_backward(const float* p1, const float* p2, const long long* idx, const float* grad, int N, int P1, int P2,
                      void* ws, float* dp1, float* dp2, cudaStream_t st) {
   const long long M = (long long)N * P1, NP2 = (long long)N * P2;
-  BackwardWs w = carve(ws, M, NP2);
+  const SegmentWs w = carve(ws, segment_layout, M, NP2);
   if (M > 0) {
     knn_grad_p1_kernel<D><<<(unsigned)((M + kKnnThreads - 1) / kKnnThreads), kKnnThreads, 0, st>>>(
         p1, p2, idx, grad, P1, P2, M, (unsigned)NP2, dp1, dp2 ? w.keys_in : nullptr, w.vals_in);
@@ -242,7 +228,7 @@ int nearest_backward(const float* p1, const float* p2, const long long* idx, con
     if (s) return s;
   }
   if (!dp2 || NP2 == 0) return RECMV_OK;
-  cudaError_t e = cudaMemsetAsync(w.beg, 0, 2 * align256((size_t)NP2 * 4), st);   // beg and end: empty ranges
+  cudaError_t e = cudaMemsetAsync(w.beg, 0, w.ranges_bytes, st);   // beg and end: empty ranges
   if (e != cudaSuccess) return (int)e;
   if (M > 0) {
     int s = sort_pairs(w.temp, w.keys_in, w.keys_out, w.vals_in, w.vals_out, M, (unsigned)NP2, st);
@@ -272,8 +258,7 @@ extern "C" int recmv_knn_workspace_bytes(int N, int64_t P1, int64_t P2, size_t* 
   size_t temp = 0;
   s = sort_temp_bytes(M, (unsigned)NP2, &temp);
   if (s) return s;
-  const size_t fwd = (size_t)S * (size_t)M * 8;
-  const size_t bwd = 4 * align256((size_t)M * 4) + 2 * align256((size_t)NP2 * 4) + temp;
+  const size_t fwd = layout_bytes(forward_layout, S, M), bwd = layout_bytes(segment_layout, M, NP2) + temp;
   *bytes = fwd > bwd ? fwd : bwd;
   return RECMV_OK;
 }

@@ -36,22 +36,16 @@ struct LapWs {
 
 __host__ __device__ __forceinline__ long long lap_chunks(long long V) { return (V + kLapThreads - 1) / kLapThreads; }
 
-size_t lap_ws_bytes(long long V) {
-  const long long nc = lap_chunks(V);
-  return 18 * align256((size_t)V * 8) + align256((size_t)(nc > 0 ? nc : 1) * kParts * 8);   // one block at V = 0
-}
-
-LapWs carve_lap(void* ws, long long V) {
+LapWs lap_layout(Carve& c, long long V) {
   LapWs w;
-  char* p = (char*)ws;
-  const size_t vec = align256((size_t)V * 8);
   double** vecs[5] = {w.y, w.r, w.p, w.w, w.q};
   for (int a = 0; a < 5; ++a)
-    for (int k = 0; k < 3; ++k, p += vec) vecs[a][k] = (double*)p;
-  w.inv_deg = (double*)p; p += vec;
-  w.dinv = (double*)p; p += vec;
-  w.cc = (double*)p; p += vec;
-  w.part = (double*)p;
+    for (int k = 0; k < 3; ++k) vecs[a][k] = c.take<double>(V);
+  w.inv_deg = c.take<double>(V);
+  w.dinv = c.take<double>(V);
+  w.cc = c.take<double>(V);
+  const long long nc = lap_chunks(V);
+  w.part = c.take<double>((nc > 0 ? nc : 1) * kParts);   // one block at V = 0
   return w;
 }
 
@@ -383,7 +377,7 @@ extern "C" int recmv_lap_edit_workspace_bytes(int64_t V, int64_t M, size_t* byte
   if (!bytes) return RECMV_E_NULL;
   const int s = lap_shape(V, M);
   if (s) return s;
-  *bytes = lap_ws_bytes(V);
+  *bytes = layout_bytes(lap_layout, V);
   return RECMV_OK;
 }
 
@@ -397,7 +391,7 @@ extern "C" int recmv_lap_edit_solve(const float* verts, int64_t V, const int32_t
   if (!row_ptr || !workspace || !stats || (V > 0 && (!verts || !deg || !out)) || (M > 0 && (!cidx || !ctgt)))
     return RECMV_E_NULL;
   cudaStream_t st = (cudaStream_t)stream;
-  LapWs w = carve_lap(workspace, V);
+  const LapWs w = carve(workspace, lap_layout, V);
   const long long nc = lap_chunks(V);
   const unsigned nb = (unsigned)(nc > 0 ? nc : 1);
   const int Vi = (int)V;

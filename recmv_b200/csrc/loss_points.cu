@@ -22,6 +22,7 @@
 #include "common.cuh"
 #include "compact.cuh"
 #include "philox.cuh"
+#include "workspace.cuh"
 
 namespace recmv {
 namespace {
@@ -196,8 +197,6 @@ __global__ void __launch_bounds__(kRowThreads) lp_emit_kernel(const PointLists L
   }
 }
 
-size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
-
 long long tiles_of(long long C) { return (C + kRowThreads - 1) / kRowThreads; }
 
 // rows and blocks of the call, or an error for a bad size
@@ -221,7 +220,9 @@ struct Workspace {
   int* cnt;                               // [3, tiles]: E, D, check
 };
 
-Workspace carve(void* ws, long long rows) { return {(unsigned char*)ws, (int*)((char*)ws + align256((size_t)rows))}; }
+Workspace lp_layout(Carve& c, long long rows, long long tiles) {
+  return {c.take<unsigned char>(rows), c.take<int>(3 * tiles)};
+}
 
 // fills the per-group fields shared by both passes; returns the next group's tile base
 long long group(PointLists& L, int g0, int G, const int64_t* M, const int64_t* V, int S, long long* row_base,
@@ -254,7 +255,7 @@ extern "C" int recmv_loss_points_workspace_bytes(int G, const int64_t* M, const 
   long long rows, tiles;
   const int s = list_sizes(G, M, V, &rows, &tiles);
   if (s) return s;
-  *bytes = align256((size_t)rows) + align256((size_t)tiles * 12);
+  *bytes = layout_bytes(lp_layout, rows, tiles);
   return RECMV_OK;
 }
 
@@ -270,7 +271,7 @@ extern "C" int recmv_loss_points_count(int G, const int64_t* M, const int64_t* V
   for (int g = 0; g < G; ++g)
     if (M[g] > 0 && !check[g]) return RECMV_E_NULL;
   cudaStream_t st = (cudaStream_t)stream;
-  const Workspace w = carve(workspace, rows);
+  const Workspace w = carve(workspace, lp_layout, rows, tiles);
   long long row_base = 0, tile_base = 0;
   unsigned long long ctr = (unsigned long long)offset;
   for (int g0 = 0; g0 < G; g0 += kMaxLists) {
@@ -313,7 +314,7 @@ extern "C" int recmv_loss_points_emit(int G, const float* const* init_pts, const
       return RECMV_E_NULL;
   }
   cudaStream_t st = (cudaStream_t)stream;
-  const Workspace w = carve(workspace, rows);
+  const Workspace w = carve(workspace, lp_layout, rows, tiles);
   long long row_base = 0, tile_base = 0;
   unsigned long long ctr = (unsigned long long)offset;
   for (int g0 = 0; g0 < G; g0 += kMaxLists) {

@@ -20,6 +20,7 @@
 // (atomics-ordered) output they are bit-identical after canonical ordering (tests/golden/mc_ref.npz).
 #include "common.cuh"
 #include "mc_tables.h"
+#include "workspace.cuh"
 
 namespace recmv {
 
@@ -382,19 +383,22 @@ struct McScratch {
   int nb;
 };
 
-static size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
-
-static McScratch carve(void* scratch, int NX, int NY, int NZ) {
+static McScratch mc_layout(Carve& c, int NX, int NY, int NZ) {
   int64_t N = (int64_t)NX * NY * NZ;
   McScratch s;
   s.nb = (int)((N + kMcThreads - 1) / kMcThreads);
-  char* p = (char*)scratch;
   s.nwords = (unsigned)((N + 31) / 32 + 2);
-  s.bits = (unsigned*)p; p += align256((size_t)s.nwords * 4);
-  s.cellinfo = (int*)p; p += align256((size_t)N * 4);
-  s.block_sums = (int2*)p; p += align256((size_t)s.nb * 8);
-  s.totals = (int*)p;
+  s.bits = c.take<unsigned>(s.nwords);
+  s.cellinfo = c.take<int>(N);
+  s.block_sums = c.take<int2>(s.nb);
+  s.totals = c.take<int>(4);
   return s;
+}
+
+static int mc_dims(int NX, int NY, int NZ) {
+  if (NX <= 0 || NY <= 0 || NZ <= 0) return RECMV_E_SHAPE;
+  if ((int64_t)NX * NY * NZ > 2000000000LL) return RECMV_E_RANGE;
+  return RECMV_OK;
 }
 
 }  // namespace recmv
@@ -403,22 +407,13 @@ using namespace recmv;
 
 extern "C" int recmv_mc_scratch_bytes(int NX, int NY, int NZ, size_t* bytes) {
   if (!bytes) return RECMV_E_NULL;
-  if (NX <= 0 || NY <= 0 || NZ <= 0) return RECMV_E_SHAPE;
-  int64_t N = (int64_t)NX * NY * NZ;
-  if (N > 2000000000LL) return RECMV_E_RANGE;
-  int nb = (int)((N + kMcThreads - 1) / kMcThreads);
-  *bytes = align256((size_t)((N + 31) / 32 + 2) * 4) + align256((size_t)N * 4) + align256((size_t)nb * 8) + 256;
+  const int s = mc_dims(NX, NY, NZ);
+  if (s) return s;
+  *bytes = layout_bytes(mc_layout, NX, NY, NZ);
   return RECMV_OK;
 }
 
 namespace {
-int mc_check(const float* sdf, const void* scratch, int NX, int NY, int NZ) {
-  if (!sdf || !scratch) return RECMV_E_NULL;
-  if (NX <= 0 || NY <= 0 || NZ <= 0) return RECMV_E_SHAPE;
-  if ((int64_t)NX * NY * NZ > 2000000000LL) return RECMV_E_RANGE;
-  return ensure_tables();
-}
-
 // passes 0-2: sign mask, per-segment counts, scan (totals stay on the device)
 int mc_classify(const float* sdf, int NX, int NY, int NZ, float iso, const McScratch& sc, cudaStream_t st) {
   const unsigned N = (unsigned)((int64_t)NX * NY * NZ);
@@ -459,10 +454,12 @@ extern "C" int recmv_mc_run(const float* sdf, int NX, int NY, int NZ, float iso,
                             int32_t* counts, recmv_stream_t stream) {
   if (!step || !origin || !counts || !verts || !faces) return RECMV_E_NULL;
   if (cap_verts < 0 || cap_faces < 0) return RECMV_E_SHAPE;
-  int s = mc_check(sdf, scratch, NX, NY, NZ);
+  if (!sdf || !scratch) return RECMV_E_NULL;
+  int s = mc_dims(NX, NY, NZ);
   if (s) return s;
+  if ((s = ensure_tables())) return s;
   cudaStream_t st = (cudaStream_t)stream;
-  McScratch sc = carve(scratch, NX, NY, NZ);
+  const McScratch sc = carve(scratch, mc_layout, NX, NY, NZ);
   s = mc_classify(sdf, NX, NY, NZ, iso, sc, st);
   if (s) return s;
   const int64_t cv = cap_verts < (1 << 25) ? cap_verts : (1 << 25) - 1;   // packed vertex ids are 26 bit signed-safe

@@ -35,31 +35,6 @@ namespace {
 constexpr int kAdjThreads = 256;
 constexpr int kNricpThreads = 256;
 
-inline int key_bits64(unsigned long long max_key) {
-  int bits = 1;
-  while (bits < 64 && (1ull << bits) <= max_key) ++bits;
-  return bits;
-}
-
-inline int sort_keys64_temp(long long M, unsigned long long max_key, size_t* bytes) {
-  *bytes = 0;
-  if (M == 0) return RECMV_OK;
-  const cudaError_t e = cub::DeviceRadixSort::SortKeys(nullptr, *bytes, (const unsigned long long*)nullptr,
-                                                       (unsigned long long*)nullptr, (int)M, 0, key_bits64(max_key));
-  return e == cudaSuccess ? RECMV_OK : (int)e;
-}
-
-inline int sort_keys64(void* temp, const unsigned long long* in, unsigned long long* out, long long M,
-                       unsigned long long max_key, cudaStream_t st) {
-  size_t bytes = 0;
-  int s = sort_keys64_temp(M, max_key, &bytes);
-  if (s) return s;
-  const cudaError_t e =
-      cub::DeviceRadixSort::SortKeys(temp, bytes, in, out, (int)M, 0, key_bits64(max_key), st);
-  if (e != cudaSuccess) return (int)e;
-  return launch_status();
-}
-
 __global__ void __launch_bounds__(kAdjThreads) adj_side_keys_kernel(const long long* __restrict__ faces, long long M,
                                                                      long long V, unsigned long long* __restrict__ keys,
                                                                      uint8_t* __restrict__ boundary) {
@@ -128,12 +103,12 @@ struct AdjWs {
   void* temp;
 };
 
-AdjWs carve_adj(void* ws, long long F) {
+// two key lists of 6F entries and, last, CUB's temporary storage, whose size the size query adds to the bytes taken
+AdjWs adj_layout(Carve& c, long long F) {
   AdjWs w;
-  char* p = (char*)ws;
-  w.a = (unsigned long long*)p; p += align256((size_t)F * 6 * 8);
-  w.b = (unsigned long long*)p; p += align256((size_t)F * 6 * 8);
-  w.temp = p;
+  w.a = c.take<unsigned long long>(6 * F);
+  w.b = c.take<unsigned long long>(6 * F);
+  w.temp = c.take<char>(0, 1);
   return w;
 }
 
@@ -369,14 +344,19 @@ struct StepWs {
 
 int step_blocks(long long V) { return (int)((V + kNricpThreads - 1) / kNricpThreads); }
 
-StepWs carve_step(void* ws, long long V) {
+StepWs step_layout(Carve& c, long long V) {
   StepWs w;
-  char* p = (char*)ws;
-  w.u = (float*)p; p += align256((size_t)V * 12);
-  w.r = (float*)p; p += align256((size_t)V * 12);
-  w.K = (float*)p; p += align256((size_t)V * 48);
-  w.part = (float4*)p;
+  w.u = c.take<float>(3 * V);
+  w.r = c.take<float>(3 * V);
+  w.K = c.take<float>(12 * V);
+  w.part = c.take<float4>(step_blocks(V));
   return w;
+}
+
+int step_shape(long long V) {
+  if (V < 0) return RECMV_E_SHAPE;
+  if (V >= 0x7fffffffLL) return RECMV_E_RANGE;
+  return RECMV_OK;
 }
 
 }  // namespace
@@ -390,11 +370,11 @@ extern "C" int recmv_mesh_adjacency_workspace_bytes(int64_t V, int64_t F, size_t
   if (s) return s;
   const unsigned long long none = (unsigned long long)V * V;
   size_t t1 = 0, t2 = 0;
-  s = sort_keys64_temp(3 * F, none, &t1);
+  s = sort_keys_temp_bytes(3 * F, none, &t1);
   if (s) return s;
-  s = sort_keys64_temp(6 * F, none, &t2);
+  s = sort_keys_temp_bytes(6 * F, none, &t2);
   if (s) return s;
-  *bytes = 2 * align256((size_t)F * 6 * 8) + (t1 > t2 ? t1 : t2);
+  *bytes = layout_bytes(adj_layout, F) + (t1 > t2 ? t1 : t2);
   return RECMV_OK;
 }
 
@@ -406,20 +386,20 @@ extern "C" int recmv_mesh_adjacency(const int64_t* faces, int64_t F, int64_t V, 
   cudaStream_t st = (cudaStream_t)stream;
   const long long M = 3 * F, M2 = 6 * F;
   const unsigned long long none = (unsigned long long)V * V;
-  AdjWs w = carve_adj(workspace, F);
+  const AdjWs w = carve(workspace, adj_layout, F);
   if (M > 0) {
     const long long n1 = M > V ? M : V;
     adj_side_keys_kernel<<<(unsigned)((n1 + kAdjThreads - 1) / kAdjThreads), kAdjThreads, 0, st>>>(
         (const long long*)faces, M, V, w.a, boundary);
     s = launch_status();
     if (s) return s;
-    s = sort_keys64(w.temp, w.a, w.b, M, none, st);
+    s = sort_keys(w.temp, w.a, w.b, M, none, st);
     if (s) return s;
     adj_mark_kernel<<<(unsigned)((M + kAdjThreads - 1) / kAdjThreads), kAdjThreads, 0, st>>>(w.b, M, V, w.a,
                                                                                             boundary);
     s = launch_status();
     if (s) return s;
-    s = sort_keys64(w.temp, w.a, w.b, M2, none, st);
+    s = sort_keys(w.temp, w.a, w.b, M2, none, st);
     if (s) return s;
   } else if (V > 0) {
     cudaError_t e = cudaMemsetAsync(boundary, 0, (size_t)V, st);
@@ -444,9 +424,9 @@ extern "C" int recmv_nricp_warp(const float* X, const float* x, const float* nor
 
 extern "C" int recmv_nricp_workspace_bytes(int64_t V, size_t* bytes) {
   if (!bytes) return RECMV_E_NULL;
-  if (V < 0) return RECMV_E_SHAPE;
-  if (V >= 0x7fffffffLL) return RECMV_E_RANGE;
-  *bytes = 2 * align256((size_t)V * 12) + align256((size_t)V * 48) + align256((size_t)step_blocks(V) * 16);
+  const int s = step_shape(V);
+  if (s) return s;
+  *bytes = layout_bytes(step_layout, V);
   return RECMV_OK;
 }
 
@@ -455,8 +435,9 @@ extern "C" int recmv_nricp_step(const float* x, const float* normals, const floa
                                 const uint8_t* boundary, int64_t V, const recmv_nricp_params_t* prm, float* X,
                                 float* exp_avg, float* exp_avg_sq, float* max_exp_avg_sq, void* workspace,
                                 float* stats, recmv_stream_t stream) {
-  if (V < 0 || T < 0) return RECMV_E_SHAPE;
-  if (V >= 0x7fffffffLL) return RECMV_E_RANGE;
+  if (T < 0) return RECMV_E_SHAPE;
+  int s = step_shape(V);
+  if (s) return s;
   if (!prm || !stats) return RECMV_E_NULL;
   if (prm->step < 1) return RECMV_E_SHAPE;
   if (V == 0) return RECMV_E_SHAPE;   // the loss divides by V
@@ -464,12 +445,12 @@ extern "C" int recmv_nricp_step(const float* x, const float* normals, const floa
       !max_exp_avg_sq || !workspace || (T > 0 && (!target_v || !target_n)))
     return RECMV_E_NULL;
   cudaStream_t st = (cudaStream_t)stream;
-  StepWs w = carve_step(workspace, V);
+  const StepWs w = carve(workspace, step_layout, V);
   const int nb = step_blocks(V);
   nricp_grad_kernel<<<nb, kNricpThreads, 0, st>>>(X, x, normals, target_v, target_n, (const long long*)corr_idx, T,
                                                   row_ptr, col, boundary, (int)V, prm->threshold, prm->gamma, w.u,
                                                   w.r, w.K, w.part);
-  int s = launch_status();
+  s = launch_status();
   if (s) return s;
   // torch.optim.AdamW's scalars, formed in double as its single-tensor step forms them
   const double t = (double)prm->step;

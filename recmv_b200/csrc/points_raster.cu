@@ -26,6 +26,7 @@
 
 #include "common.cuh"
 #include "tile_scan.cuh"
+#include "workspace.cuh"
 
 namespace recmv {
 namespace {
@@ -308,27 +309,31 @@ struct PointsWs {
   int* list;
 };
 
-size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
-
-PointsWs carve(void* ws, long long NP, long long ntiles) {
+PointsWs points_layout(Carve& c, long long NP, long long ntiles, long long capacity) {
   PointsWs w;
-  char* p = (char*)ws;
-  w.recs = (PointRec*)p; p += align256((size_t)NP * sizeof(PointRec));
-  w.point_counts = (int*)p; p += align256((size_t)NP * 4);
-  w.point_off = (long long*)p; p += align256((size_t)(NP + 1) * 8);
-  w.tile_counts = (int*)p; p += align256((size_t)ntiles * 4);
-  w.tile_off = (long long*)p; p += align256((size_t)(ntiles + 1) * 8);
-  w.cursor = (long long*)p; p += align256((size_t)ntiles * 8);
-  w.list = (int*)p;
+  w.recs = c.take<PointRec>(NP);
+  w.point_counts = c.take<int>(NP);
+  w.point_off = c.take<long long>(NP + 1);
+  w.tile_counts = c.take<int>(ntiles);
+  w.tile_off = c.take<long long>(ntiles + 1);
+  w.cursor = c.take<long long>(ntiles);
+  w.list = c.take<int>(capacity);
   return w;
 }
 
+int points_dims(int N, int64_t P, int H, int W) {
+  if (N < 0 || P < 0 || H <= 0 || W <= 0) return RECMV_E_SHAPE;
+  if ((int64_t)N * P > 0x7fffffffLL || (int64_t)N * H * W > 2000000000LL) return RECMV_E_RANGE;
+  return RECMV_OK;
+}
+
 int check_args(int N, int64_t P, int H, int W, float radius, int K, int64_t split_size, int num_images) {
-  if (N < 0 || P < 0 || H <= 0 || W <= 0 || K < 1 || split_size < 0 || split_size > P) return RECMV_E_SHAPE;
+  if (K < 1 || split_size < 0 || split_size > P) return RECMV_E_SHAPE;
   if (!(radius > 0.f) || !isfinite(radius)) return RECMV_E_SHAPE;
   if (num_images != 1 && num_images != 2) return RECMV_E_SHAPE;
+  const int s = points_dims(N, P, H, W);
+  if (s) return s;
   if (K > kMaxK) return RECMV_E_RANGE;
-  if ((int64_t)N * P > 0x7fffffffLL || (int64_t)N * H * W > 2000000000LL) return RECMV_E_RANGE;
   if (N > 65535) return RECMV_E_RANGE;   // frames are the tile pass's grid.y
   return RECMV_OK;
 }
@@ -355,13 +360,12 @@ using namespace recmv;
 
 extern "C" int recmv_points_raster_workspace_bytes(int N, int64_t P, int H, int W, int64_t capacity, size_t* bytes) {
   if (!bytes) return RECMV_E_NULL;
-  if (N < 0 || P < 0 || H <= 0 || W <= 0 || capacity < 0) return RECMV_E_SHAPE;
-  if ((int64_t)N * P > 0x7fffffffLL || capacity > 0x7fffffffLL || (int64_t)N * H * W > 2000000000LL) return RECMV_E_RANGE;
-  const int64_t NP = (int64_t)N * P;
-  const int64_t tiles = (int64_t)N * ((W + kTileW - 1) / kTileW) * ((H + kTileH - 1) / kTileH);
-  *bytes = align256((size_t)NP * sizeof(PointRec)) + align256((size_t)NP * 4) + align256((size_t)(NP + 1) * 8) +
-           align256((size_t)tiles * 4) + align256((size_t)(tiles + 1) * 8) + align256((size_t)tiles * 8) +
-           align256((size_t)capacity * 4);
+  if (capacity < 0) return RECMV_E_SHAPE;
+  const int s = points_dims(N, P, H, W);
+  if (s) return s;
+  if (capacity > 0x7fffffffLL) return RECMV_E_RANGE;
+  const long long ntiles = (long long)N * ((W + kTileW - 1) / kTileW) * ((H + kTileH - 1) / kTileH);
+  *bytes = layout_bytes(points_layout, (long long)N * P, ntiles, capacity);
   return RECMV_OK;
 }
 
@@ -384,7 +388,7 @@ extern "C" int recmv_rasterize_points(const float* points, const float* features
   const int tiles_per_frame = tiles_x * tiles_y;
   const long long ntiles = (long long)N * tiles_per_frame;
   const long long NP = (long long)N * P;
-  PointsWs w = carve(workspace, NP, ntiles);
+  const PointsWs w = carve(workspace, points_layout, NP, ntiles, capacity);
   e = cudaMemsetAsync(w.tile_counts, 0, (size_t)ntiles * 4, st);
   if (e != cudaSuccess) return (int)e;
   const int nb = (int)((NP + kSetupThreads - 1) / kSetupThreads);
@@ -426,7 +430,8 @@ extern "C" int recmv_rasterize_points_backward(int N, int64_t P, int H, int W, f
   const int tiles_per_frame = tiles_x * tiles_y;
   const long long ntiles = (long long)N * tiles_per_frame;
   const long long NP = (long long)N * P;
-  PointsWs w = carve(const_cast<void*>(workspace), NP, ntiles);
+  // the list holds the forward's pairs
+  const PointsWs w = carve(const_cast<void*>(workspace), points_layout, NP, ntiles, pairs);
   TileArgs a{w.recs, w.list, w.tile_off, w.point_off, H, W, tiles_x, tiles_per_frame, K, (int)split_size, num_images,
              (long long)P, radius * radius};
   float2* pg = reinterpret_cast<float2*>(pair_scratch);

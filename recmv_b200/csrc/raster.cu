@@ -26,6 +26,7 @@
 #include "common.cuh"
 #include "raster_common.cuh"
 #include "tile_scan.cuh"
+#include "workspace.cuh"
 
 namespace recmv {
 namespace {
@@ -199,17 +200,21 @@ struct RasterWs {
   int* list;
 };
 
-size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
-
-RasterWs carve(void* ws, long long NF, long long ntiles) {
+RasterWs raster_layout(Carve& c, long long NF, long long ntiles, long long capacity) {
   RasterWs w;
-  char* p = (char*)ws;
-  w.recs = (FaceRec*)p; p += align256((size_t)NF * sizeof(FaceRec));
-  w.tile_counts = (int*)p; p += align256((size_t)ntiles * 4);
-  w.offsets = (long long*)p; p += align256((size_t)(ntiles + 1) * 8);
-  w.cursor = (long long*)p; p += align256((size_t)ntiles * 8);
-  w.list = (int*)p;
+  w.recs = c.take<FaceRec>(NF);
+  w.tile_counts = c.take<int>(ntiles);
+  w.offsets = c.take<long long>(ntiles + 1);
+  w.cursor = c.take<long long>(ntiles);
+  w.list = c.take<int>(capacity);
   return w;
+}
+
+int raster_shape(int N, int64_t F, int H, int W, int64_t capacity) {
+  if (N < 0 || F < 0 || H <= 0 || W <= 0 || capacity < 0) return RECMV_E_SHAPE;
+  if ((int64_t)N * F > 0x7fffffffLL || capacity > 0x7fffffffLL || (int64_t)N * H * W > 2000000000LL)
+    return RECMV_E_RANGE;
+  return RECMV_OK;
 }
 
 }  // namespace
@@ -219,11 +224,10 @@ using namespace recmv;
 
 extern "C" int recmv_raster_workspace_bytes(int N, int64_t F, int H, int W, int64_t capacity, size_t* bytes) {
   if (!bytes) return RECMV_E_NULL;
-  if (N < 0 || F < 0 || H <= 0 || W <= 0 || capacity < 0) return RECMV_E_SHAPE;
-  if ((int64_t)N * F > 0x7fffffffLL || capacity > 0x7fffffffLL || (int64_t)N * H * W > 2000000000LL) return RECMV_E_RANGE;
-  const int64_t tiles = (int64_t)N * ((W + kTileW - 1) / kTileW) * ((H + kTileH - 1) / kTileH);
-  *bytes = align256((size_t)N * F * sizeof(FaceRec)) + align256((size_t)tiles * 4) + align256((size_t)(tiles + 1) * 8) +
-           align256((size_t)tiles * 8) + align256((size_t)capacity * 4);
+  const int s = raster_shape(N, F, H, W, capacity);
+  if (s) return s;
+  const long long ntiles = (long long)N * ((W + kTileW - 1) / kTileW) * ((H + kTileH - 1) / kTileH);
+  *bytes = layout_bytes(raster_layout, (long long)N * F, ntiles, capacity);
   return RECMV_OK;
 }
 
@@ -231,8 +235,9 @@ extern "C" int recmv_rasterize_meshes(const float* verts, int V, const int64_t* 
                                       const float* camera, int H, int W, float z_clip, float area_eps, void* workspace,
                                       int64_t capacity, int64_t* out_pix_to_face, float* out_zbuf, float* out_bary,
                                       float* out_dists, int32_t* counters, recmv_stream_t stream) {
-  if (V < 0 || F < 0 || N < 0 || H <= 0 || W <= 0 || capacity < 0 || (F > 0 && V == 0)) return RECMV_E_SHAPE;
-  if ((int64_t)N * F > 0x7fffffffLL || capacity > 0x7fffffffLL || (int64_t)N * H * W > 2000000000LL) return RECMV_E_RANGE;
+  if (V < 0 || (F > 0 && V == 0)) return RECMV_E_SHAPE;
+  int s = raster_shape(N, F, H, W, capacity);
+  if (s) return s;
   if (N > 65535) return RECMV_E_RANGE;   // frames are the tile pass's grid.y
   if (!counters) return RECMV_E_NULL;
   if (N > 0 && (!camera || !workspace || !out_pix_to_face || !out_zbuf || !out_bary)) return RECMV_E_NULL;
@@ -245,18 +250,18 @@ extern "C" int recmv_rasterize_meshes(const float* verts, int V, const int64_t* 
   const int tiles_per_frame = tiles_x * tiles_y;
   const long long ntiles = (long long)N * tiles_per_frame;
   const long long NF = (long long)N * F;
-  RasterWs w = carve(workspace, NF, ntiles);
+  const RasterWs w = carve(workspace, raster_layout, NF, ntiles, capacity);
   e = cudaMemsetAsync(w.tile_counts, 0, (size_t)ntiles * 4, st);
   if (e != cudaSuccess) return (int)e;
   const int nb = (int)((NF + kSetupThreads - 1) / kSetupThreads);
   if (NF > 0) {
     raster_setup_kernel<<<nb, kSetupThreads, 0, st>>>(verts, V, (const long long*)faces, (int)F, N, camera, H, W, z_clip,
                                                       area_eps, tiles_x, tiles_per_frame, w.recs, w.tile_counts, counters);
-    int s = launch_status();
+    s = launch_status();
     if (s) return s;
   }
   raster_scan_kernel<<<1, kScanThreads, 0, st>>>(w.tile_counts, (int)ntiles, w.offsets, w.cursor, capacity, counters);
-  int s = launch_status();
+  s = launch_status();
   if (s) return s;
   if (NF > 0) {
     raster_emit_kernel<<<nb, kSetupThreads, 0, st>>>(w.recs, NF, (int)F, tiles_x, tiles_per_frame, w.cursor, capacity,

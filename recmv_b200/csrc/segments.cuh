@@ -2,21 +2,22 @@
 // sort groups each slot's items in increasing item order, and segment_bounds_kernel finds every slot's [begin, end)
 // range in the sorted list.  One thread per slot then sums its range in order, so the result is bit-identical from
 // run to run and independent of the SM count.  Used by the vertex normals (shade.cu) and the KNN backward (knn.cu).
+// The mesh adjacency (nricp.cu) uses the 64-bit key sort alone.
 #pragma once
 #include <cub/device/device_radix_sort.cuh>
 
 #include "common.cuh"
+#include "workspace.cuh"
 
 namespace recmv {
 namespace {
 
 constexpr int kSegThreads = 256;
 
-inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
-
-inline int key_bits(unsigned max_key) {   // bits that hold the keys 0..max_key
+template <class K>
+int key_bits(K max_key) {   // bits that hold the keys 0..max_key
   int bits = 1;
-  while (bits < 32 && (1ull << bits) <= (unsigned long long)max_key) ++bits;
+  while (bits < 8 * (int)sizeof(K) && (1ull << bits) <= (unsigned long long)max_key) ++bits;
   return bits;
 }
 
@@ -41,6 +42,50 @@ inline int sort_pairs(void* temp, const unsigned* keys_in, unsigned* keys_out, c
                                                         key_bits(max_key), st);
   if (e != cudaSuccess) return (int)e;
   return launch_status();
+}
+
+// The same two calls for a sort of M keys alone.  Templates, so that only a file that sorts keys instantiates CUB's
+// kernels for them.
+template <class K>
+int sort_keys_temp_bytes(long long M, K max_key, size_t* bytes) {
+  *bytes = 0;
+  if (M == 0) return RECMV_OK;
+  const cudaError_t e =
+      cub::DeviceRadixSort::SortKeys(nullptr, *bytes, (const K*)nullptr, (K*)nullptr, (int)M, 0, key_bits(max_key));
+  return e == cudaSuccess ? RECMV_OK : (int)e;
+}
+
+template <class K>
+int sort_keys(void* temp, const K* in, K* out, long long M, K max_key, cudaStream_t st) {
+  size_t bytes = 0;
+  int s = sort_keys_temp_bytes(M, max_key, &bytes);
+  if (s) return s;
+  const cudaError_t e = cub::DeviceRadixSort::SortKeys(temp, bytes, in, out, (int)M, 0, key_bits(max_key), st);
+  if (e != cudaSuccess) return (int)e;
+  return launch_status();
+}
+
+// The workspace of a segmented sum of M items into S slots: the sort's keys and values, the slots' [beg, end) ranges
+// and, last, CUB's temporary storage, whose sort_temp_bytes the size query adds to the bytes taken.
+struct SegmentWs {
+  unsigned *keys_in, *keys_out, *vals_in, *vals_out;
+  int *beg, *end;
+  size_t ranges_bytes;   // beg and end, which are cleared together
+  void* temp;
+};
+
+inline SegmentWs segment_layout(Carve& c, long long M, long long S) {
+  SegmentWs w;
+  w.keys_in = c.take<unsigned>(M);
+  w.keys_out = c.take<unsigned>(M);
+  w.vals_in = c.take<unsigned>(M);
+  w.vals_out = c.take<unsigned>(M);
+  const size_t ranges = c.used;
+  w.beg = c.take<int>(S);
+  w.end = c.take<int>(S);
+  w.ranges_bytes = c.used - ranges;
+  w.temp = c.take<char>(0, 1);
+  return w;
 }
 
 // The [beg, end) range of every slot k < S in the sorted keys; keys >= S (invalid items) are skipped.  beg and end

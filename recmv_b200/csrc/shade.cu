@@ -147,25 +147,6 @@ __global__ void __launch_bounds__(kShadeThreads) shade_phong_kernel(
   out[pix] = make_float4(rgb[0], rgb[1], rgb[2], 1.f);
 }
 
-struct NormalsWs {
-  unsigned *keys_in, *keys_out, *vals_in, *vals_out;
-  int *beg, *end;
-  void* temp;
-};
-
-NormalsWs carve(void* ws, long long M, int V) {
-  NormalsWs w;
-  char* p = (char*)ws;
-  w.keys_in = (unsigned*)p; p += align256((size_t)M * 4);
-  w.keys_out = (unsigned*)p; p += align256((size_t)M * 4);
-  w.vals_in = (unsigned*)p; p += align256((size_t)M * 4);
-  w.vals_out = (unsigned*)p; p += align256((size_t)M * 4);
-  w.beg = (int*)p; p += align256((size_t)V * 4);
-  w.end = (int*)p; p += align256((size_t)V * 4);
-  w.temp = p;
-  return w;
-}
-
 int normals_shape(int V, int64_t F) {
   if (V < 0 || F < 0) return RECMV_E_SHAPE;
   if (3 * F > 0x7fffffffLL || V == 0x7fffffff) return RECMV_E_RANGE;   // int list positions; V is the sentinel key
@@ -185,7 +166,7 @@ extern "C" int recmv_vertex_normals_workspace_bytes(int V, int64_t F, size_t* by
   size_t temp = 0;
   s = sort_temp_bytes(M, (unsigned)V, &temp);
   if (s) return s;
-  *bytes = 4 * align256((size_t)M * 4) + 2 * align256((size_t)V * 4) + temp;
+  *bytes = layout_bytes(segment_layout, M, V) + temp;
   return RECMV_OK;
 }
 
@@ -199,8 +180,8 @@ extern "C" int recmv_vertex_normals(const float* verts, int N, int V, const int6
   if (!verts || !out_normals || !workspace || (F > 0 && !faces)) return RECMV_E_NULL;
   cudaStream_t st = (cudaStream_t)stream;
   const long long M = 3 * (long long)F;
-  NormalsWs w = carve(workspace, M, V);
-  cudaError_t e = cudaMemsetAsync(w.beg, 0, 2 * align256((size_t)V * 4), st);   // beg and end: empty ranges
+  const SegmentWs w = carve(workspace, segment_layout, M, V);
+  cudaError_t e = cudaMemsetAsync(w.beg, 0, w.ranges_bytes, st);   // beg and end: empty ranges
   if (e != cudaSuccess) return (int)e;
   if (M > 0) {
     const int nb = (int)((M + kNormThreads - 1) / kNormThreads);

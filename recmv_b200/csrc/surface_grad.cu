@@ -17,6 +17,7 @@
 #include "../../include/recmv_b200_diag.h"   // recmv_implicit_grad_grid (diagnostics entry, not in the product header)
 #include "common.cuh"
 #include "frame_mean.cuh"
+#include "workspace.cuh"
 
 namespace recmv {
 namespace {
@@ -192,8 +193,6 @@ __global__ void __launch_bounds__(kMeanThreads) implicit_grad_finish_kernel(cons
   }
 }
 
-size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
-
 long long chunks_of(long long rows) { return (rows + kChunkRows - 1) / kChunkRows; }
 
 // an upper bound of the call's chunks: every garment adds at most one partial chunk
@@ -203,6 +202,13 @@ int grad_sizes(int64_t n, int G) {
   if (n < 0 || G < 0) return RECMV_E_SHAPE;
   if (n > 0x7fffffffLL) return RECMV_E_RANGE;
   return RECMV_OK;
+}
+
+struct GradWs { double* part_sum; int* part_cnt; };
+
+GradWs grad_layout(Carve& c, int64_t n, int G) {
+  const long long chunks = max_chunks(n, G);
+  return {c.take<double>(3 * chunks), c.take<int>(chunks)};
 }
 
 int implicit_grad(const float* grad_l_p, const float* grad_f_p, const float* jac, const float* rays, const float* d,
@@ -219,8 +225,7 @@ int implicit_grad(const float* grad_l_p, const float* grad_f_p, const float* jac
   if (n > 0 && (!grad_l_p || !grad_f_p || !jac || !rays || !sdf_coef || !def_vec || !ok)) return RECMV_E_NULL;
   if (ray_grad && (!d || !cam_pos)) return RECMV_E_NULL;
   const RowIO io{grad_l_p, grad_f_p, jac, rays, d, cam_pos, sdf_coef, def_vec, ray_grad, (unsigned char*)ok};
-  double* part_sum = (double*)workspace;
-  int* part_cnt = (int*)((char*)workspace + align256((size_t)max_chunks(n, G) * 3 * sizeof(double)));
+  const GradWs w = carve(workspace, grad_layout, n, G);
   const int cap = num_sms() * 4;   // the row kernel's residency at 62 registers
   int chunk = 0;
   for (int g0 = 0; g0 < G; g0 += kMaxGarments) {
@@ -238,10 +243,10 @@ int implicit_grad(const float* grad_l_p, const float* grad_f_p, const float* jac
     if (chunks > 0) {
       int grid = chunks < cap ? chunks : cap;
       if (max_ctas > 0 && grid > max_ctas) grid = max_ctas;
-      implicit_grad_kernel<<<grid, kMeanThreads, 0, st>>>(L, io, part_sum, part_cnt);
+      implicit_grad_kernel<<<grid, kMeanThreads, 0, st>>>(L, io, w.part_sum, w.part_cnt);
       if ((s = launch_status())) return s;
     }
-    implicit_grad_finish_kernel<<<L.G, kMeanThreads, 0, st>>>(L, part_sum, part_cnt, ok_count, cam_grad);
+    implicit_grad_finish_kernel<<<L.G, kMeanThreads, 0, st>>>(L, w.part_sum, w.part_cnt, ok_count, cam_grad);
     if ((s = launch_status())) return s;
   }
   return RECMV_OK;
@@ -268,8 +273,7 @@ extern "C" int recmv_implicit_grad_workspace_bytes(int64_t n, int G, size_t* byt
   if (!bytes) return RECMV_E_NULL;
   const int s = grad_sizes(n, G);
   if (s) return s;
-  const size_t chunks = (size_t)max_chunks(n, G);
-  *bytes = align256(chunks * 3 * sizeof(double)) + align256(chunks * sizeof(int));
+  *bytes = layout_bytes(grad_layout, n, G);
   return RECMV_OK;
 }
 

@@ -16,6 +16,7 @@
 
 #include "common.cuh"
 #include "philox.cuh"
+#include "workspace.cuh"
 
 namespace recmv {
 namespace {
@@ -125,8 +126,6 @@ __global__ void __launch_bounds__(kSampleThreads) sample_kernel(const float* __r
   o[2] = __double2float_rn(__dadd_rn(__dadd_rn(__dmul_rn(a, t.e1z), __dmul_rn(b, t.e2z)), t.v0z));
 }
 
-size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
-
 int sample_shape(int M, int V, int64_t F) {
   if (M < 0 || V < 0 || F < 0) return RECMV_E_SHAPE;
   if (M > 65535) return RECMV_E_RANGE;                               // grid.y of the area pass
@@ -135,6 +134,12 @@ int sample_shape(int M, int V, int64_t F) {
 }
 
 long long num_chunks(int64_t F) { return (F + kChunk - 1) / kChunk; }
+
+struct SampleWs { double *local, *tot; };
+
+SampleWs sample_layout(Carve& c, int M, int64_t F) {
+  return {c.take<double>((long long)M * F), c.take<double>((long long)M * num_chunks(F))};
+}
 
 }  // namespace
 }  // namespace recmv
@@ -145,7 +150,7 @@ extern "C" int recmv_surface_sample_workspace_bytes(int M, int64_t F, size_t* by
   if (!bytes) return RECMV_E_NULL;
   const int s = sample_shape(M, 0, F);
   if (s) return s;
-  *bytes = align256((size_t)M * F * 8) + align256((size_t)M * num_chunks(F) * 8);
+  *bytes = layout_bytes(sample_layout, M, F);
   return RECMV_OK;
 }
 
@@ -164,17 +169,16 @@ extern "C" int recmv_surface_sample(const float* verts, int M, int V, const int6
   if (!faces || !workspace || !out || (V > 0 && !verts)) return RECMV_E_NULL;
   cudaStream_t st = (cudaStream_t)stream;
   const long long nch = num_chunks(F);
-  double* local = (double*)workspace;
-  double* tot = (double*)((char*)workspace + align256((size_t)M * F * 8));
+  const SampleWs w = carve(workspace, sample_layout, M, F);
   area_scan_kernel<<<dim3((unsigned)nch, (unsigned)M), kChunk, 0, st>>>(verts, V, (const long long*)faces, F, nch,
-                                                                        local, tot);
+                                                                        w.local, w.tot);
   s = launch_status();
   if (s) return s;
-  chunk_scan_kernel<<<(unsigned)M, 32, 0, st>>>(tot, nch);
+  chunk_scan_kernel<<<(unsigned)M, 32, 0, st>>>(w.tot, nch);
   s = launch_status();
   if (s) return s;
-  sample_kernel<<<(unsigned)blocks, kSampleThreads, 0, st>>>(verts, V, (const long long*)faces, F, nch, local, tot, S,
-                                                             total, (unsigned long long)seed,
+  sample_kernel<<<(unsigned)blocks, kSampleThreads, 0, st>>>(verts, V, (const long long*)faces, F, nch, w.local, w.tot,
+                                                             S, total, (unsigned long long)seed,
                                                              (unsigned long long)offset, out);
   return launch_status();
 }

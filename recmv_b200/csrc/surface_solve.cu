@@ -10,6 +10,7 @@
 // points are frozen by a flag instead of being compacted away, and nothing ever waits for the host.
 #include "../../include/recmv_b200.h"
 #include "common.cuh"
+#include "workspace.cuh"
 
 namespace recmv {
 namespace {
@@ -55,13 +56,24 @@ __global__ void __launch_bounds__(256) surface_update_kernel(float* __restrict__
   }
 }
 
+struct SolveWs { float *f, *gf, *d, *J; };   // SDF value and gradient, deformed point and its Jacobian
+
+// Packed with 4-byte alignment.  No kernel reads the 256 bytes after J and nothing records what they were for; they
+// stay so that the size does not change.
+SolveWs solve_layout(Carve& c, int64_t P) {
+  const SolveWs w{c.take<float>(P, 4), c.take<float>(3 * P, 4), c.take<float>(3 * P, 4), c.take<float>(9 * P, 4)};
+  c.take<char>(256, 4);
+  return w;
+}
+
 }  // namespace
 }  // namespace recmv
 
 using namespace recmv;
 
 extern "C" size_t recmv_surface_solve_workspace(int64_t P) {
-  return P <= 0 ? 0 : (size_t)P * (4 + 12 + 12 + 36) + 256;
+  if (P <= 0) return 0;
+  return layout_bytes(solve_layout, P);
 }
 
 extern "C" int recmv_surface_solve(const float* cam_pos, const float* rays, float* ps, const int64_t* batch_inds,
@@ -78,23 +90,20 @@ extern "C" int recmv_surface_solve(const float* cam_pos, const float* rays, floa
   if (workspace_bytes < recmv_surface_solve_workspace(P)) return RECMV_E_SHAPE;
   if (mode != RECMV_MLP_TC_F16X3 && mode != RECMV_MLP_TC_F16X1) return RECMV_E_UNSUPPORTED;
   cudaStream_t st = (cudaStream_t)stream;
-  float* f = (float*)workspace;
-  float* gf = f + P;
-  float* d = gf + 3 * P;
-  float* J = d + 3 * P;
+  const SolveWs w = carve(workspace, solve_layout, P);
   cudaError_t e = cudaMemsetAsync(ok, 0, (size_t)P, st);
   if (e != cudaSuccess) return (int)e;
   SolveCfg c;
   c.cam[0] = cam_pos[0]; c.cam[1] = cam_pos[1]; c.cam[2] = cam_pos[2];
   c.dthr = dthreshold; c.athr_deg = athreshold_deg; c.w1 = w1; c.w2 = w2;
   for (int round = 0; round <= times; ++round) {
-    int s = recmv_sdf_mlp_fwd_grad(ps, sdf_packed, sdf_pe_w, f, nullptr, gf, P, mode, stream);
+    int s = recmv_sdf_mlp_fwd_grad(ps, sdf_packed, sdf_pe_w, w.f, nullptr, w.gf, P, mode, stream);
     if (s) return s;
     s = recmv_deformer_fwd_jac(ps, conds, batch_inds, batch_inds ? 0 : P, num_frames, tr_packed, tr_pe_w, A, trans, vox,
-                               nullptr, nullptr, d, J, P, mode, stream);
+                               nullptr, nullptr, w.d, w.J, P, mode, stream);
     if (s) return s;
     c.allow_step = round < times ? 1 : 0;
-    surface_update_kernel<<<stride_grid(P, 256, 4), 256, 0, st>>>(ps, rays, f, gf, d, J, ok, P, c);
+    surface_update_kernel<<<stride_grid(P, 256, 4), 256, 0, st>>>(ps, rays, w.f, w.gf, w.d, w.J, ok, P, c);
     s = launch_status();
     if (s) return s;
   }

@@ -19,6 +19,7 @@
 #include "common.cuh"
 #include "compact.cuh"
 #include "philox.cuh"
+#include "workspace.cuh"
 
 namespace recmv {
 namespace {
@@ -141,8 +142,6 @@ __global__ void __launch_bounds__(kRowThreads) tr_emit_kernel(const RayLists L, 
   for (int a = 0; a < 3; ++a) L.out_rays[g][3 * slot + a] = ray[a];
 }
 
-size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
-
 long long tiles_of(int64_t P) { return (P + kRowThreads - 1) / kRowThreads; }
 
 // rows and blocks of the call, or an error for a bad length
@@ -161,6 +160,15 @@ int list_sizes(int G, const int64_t* lengths, long long* rows, long long* tiles)
   return RECMV_OK;
 }
 
+struct RayWs {
+  unsigned char* flags;
+  int *cand, *keep, *pnum;
+};
+
+RayWs rays_layout(Carve& c, int G, long long rows, long long tiles) {
+  return {c.take<unsigned char>(rows), c.take<int>(tiles), c.take<int>(tiles), c.take<int>(G)};
+}
+
 }  // namespace
 }  // namespace recmv
 
@@ -171,7 +179,7 @@ extern "C" int recmv_train_rays_workspace_bytes(int G, const int64_t* lengths, s
   long long rows, tiles;
   const int s = list_sizes(G, lengths, &rows, &tiles);
   if (s) return s;
-  *bytes = align256((size_t)rows) + 2 * align256((size_t)tiles * 4) + align256((size_t)G * 4);
+  *bytes = layout_bytes(rays_layout, G, rows, tiles);
   return RECMV_OK;
 }
 
@@ -197,10 +205,7 @@ extern "C" int recmv_train_rays_sample(int G, const int64_t* const* batch, const
     if (lengths[g] > 0 && (!batch[g] || !row[g] || !col[g] || !init_pts[g] || !masks[g] || !out_batch[g] ||
                            !out_row[g] || !out_col[g] || !out_pts[g] || !out_rays[g]))
       return RECMV_E_NULL;
-  unsigned char* flags = (unsigned char*)workspace;
-  int* cand = (int*)((char*)workspace + align256((size_t)rows));
-  int* keep = (int*)((char*)cand + align256((size_t)tiles * 4));
-  int* pnum = (int*)((char*)keep + align256((size_t)tiles * 4));
+  const RayWs w = carve(workspace, rays_layout, G, rows, tiles);
   long long row_base = 0, tile_base = 0;
   unsigned long long ctr = (unsigned long long)offset;
   for (int g0 = 0; g0 < G; g0 += kMaxLists) {
@@ -224,20 +229,20 @@ extern "C" int recmv_train_rays_sample(int G, const int64_t* const* batch, const
     L.tile_base[L.G] = (int)tile_base;
     const int nb = L.tile_base[L.G] - L.tile_base[0];
     if (nb > 0) {
-      tr_count_kernel<<<nb, kRowThreads, 0, st>>>(L, N, H, W, flags, cand);
+      tr_count_kernel<<<nb, kRowThreads, 0, st>>>(L, N, H, W, w.flags, w.cand);
       if ((s = launch_status())) return s;
     }
-    tr_scan_kernel<<<L.G, 1024, 0, st>>>(L, cand, pnum);
+    tr_scan_kernel<<<L.G, 1024, 0, st>>>(L, w.cand, w.pnum);
     if ((s = launch_status())) return s;
     if (nb > 0) {
-      tr_draw_kernel<<<nb, kRowThreads, 0, st>>>(L, (long long)target, (unsigned long long)seed, flags, cand, pnum,
-                                                 keep);
+      tr_draw_kernel<<<nb, kRowThreads, 0, st>>>(L, (long long)target, (unsigned long long)seed, w.flags, w.cand,
+                                                 w.pnum, w.keep);
       if ((s = launch_status())) return s;
     }
-    tr_scan_kernel<<<L.G, 1024, 0, st>>>(L, keep, counts);
+    tr_scan_kernel<<<L.G, 1024, 0, st>>>(L, w.keep, counts);
     if ((s = launch_status())) return s;
     if (nb > 0) {
-      tr_emit_kernel<<<nb, kRowThreads, 0, st>>>(L, flags, keep, camera);
+      tr_emit_kernel<<<nb, kRowThreads, 0, st>>>(L, w.flags, w.keep, camera);
       if ((s = launch_status())) return s;
     }
   }

@@ -29,6 +29,7 @@
 #include "common.cuh"
 #include "raster_common.cuh"
 #include "tile_scan.cuh"
+#include "workspace.cuh"
 
 namespace recmv {
 namespace {
@@ -190,23 +191,15 @@ struct ProbeWs {
   int* counters;        // the scan's 4 counters (unused: the list always fits)
 };
 
-size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
-
-size_t probe_bytes(long long T, long long ntiles) {
-  return align256((size_t)T * 8) + 2 * align256((size_t)T * 4) + align256((size_t)ntiles * 4) +
-         align256((size_t)(ntiles + 1) * 8) + align256((size_t)ntiles * 8) + align256(16);
-}
-
-ProbeWs carve(void* ws, long long T, long long ntiles) {
+ProbeWs probe_layout(Carve& c, long long T, long long ntiles) {
   ProbeWs w;
-  char* p = (char*)ws;
-  w.keys = (unsigned long long*)p; p += align256((size_t)T * 8);
-  w.tap_pix = (int*)p; p += align256((size_t)T * 4);
-  w.list = (int*)p; p += align256((size_t)T * 4);
-  w.tile_counts = (int*)p; p += align256((size_t)ntiles * 4);
-  w.offsets = (long long*)p; p += align256((size_t)(ntiles + 1) * 8);
-  w.cursor = (long long*)p; p += align256((size_t)ntiles * 8);
-  w.counters = (int*)p;
+  w.keys = c.take<unsigned long long>(T);
+  w.tap_pix = c.take<int>(T);
+  w.list = c.take<int>(T);
+  w.tile_counts = c.take<int>(ntiles);
+  w.offsets = c.take<long long>(ntiles + 1);
+  w.cursor = c.take<long long>(ntiles);
+  w.counters = c.take<int>(4);
   return w;
 }
 
@@ -226,7 +219,7 @@ extern "C" int recmv_zbuf_probe_workspace_bytes(int N, int64_t Q, int H, int W, 
   const int s = probe_dims(N, Q, H, W);
   if (s) return s;
   const long long ntiles = (long long)N * ((W + kTileW - 1) / kTileW) * ((H + kTileH - 1) / kTileH);
-  *bytes = probe_bytes(4ll * N * Q, ntiles);
+  *bytes = layout_bytes(probe_layout, 4ll * N * Q, ntiles);
   return RECMV_OK;
 }
 
@@ -247,7 +240,7 @@ extern "C" int recmv_zbuf_probe(const float* verts, int V, const int64_t* faces,
   const int tiles_x = (W + kTileW - 1) / kTileW, tiles_y = (H + kTileH - 1) / kTileH;
   const int tiles_per_frame = tiles_x * tiles_y;
   const long long ntiles = (long long)N * tiles_per_frame, T = 4 * NQ, NF = (long long)N * F;
-  ProbeWs w = carve(workspace, T, ntiles);
+  const ProbeWs w = carve(workspace, probe_layout, T, ntiles);
   cudaError_t e = cudaMemsetAsync(w.tile_counts, 0, (size_t)ntiles * 4, st);
   if (e != cudaSuccess) return (int)e;
   zprobe_tap_kernel<<<(int)((NQ + kThreads - 1) / kThreads), kThreads, 0, st>>>(
