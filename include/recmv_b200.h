@@ -539,6 +539,23 @@ RECMV_API int recmv_normal_frame_mean_backward(const float* gtn, const float* J,
                                       const float* grad_loss, float* dgtn, float* dJ, float* dnx,
                                       recmv_stream_t stream);
 
+/* ---- mask_loss's ground-truth dilation and soft silhouette IoU, all garments and frames in one call --------------
+ * m[g], gt[g]: DEVICE f32 [N,H,W] per garment (silhouette, ground-truth mask); r: radius, 1..32 (r < 1 is
+ * RECMV_E_SHAPE, r > 32 RECMV_E_RANGE).  Forward writes mgt[g] f32 [N,H,W] = max_pool2d(gt[g], 2r+1, stride 1,
+ * padding r) bit for bit (out-of-image taps ignored, a NaN tap wins); iu f64 [G,N,2] = (I, U) with I = sum m g',
+ * U = sum |(m + g') - m g'| (each pixel term formed in f32, summed in f64 over fixed 32 x 32 tiles, the tiles combined
+ * in order); loss_gn f32 [G,N] = 1 - I / U (NaN when U = 0); loss f32 [G] = mean_n loss_gn.  No float atomics:
+ * bit-identical from run to run (DESIGN section 1m).  workspace: recmv_mask_iou_workspace_bytes(G, N, H, W, r).
+ * Backward: grad_loss DEVICE f32 [G], dm[g] f32 [N,H,W] = -(grad_loss[g] / N) (g' U - I s (1 - g')) / U^2 with
+ * s = sign((m + g') - m g'), sign(0) = 0, in double from the forward's mgt and iu, rounded once.  The host arrays m,
+ * gt, mgt and dm hold G device pointers.  N > 65535 is RECMV_E_RANGE.  No host synchronisation.                    */
+RECMV_API int recmv_mask_iou_workspace_bytes(int G, int N, int H, int W, int r, size_t* bytes);
+RECMV_API int recmv_mask_iou(int G, const float* const* m, const float* const* gt, int N, int H, int W, int r,
+                    void* workspace, float* const* mgt, double* iu, float* loss_gn, float* loss,
+                    recmv_stream_t stream);
+RECMV_API int recmv_mask_iou_backward(int G, const float* const* m, const float* const* mgt, int N, int H, int W,
+                             const double* iu, const float* grad_loss, float* const* dm, recmv_stream_t stream);
+
 /* ---- nearest neighbour (K = 1 knn_points): the feature-curve chamfer loss and template registration --------------
  * replaces pytorch3d's KNN extension behind `knn_points` / `chamfer_distance` (DESIGN section 1e).
  * p1 [N,P1,D] queries, p2 [N,P2,D] candidates, f32, D = 2 or 3; lengths1 / lengths2 DEVICE int64[N] or NULL (= P1, P2),

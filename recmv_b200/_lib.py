@@ -155,6 +155,11 @@ SIGNATURES = {
                                         + [c_void_p] * 4),
     "recmv_normal_frame_mean": (c_int, [c_void_p] * 5 + [c_int64, c_int] + [c_void_p] * 4),
     "recmv_normal_frame_mean_backward": (c_int, [c_void_p] * 5 + [c_int64, c_int] + [c_void_p] * 6),
+    "recmv_mask_iou_workspace_bytes": (c_int, [c_int] * 5 + [POINTER(c_size_t)]),
+    "recmv_mask_iou": (c_int, [c_int, POINTER(c_void_p), POINTER(c_void_p)] + [c_int] * 4
+                       + [c_void_p, POINTER(c_void_p)] + [c_void_p] * 4),
+    "recmv_mask_iou_backward": (c_int, [c_int, POINTER(c_void_p), POINTER(c_void_p)] + [c_int] * 3
+                                + [c_void_p, c_void_p, POINTER(c_void_p), c_void_p]),
     "recmv_knn_workspace_bytes":(c_int, [c_int, c_int64, c_int64, POINTER(c_size_t)]),
     "recmv_knn_nearest": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int64, c_int64, c_int, c_void_p,
                                   c_void_p, c_void_p, c_void_p]),

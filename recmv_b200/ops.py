@@ -1748,6 +1748,90 @@ class NormalFrameMeanFunction(torch.autograd.Function):
         return (dgtn if need[0] else None), (dJ if need[1] else None), (dnx if need[2] else None), None, None, None
 
 
+def _mask_iou_inputs(fn, a, b, names):
+    """Check two lists of G f32 [N,H,W] CUDA tensors of one shape on one device; returns (G, N, H, W)."""
+    if len(a) == 0 or len(a) != len(b):
+        raise RuntimeError(f"{fn}: expected the same number (>= 1) of {names[0]} and {names[1]}, got {len(a)} and "
+                           f"{len(b)}")
+    dev = a[0].device
+    _expect(fn, names[0], a[0], torch.float32, ("N", "H", "W"))
+    for t, name in [(t, names[0]) for t in a] + [(t, names[1]) for t in b]:
+        _check_input(t, name)
+        _expect(fn, name, t, torch.float32, tuple(a[0].shape), dev)
+    return (len(a),) + tuple(int(s) for s in a[0].shape)
+
+
+def mask_iou(masks, gt_masks, r):
+    """Dilation and soft IoU of `mask_loss` for G garments (recmv_mask_iou, DESIGN section 1m): masks, gt_masks lists of
+    G contiguous f32 [N,H,W] CUDA tensors of one shape, r in 1..32.  Returns (loss [G] f32 = mean_n (1 - I_gn / U_gn), loss_gn [G,N] f32,
+    iu [G,N,2] f64 = (I, U), [G dilated masks f32 [N,H,W]]) with the dilation max_pool2d(gt, 2r+1, 1, r) bit for bit,
+    I = sum m g', U = sum |m + g' - m g'|.  One pixel launch per 8 garments and one combine launch; deterministic;
+    no host synchronisation.  Not differentiable: see MaskIouFunction."""
+    G, N, H, W = _mask_iou_inputs("mask_iou", masks, gt_masks, ("masks", "gt_masks"))
+    dev = masks[0].device
+    with torch.cuda.device(dev):
+        ws = _scratch(dev, "mask_iou_ws", _size("recmv_mask_iou_workspace_bytes", G, N, H, W, int(r)))
+    mgt = [torch.empty_like(g) for g in gt_masks]
+    iu = torch.empty((G, N, 2), dtype=torch.float64, device=dev)
+    loss_gn = torch.empty((G, N), dtype=torch.float32, device=dev)
+    loss = torch.empty((G,), dtype=torch.float32, device=dev)
+    ptrs = lambda ts: (ctypes.c_void_p * G)(*[t.data_ptr() for t in ts])  # noqa: E731
+    _launch("recmv_mask_iou", masks[0], G, ptrs(masks), ptrs(gt_masks), N, H, W, int(r), _ptr(ws), ptrs(mgt),
+            _ptr(iu), _ptr(loss_gn), _ptr(loss))
+    return loss, loss_gn, iu, mgt
+
+
+def mask_iou_backward(masks, mgt, iu, grad_loss):
+    """dL/dm of mask_iou for the upstream gradient grad_loss [G] f32 (recmv_mask_iou_backward): G f32 [N,H,W] tensors
+    -(w_g / N) (g' U - I s (1 - g')) / U^2, s = sign(m + g' - m g') with sign(0) = 0, from the forward's dilated masks
+    and iu.  One launch per 8 garments; no host synchronisation."""
+    G, N, H, W = _mask_iou_inputs("mask_iou_backward", masks, mgt, ("masks", "mgt"))
+    dev = masks[0].device
+    _expect("mask_iou_backward", "iu", iu, torch.float64, (G, N, 2), dev)
+    grad_loss = grad_loss.contiguous().float().reshape(G)
+    _check_input(grad_loss, "grad_loss")
+    dm = [torch.empty_like(m) for m in masks]
+    ptrs = lambda ts: (ctypes.c_void_p * G)(*[t.data_ptr() for t in ts])  # noqa: E731
+    _launch("recmv_mask_iou_backward", masks[0], G, ptrs(masks), ptrs(mgt), N, H, W, _ptr(iu), _ptr(grad_loss),
+            ptrs(dm))
+    return dm
+
+
+class MaskIouFunction(torch.autograd.Function):
+    """The per-garment mask loss of `mask_loss` (OptimGarmentNetwork.py:621-629, 941-947) for G garments:
+    apply(r, m_0 .. m_{G-1}, gt_0 .. gt_{G-1}) with silhouettes m_g and ground-truth masks gt_g f32 [N,H,W] on one CUDA
+    device -> (loss [G] f32, mgt_0 .. mgt_{G-1}): loss_g = mean_n (1 - I / U) against mgt_g = max_pool2d(gt_g, 2r+1,
+    1, r) (mask_iou).  Differentiable (first order) in the silhouettes; the ground-truth masks must not require grad
+    and the dilated masks carry none.  Saves the dilated masks and (I, U) for the backward.  No host
+    synchronisation."""
+
+    @staticmethod
+    def forward(ctx, r, *tensors):
+        G = len(tensors) // 2
+        if len(tensors) != 2 * G or G == 0:
+            raise RuntimeError("MaskIouFunction: expected G silhouettes followed by G ground-truth masks")
+        masks, gts = tensors[:G], tensors[G:]
+        if any(g.requires_grad for g in gts):
+            raise RuntimeError("MaskIouFunction: the ground-truth masks get no gradient; pass them detached")
+        loss, _, iu, mgt = mask_iou(masks, gts, r)
+        ctx.save_for_backward(iu, *masks, *mgt)
+        ctx.G = G
+        ctx.mark_non_differentiable(*mgt)
+        return (loss, *mgt)
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_loss, *grad_mgt):
+        G = ctx.G
+        saved = ctx.saved_tensors
+        iu, masks, mgt = saved[0], saved[1:1 + G], saved[1 + G:]
+        nothing = (None,) * (1 + 2 * G)
+        if not any(ctx.needs_input_grad[1:1 + G]) or grad_loss is None:
+            return nothing
+        dm = mask_iou_backward(masks, mgt, iu, grad_loss)
+        return (None, *[d if need else None for d, need in zip(dm, ctx.needs_input_grad[1:1 + G])]) + (None,) * G
+
+
 def shade_phong(frags, verts, normals, colors, faces, params):
     """Hard Phong shading of K = 1 mesh fragments (recmv_shade_phong).  frags: an object with pix_to_face [N,H,W,1]
     int64 and bary_coords [N,H,W,1,3] f32 (raster.Fragments), or the tuple of rasterize_meshes; verts, normals [N,V,3]

@@ -268,6 +268,134 @@ def make_surface_render_loss():
     return surface_render_loss
 
 
+class Meshes:
+    """pytorch3d's `Meshes(verts=[...], faces=[...])` for what `mask_loss`'s results feed: `verts_list`, `faces_list`,
+    `verts_padded` (meshes of equal size), and `verts_packed` / `faces_packed` (faces offset by the preceding meshes'
+    vertex counts, as pytorch3d packs them)."""
+
+    def __init__(self, verts, faces):
+        self._v, self._f = list(verts), list(faces)
+
+    def __len__(self):
+        return len(self._v)
+
+    def verts_list(self):
+        return self._v
+
+    def faces_list(self):
+        return self._f
+
+    def verts_padded(self):
+        return torch.stack(self._v)
+
+    def verts_packed(self):
+        return torch.cat(self._v)
+
+    def faces_packed(self):
+        base, out = 0, []
+        for v, f in zip(self._v, self._f):
+            out.append(f + base)
+            base += int(v.shape[0])
+        return torch.cat(out)
+
+
+class _Cloud:
+    """The point clouds `pcRender` reads: padded points [N,P,3] and one scalar feature per point."""
+
+    def __init__(self, points, features):
+        self._p, self._f = points, features
+
+    def points_padded(self):
+        return self._p
+
+    def features_packed(self):
+        return self._f
+
+
+def make_mask_loss():
+    """`OptimGarmentNetwork.mask_loss(self, N, H, W, frame_ids, ratio, gt_garment_masks_list, device)`
+    (OptimGarmentNetwork.py:621-667, 841-981) with the ground-truth dilation and the soft IoU on the GPU; bind it as
+    `OptimGarmentNetwork.mask_loss = make_mask_loss()` (the Large-Pose class inherits it).
+    As the reference: per garment the N-expanded deformer call with its offset type and a `Meshes` of the deformed
+    copies; `find_surface_ps` through `self.maskRender`; one `self.pcRender` call on the concatenated garment cloud
+    with `split_size` and `all_size`; the radius int(round(radius / 2 min(H, W) / 1.2)) of the renderer's NDC radius;
+    per garment the mask loss times `pc_weight.mask_weight` (1 without it) and, with `pc_weight.def_consistent`, the
+    template-consistency term against `self.deformer.defs[1]` (GM robust error when `c` > 0, else the mean distance);
+    `garment_optimizer` zero_grad / backward / step, so the backward also reaches the deformer, the conditions, the
+    poses, the translations and any learnable camera; then mean |f + sdfShrinkRadius| per garment times
+    `pc_weight.weight` (60 without `pc_weight`) plus `self.curve_aware_loss(ratio)`.  Returns
+    (def_garment_meshes, garment_masks_list, mgt_garment_masks_list, pc_sdf_loss, surface_ps_list).
+    Unlike the reference: the dilation and the IoU of all garments are one ops.MaskIouFunction (csrc/mask_iou.cu);
+    the info values are detached 0-d tensors; nothing is read back to the host beyond the renderers' own reads.  A
+    positive `pc_weight.laplacian_weight`, `edge_weight` or `norm_weight` raises NotImplementedError (the reference's
+    branches read an undefined template mesh), as do more than two garments and a radius that rounds to 0 pixels
+    (where the reference's `raise NotImplemented` fails); CPU tensors raise."""
+
+    def mask_loss(self, N, H, W, frame_ids, ratio, gt_garment_masks_list, device):
+        conf = self.conf
+        for key in ('laplacian_weight', 'edge_weight', 'norm_weight'):
+            if (conf.get_float('pc_weight.' + key) if 'pc_weight' in conf else -1.) > 0.:
+                raise NotImplementedError(f"mask_loss: pc_weight.{key} > 0 is not supported")
+        G = self.garment_size
+        if G > 2:
+            raise NotImplementedError('only support less or equal than 2 garment_type')
+        for t in list(gt_garment_masks_list) + list(self.garment_vs):
+            if not t.is_cuda:
+                raise RuntimeError("mask_loss runs on CUDA tensors only (no CPU path)")
+        d_cond_list, poses, trans, rendcond = self.get_grad_parameters(frame_ids, device)
+        def_garment_vs = [self.deformer(self.garment_vs[g][None, :, :].expand(N, -1, 3),
+                                        [d_cond_list[g + 1], [poses, trans]], ratio=ratio, offset_type=name)
+                          for g, name in zip(range(G), self.garment_names)]
+        def_garment_meshes = [Meshes(verts=[vs.view(int(v.shape[0]), 3) for vs in torch.split(dv, 1)],
+                                     faces=[fs for _ in range(N)])
+                              for v, fs, dv in zip(self.garment_vs, self.garment_fs, def_garment_vs)]
+        self.info['pc_loss'] = {}
+        surface_ps_list = self.find_surface_ps(def_garment_meshes)
+        points = torch.cat(def_garment_vs, 1)
+        P = int(points.shape[1])
+        features = torch.ones((N * P, 1), device=points.device)
+        garment_masks_list, _ = self.pcRender(_Cloud(points, features), split_size=int(self.garment_vs[0].shape[0]),
+                                              all_size=P)
+        radius = self.pcRender.rasterizer.raster_settings.radius
+        radius = int(round(radius / 2. * float(min(H, W)) / 1.2))
+        if radius <= 0:
+            raise NotImplementedError("mask_loss: the point radius rounds to 0 pixels")
+        out = _ops.MaskIouFunction.apply(radius, *[m[..., -1] for m in garment_masks_list[:G]],
+                                         *gt_garment_masks_list[:G])
+        mask_losses, mgt_garment_masks_list = out[0], list(out[1:])
+        mask_weight = conf.get_float('pc_weight.mask_weight') if 'pc_weight.mask_weight' in conf else 1.
+        consistent_weight = (conf.get_float('pc_weight.def_consistent.weight') if 'pc_weight.def_consistent' in conf
+                             else -1.)
+        garment_loss = 0.
+        for g, name in enumerate(self.garment_names[:G]):
+            self.info['pc_loss']['{}_mask_loss'.format(name)] = mask_losses[g].detach()
+            loss = mask_losses[g] * mask_weight
+            if consistent_weight > 0.:
+                offset2 = def_garment_vs[g] - self.deformer.defs[1](self.garment_vs[g].view(1, -1, 3).expand(N, -1, 3),
+                                                                    [poses, trans])
+                offset2 = (offset2 * offset2).sum(-1)
+                c = conf.get_float('pc_weight.def_consistent.c')
+                consistent_loss = GMRobustError(offset2, c, True).mean() if c > 0. else torch.sqrt(offset2).mean()
+                self.info['pc_loss']['garment_{}_defconst_loss'.format(name)] = consistent_loss.detach()
+                loss = loss + consistent_loss * consistent_weight
+            garment_loss += loss
+        self.garment_optimizer.zero_grad()
+        garment_loss.backward()
+        self.garment_optimizer.step()
+
+        pc_sdf_loss = 0.
+        weight = conf.get_float('pc_weight.weight') if 'pc_weight' in conf else 60.
+        for g, (garment_vs, name) in enumerate(zip(self.garment_vs, self.garment_names)):
+            mnfld_pred = self.garment_nets[g](garment_vs, ratio).view(-1)
+            sdf_loss = (mnfld_pred + self.sdfShrinkRadius).abs().mean()
+            self.info['pc_{}_loss_sdf'.format(name)] = sdf_loss.detach()
+            pc_sdf_loss += sdf_loss * weight
+        pc_sdf_loss += self.curve_aware_loss(ratio)
+        return def_garment_meshes, garment_masks_list, mgt_garment_masks_list, pc_sdf_loss, surface_ps_list
+
+    return mask_loss
+
+
 def _repeat_rows(t, G):
     return t.repeat(G, *([1] * (t.dim() - 1)))
 
