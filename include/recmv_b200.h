@@ -556,6 +556,39 @@ RECMV_API int recmv_mask_iou(int G, const float* const* m, const float* const* g
 RECMV_API int recmv_mask_iou_backward(int G, const float* const* m, const float* const* mgt, int N, int H, int W,
                              const double* iu, const float* grad_loss, float* const* dm, recmv_stream_t stream);
 
+/* ---- project_2d_loss's feature curves: evaluation and regulariser, projection, visibility and compaction ---------
+ * Curve (DESIGN section 1n): C curves of S points (2 <= S <= 1024, C <= 65535), DEVICE f32 center [C,3], dirs [C,S,3],
+ * init_scale [C,S], nx [C,3], scale [C,S], nx_scale [C,S].  v [C,S,3] = center + dirs init_scale relu(scale) +
+ * nx_scale nx; reg [C,2] = (sum_i 1 - cos(u_i, u_{i+1}), sum_j |mean_s v_sj - center_j|) per curve with u_i the
+ * closed-loop differences (plus one wrap) over (|e_i| + 1e-6) and torch's cosine_similarity (eps 1e-8), all formed in
+ * double and rounded once.  Backward: dv [C,S,3] (NULL = 0) and DEVICE dreg [C,2] -> dscale, dnx_scale [C,S] with
+ * torch's derivative rules at the kinks (relu'(0) = 0, d|e|/de = 0 at e = 0, sign(0) = 0, the cosine eps clamp not
+ * differentiated).  One CTA per curve, no atomics.
+ * Projection: X [R,3] DEVICE f32 rows; cams DEVICE f32 [N,16] {fx, fy, px, py, R row-major, T} in pixels; image W x H.
+ * HOST curves int32 [K,3] = {base, stride, column} and HOST thresholds f32 [K] (K <= 64): curve k owns in frame n the
+ * rows base + n stride + s, s < S, reads fl_masks[n, column] (DEVICE f32 [N,M]) and compares body (DEVICE f32 [R]) with
+ * its threshold; the K N ranges of S rows must cover the R rows exactly once (R != K N S, a range past R or two
+ * overlapping ranges is RECMV_E_SHAPE).
+ * Writes screen f32 [R,3] = transform_points_screen (x, y, ndc z) in double rounded once, visible u8 [R] =
+ * fl_masks != 0 && body < threshold, clouds f32 [K N, S, 2] = each (k, n) cloud's visible (x, y) in row order then
+ * zeros, counts int64 [K N], slot int32 [R] = the clouds row a visible row went to, else -1.  workspace:
+ * recmv_curve_project_workspace_bytes(K, N, S).  Backward: dX f32 [R,3] = J^T dclouds[slot] (0 without a slot), J
+ * the 2 x 3 Jacobian of the screen (x, y); the cameras get no gradient.  No atomics; no host synchronisation.      */
+RECMV_API int recmv_curve_fit(int C, int S, const float* center, const float* dirs, const float* init_scale,
+                              const float* nx, const float* scale, const float* nx_scale, float* v, float* reg,
+                              recmv_stream_t stream);
+RECMV_API int recmv_curve_fit_backward(int C, int S, const float* center, const float* dirs, const float* init_scale,
+                                       const float* nx, const float* scale, const float* nx_scale, const float* dv,
+                                       const float* dreg, float* dscale, float* dnx_scale, recmv_stream_t stream);
+RECMV_API int recmv_curve_project_workspace_bytes(int K, int N, int S, size_t* bytes);
+RECMV_API int recmv_curve_project(const float* X, int64_t R, const float* cams, int N, int W, int H,
+                                  const int32_t* curves, const float* thresholds, int K, int S, const float* fl_masks,
+                                  int M, const float* body, void* workspace, float* screen, uint8_t* visible,
+                                  int32_t* slot, float* clouds, int64_t* counts, recmv_stream_t stream);
+RECMV_API int recmv_curve_project_backward(const float* X, int64_t R, const float* cams, int N, int K, int S,
+                                           const int32_t* slot, const float* dclouds, float* dX,
+                                           recmv_stream_t stream);
+
 /* ---- nearest neighbour (K = 1 knn_points): the feature-curve chamfer loss and template registration --------------
  * replaces pytorch3d's KNN extension behind `knn_points` / `chamfer_distance` (DESIGN section 1e).
  * p1 [N,P1,D] queries, p2 [N,P2,D] candidates, f32, D = 2 or 3; lengths1 / lengths2 DEVICE int64[N] or NULL (= P1, P2),

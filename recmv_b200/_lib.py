@@ -160,6 +160,12 @@ SIGNATURES = {
                        + [c_void_p, POINTER(c_void_p)] + [c_void_p] * 4),
     "recmv_mask_iou_backward": (c_int, [c_int, POINTER(c_void_p), POINTER(c_void_p)] + [c_int] * 3
                                 + [c_void_p, c_void_p, POINTER(c_void_p), c_void_p]),
+    "recmv_curve_fit": (c_int, [c_int] * 2 + [c_void_p] * 9),
+    "recmv_curve_fit_backward": (c_int, [c_int] * 2 + [c_void_p] * 11),
+    "recmv_curve_project_workspace_bytes": (c_int, [c_int] * 3 + [POINTER(c_size_t)]),
+    "recmv_curve_project": (c_int, [c_void_p, c_int64, c_void_p] + [c_int] * 3 + [c_void_p] * 2 + [c_int] * 2
+                            + [c_void_p, c_int] + [c_void_p] * 8),
+    "recmv_curve_project_backward": (c_int, [c_void_p, c_int64, c_void_p] + [c_int] * 3 + [c_void_p] * 4),
     "recmv_knn_workspace_bytes":(c_int, [c_int, c_int64, c_int64, POINTER(c_size_t)]),
     "recmv_knn_nearest": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int64, c_int64, c_int, c_void_p,
                                   c_void_p, c_void_p, c_void_p]),

@@ -1832,6 +1832,150 @@ class MaskIouFunction(torch.autograd.Function):
         return (None, *[d if need else None for d, need in zip(dm, ctx.needs_input_grad[1:1 + G])]) + (None,) * G
 
 
+def _curve_inputs(fn, center, dirs, init_scale, nx, scale, nx_scale):
+    """Check the curve tensors (f32, contiguous, one CUDA device): center [C,1,3] or [C,3], dirs [C,S,3], init_scale,
+    scale, nx_scale [C,S,1] or [C,S], nx [C,1,3] or [C,3].  Returns (C, S)."""
+    for t, name in ((center, "center"), (dirs, "dirs"), (init_scale, "init_scale"), (nx, "nx"), (scale, "scale"),
+                    (nx_scale, "nx_scale")):
+        _check_input(t, name)
+    dev = dirs.device
+    _expect(fn, "dirs", dirs, torch.float32, ("C", "S", 3), dev)
+    C, S = int(dirs.shape[0]), int(dirs.shape[1])
+    for t, name in ((center, "center"), (nx, "nx")):
+        _expect(fn, name, t.reshape(-1, 3) if t.numel() == 3 * C else t, torch.float32, (C, 3), dev)
+    for t, name in ((init_scale, "init_scale"), (scale, "scale"), (nx_scale, "nx_scale")):
+        _expect(fn, name, t.reshape(C, S) if t.numel() == C * S else t, torch.float32, (C, S), dev)
+    return C, S
+
+
+def curve_fit(center, dirs, init_scale, nx, scale, nx_scale):
+    """The feature curves and their regulariser (recmv_curve_fit, DESIGN section 1n): Intersect_Free_Curve's buffers
+    and parameters (see _curve_inputs) -> (v [C,S,3] = center + dirs init_scale relu(scale) + nx_scale nx,
+    reg [C,2] = (sum of 1 - cosine of consecutive normalised differences, sum |mean v - center|) per curve).
+    Formed in double, rounded once; one launch; deterministic."""
+    C, S = _curve_inputs("curve_fit", center, dirs, init_scale, nx, scale, nx_scale)
+    v = torch.empty((C, S, 3), dtype=torch.float32, device=dirs.device)
+    reg = torch.empty((C, 2), dtype=torch.float32, device=dirs.device)
+    _launch("recmv_curve_fit", dirs, C, S, *map(_ptr, (center, dirs, init_scale, nx, scale, nx_scale, v, reg)))
+    return v, reg
+
+
+def curve_fit_backward(center, dirs, init_scale, nx, scale, nx_scale, dv, dreg):
+    """(dscale, dnx_scale) [C,S,1] of curve_fit for the upstream dv [C,S,3] (None = 0) and dreg [C,2], with torch's
+    rules at relu(0), zero-length differences and the cosine eps clamp (recmv_curve_fit_backward)."""
+    C, S = _curve_inputs("curve_fit_backward", center, dirs, init_scale, nx, scale, nx_scale)
+    dev = dirs.device
+    if dv is not None:
+        dv = dv.float().contiguous()
+        _expect("curve_fit_backward", "dv", dv, torch.float32, (C, S, 3), dev)
+    dreg = dreg.float().contiguous()
+    _expect("curve_fit_backward", "dreg", dreg, torch.float32, (C, 2), dev)
+    dscale = torch.empty((C, S, 1), dtype=torch.float32, device=dev)
+    dnx = torch.empty((C, S, 1), dtype=torch.float32, device=dev)
+    _launch("recmv_curve_fit_backward", dirs, C, S,
+            *map(_ptr, (center, dirs, init_scale, nx, scale, nx_scale, dv, dreg, dscale, dnx)))
+    return dscale, dnx
+
+
+class CurveFitFunction(torch.autograd.Function):
+    """Intersect_Free_Curve.forward plus its regulariser's terms for all C curves (engineer/utils/
+    garment_structure.py:109-145): apply(center, dirs, init_scale, nx, scale, nx_scale) -> (v [C,S,3], reg [C,2])
+    as curve_fit.  Differentiable (first order) in scale and nx_scale; the buffers get no gradient.  Deterministic
+    backward; no host synchronisation."""
+
+    @staticmethod
+    def forward(ctx, center, dirs, init_scale, nx, scale, nx_scale):
+        ins = [t.detach().contiguous() for t in (center, dirs, init_scale, nx, scale, nx_scale)]
+        v, reg = curve_fit(*ins)
+        ctx.save_for_backward(*ins)
+        return v, reg
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, dv, dreg):
+        if not any(ctx.needs_input_grad[4:6]):
+            return (None,) * 6
+        ins = ctx.saved_tensors
+        if dreg is None:
+            dreg = torch.zeros((ins[1].shape[0], 2), dtype=torch.float32, device=ins[1].device)
+        dscale, dnx = curve_fit_backward(*ins, dv, dreg)
+        return (None,) * 4 + (dscale.view_as(ins[4]) if ctx.needs_input_grad[4] else None,
+                              dnx.view_as(ins[5]) if ctx.needs_input_grad[5] else None)
+
+
+def curve_project(X, cams, W, H, curves, thresholds, S, fl_masks, body):
+    """Projection, visibility and compaction of the feature-curve rows (recmv_curve_project, DESIGN section 1n).
+    X [R,3] f32 rows; cams [N,16] f32 {fx, fy, px, py, R, T} (raster.camera_rows); image W x H; curves a host list
+    of K (base, stride, column) and thresholds K floats: curve k owns in frame n the S rows base + n stride + s, reads
+    fl_masks [N,M] column `column` and tests body [R] < threshold.  Returns (screen [R,3] (x, y, ndc z), visible [R]
+    bool, slot [R] int32, clouds [K N, S, 2], counts [K N] int64).  One launch; no host synchronisation."""
+    for t, name in ((X, "X"), (cams, "cams"), (fl_masks, "fl_masks"), (body, "body")):
+        _check_input(t, name)
+    dev = X.device
+    _expect("curve_project", "X", X, torch.float32, ("R", 3), dev)
+    R = int(X.shape[0])
+    _expect("curve_project", "cams", cams, torch.float32, ("N", 16), dev)
+    N = int(cams.shape[0])
+    _expect("curve_project", "fl_masks", fl_masks, torch.float32, (N, "M"), dev)
+    _expect("curve_project", "body", body, torch.float32, (R,), dev)
+    K = len(curves)
+    if K == 0 or len(thresholds) != K:
+        raise RuntimeError(f"curve_project: expected K >= 1 curves and K thresholds, got {K} and {len(thresholds)}")
+    table = (ctypes.c_int32 * (3 * K))(*[int(x) for c in curves for x in c])
+    thr = (c_float * K)(*[float(t) for t in thresholds])
+    with torch.cuda.device(dev):
+        ws = _scratch(dev, "curve_project_ws", _size("recmv_curve_project_workspace_bytes", K, N, int(S)))
+    screen = torch.empty((R, 3), dtype=torch.float32, device=dev)
+    visible = torch.empty((R,), dtype=torch.bool, device=dev)
+    slot = torch.empty((R,), dtype=torch.int32, device=dev)
+    clouds = torch.empty((K * N, int(S), 2), dtype=torch.float32, device=dev)
+    counts = torch.empty((K * N,), dtype=torch.int64, device=dev)
+    _launch("recmv_curve_project", X, _ptr(X), R, _ptr(cams), N, int(W), int(H), table, thr, K, int(S),
+            _ptr(fl_masks), int(fl_masks.shape[1]), _ptr(body), _ptr(ws), _ptr(screen), _ptr(visible), _ptr(slot),
+            _ptr(clouds), _ptr(counts))
+    return screen, visible, slot, clouds, counts
+
+
+def curve_project_backward(X, cams, K, S, slot, dclouds):
+    """dX [R,3] of curve_project's clouds for dclouds [K N, S, 2]: J^T dclouds[slot] per row, 0 for rows without a
+    slot (recmv_curve_project_backward); a gather, no atomics."""
+    dev = X.device
+    R, N = int(X.shape[0]), int(cams.shape[0])
+    dclouds = dclouds.float().contiguous()
+    _expect("curve_project_backward", "dclouds", dclouds, torch.float32, (K * N, S, 2), dev)
+    _expect("curve_project_backward", "slot", slot, torch.int32, (R,), dev)
+    dX = torch.empty((R, 3), dtype=torch.float32, device=dev)
+    _launch("recmv_curve_project_backward", X, _ptr(X), R, _ptr(cams), N, int(K), int(S), _ptr(slot), _ptr(dclouds),
+            _ptr(dX))
+    return dX
+
+
+class CurveProjectFunction(torch.autograd.Function):
+    """The screen projection, z-buffer visibility and per-(curve, frame) compaction of `project_2d_loss` for every
+    garment's curves: apply(X, cams, W, H, curves, thresholds, S, fl_masks, body) -> (screen, visible, counts,
+    clouds) as curve_project.  Differentiable (first order) in X through the clouds only; the screen points, flags
+    and counts carry no gradient and the cameras are constants.  Deterministic backward; no host synchronisation."""
+
+    @staticmethod
+    def forward(ctx, X, cams, W, H, curves, thresholds, S, fl_masks, body):
+        X, cams = X.detach().contiguous(), cams.detach().contiguous()
+        screen, visible, slot, clouds, counts = curve_project(X, cams, W, H, curves, thresholds, S,
+                                                              fl_masks.detach().float().contiguous(),
+                                                              body.detach().float().contiguous())
+        ctx.save_for_backward(X, cams, slot)
+        ctx.K, ctx.S = len(curves), int(S)
+        ctx.mark_non_differentiable(screen, visible, counts)
+        return screen, visible, counts, clouds
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, d_screen, d_visible, d_counts, dclouds):
+        if not ctx.needs_input_grad[0] or dclouds is None:
+            return (None,) * 9
+        X, cams, slot = ctx.saved_tensors
+        return (curve_project_backward(X, cams, ctx.K, ctx.S, slot, dclouds),) + (None,) * 8
+
+
 def shade_phong(frags, verts, normals, colors, faces, params):
     """Hard Phong shading of K = 1 mesh fragments (recmv_shade_phong).  frags: an object with pix_to_face [N,H,W,1]
     int64 and bary_coords [N,H,W,1,3] f32 (raster.Fragments), or the tuple of rasterize_meshes; verts, normals [N,V,3]

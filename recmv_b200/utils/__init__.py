@@ -47,6 +47,23 @@ def fl_proj_loss(fl_pts_list, gt_fl_pts_list, fl_masks, proj_fl_weights=None):
     return (w * S / V.clamp_min(1) / Q.clamp_min(1)).sum() / C
 
 
+def _fl_proj_loss_compacted(clouds, counts, gt, spans, proj_fl_weights):
+    """fl_proj_loss from clouds already compacted on the device (ops.CurveProjectFunction): clouds [K N, P, 2] with
+    each (curve, frame) cloud's visible points first and counts [K N] int64 (curve-major), annotations gt [K N, M, 2],
+    spans a list of (start, end) curve ranges reduced together and proj_fl_weights K Python numbers.  Returns [G]:
+    per span fl_proj_loss of its curves, mean over the span of w_c sum_n S_{n,c} / (V_c or 1) / (Q_c or 1), as
+    fl_proj_loss divides each garment by its own curve count.  One nearest-neighbour call per direction for all
+    spans; no host synchronisation."""
+    K = len(proj_fl_weights)
+    N = int(clouds.shape[0]) // K
+    S = chamfer_distance(clouds, gt, counts, None, batch_reduction=None, point_reduction="sum")[0].view(K, N).sum(1)
+    cnt = counts.view(K, N)
+    V, Q = (cnt > 0).sum(1), cnt.sum(1)
+    w = torch.tensor([float(v) for v in proj_fl_weights], dtype=S.dtype).pin_memory().to(S.device, non_blocking=True)
+    term = w * S / V.clamp_min(1) / Q.clamp_min(1)
+    return torch.stack([term[a:b].sum() / (b - a) for a, b in spans])
+
+
 def _curve_index(fl_names, target):
     """The reference's `for fl_idx, name in enumerate(fl_names): if name == target: break`: a missing name falls
     through to the last curve."""
@@ -394,6 +411,130 @@ def make_mask_loss():
         return def_garment_meshes, garment_masks_list, mgt_garment_masks_list, pc_sdf_loss, surface_ps_list
 
     return mask_loss
+
+
+def make_project_2d_loss(sdf_scale=10., proj_scale=1.):
+    """`project_2d_loss(self, N, H, W, frame_ids, ratio, cameras, fl_masks, gt_fl_pts, device)` of
+    OptimGarmentNetwork (OptimGarmentNetwork.py:1772-1883, with deform_feature_line :1516-1602 and
+    compute_fl_proj_loss :1604-1712) with the curve evaluation, projection, visibility and compaction on the GPU.
+    Bind `make_project_2d_loss()` on OptimGarmentNetwork and `make_project_2d_loss(0., 0.)` on
+    OptimGarmentNetwork_LargePose, whose override differs only in the loss weights: loss = sdf_scale * SDF term +
+    proj_scale * projection term.
+    As the reference: `fl_visible_method` must be `zbuff`; the curves of garment g are FL_EXTRACT[name] and its
+    visibility is `self.fl_visible_by_body_zbuff` (whichever binding is installed), its body column compared with
+    ZBUF_THRESHOLD per curve (both looked up in the bound class's module); the annotations are gt_fl_pts split over
+    all of `self.fl_names`; per garment the projection loss times `fl_weight.weight` (1), the centre term
+    0 * used * |mean - centre| times `alpha_weight.center_weight` (1) and the diff-a term of ALL curves times
+    `alpha_weight.diff_weight` (1), so the regulariser counts once per garment; the canonical SDF term times
+    `fl_weight.sdf_weight` (60 without `fl_weight`); `fl_optimizer` zero_grad / backward / step; the four info values
+    per garment; `deformer.defs[0].offset[<curve>]` holds the curve's [N,S,3] rows; returns (per garment the split
+    detached screen points (x, y, ndc z), per garment the per-curve visible masks [N,S,3] bool, per garment the
+    per-curve label masks fl_masks[:, None, c:c+1] expanded to [N,S,3], per garment the annotations [N,C_g M,2]).
+    Unlike the reference: the curves are evaluated once with their regulariser (ops.CurveFitFunction,
+    csrc/curve_fit.cu); all garments' curves go through ONE deformer forward on flat rows (frame g N + n reads
+    garment g's condition row n); the projection, visibility and compaction of all garments are ONE
+    ops.CurveProjectFunction (csrc/curve_project.cu) and the chamfer terms ONE nearest-neighbour call per direction;
+    the unused `view_rays` call is dropped; the info values are detached 0-d tensors; nothing is read back to the
+    host.  CPU tensors raise."""
+    binds_cache = {}
+
+    def project_2d_loss(self, N, H, W, frame_ids, ratio, cameras, fl_masks, gt_fl_pts, device):
+        conf = self.conf
+        if conf.get_string('fl_visible_method') != 'zbuff':
+            raise NotImplementedError("project_2d_loss: only fl_visible_method = zbuff is supported")
+        for t in (fl_masks, gt_fl_pts):
+            if not t.is_cuda:
+                raise RuntimeError("project_2d_loss runs on CUDA tensors only (no CPU path)")
+        module = sys.modules[type(self).__module__]
+        self.info['fl_loss'] = {}
+        proj_img_size = torch.stack([torch.full((N,), float(W), device=device),
+                                     torch.full((N,), float(H), device=device)], 1)
+        d_cond_list, poses, trans, _ = self.get_grad_parameters(frame_ids, device)
+        curve = self.inter_free_curve
+        v, reg = _ops.CurveFitFunction.apply(curve.cano_verts_center, curve.cano_v_dirs, curve.init_scale,
+                                             curve.cano_nx, curve.scale, curve.nx_scale)
+        S = int(v.shape[1])
+        index = {name: i for i, name in enumerate(self.fl_names)}     # the reference's dicts: a repeat wins last
+        gt_curves = torch.split(gt_fl_pts, gt_fl_pts.shape[1] // len(self.fl_names), dim=1)
+        names = list(self.garment_names)
+        G = len(names)
+        groups = [list(module.FL_EXTRACT[name]) for name in names]
+        sizes = tuple(len(fl) for fl in groups)
+        # rows (garment, frame, curve, point): garment g's block starts at bases[g] and holds N C_g S rows
+        bases = [0]
+        for Cg in sizes:
+            bases.append(bases[-1] + N * Cg * S)
+        canos = [torch.cat([v[index[n]] for n in fl], 0) for fl in groups]
+        X = torch.cat([c[None].expand(N, -1, -1).reshape(-1, 3) for c in canos])
+        key = (device, N, S, sizes)
+        if key not in binds_cache:
+            binds_cache[key] = torch.cat([torch.arange(g * N, (g + 1) * N).repeat_interleave(Cg * S)
+                                          for g, Cg in enumerate(sizes)]).to(device)
+        binds = binds_cache[key]
+        defconds = [torch.cat([d_cond_list[1 + g] for g in range(G)]), [_repeat_rows(poses, G), _repeat_rows(trans, G)]]
+        D = self.deformer(X, defconds, binds, ratio=ratio, offset_type=groups[0][0])
+        tr = self.deformer.defs[0]
+        off = getattr(tr, 'offset', {}).get(groups[0][0])
+        body, table, thresholds, spans, weights = [], [], [], [], []
+        for g, (name, fl) in enumerate(zip(names, groups)):
+            Cg = len(fl)
+            Dg = D[bases[g]:bases[g + 1]].view(N, Cg * S, 3)
+            if off is not None and off.shape[0] == bases[-1]:
+                og = off[bases[g]:bases[g + 1]].view(N, Cg, S, 3)
+                for c, n in enumerate(fl):
+                    tr.offset[n] = og[:, c]
+            def_fl_vs = [Dg[:, c * S:(c + 1) * S] for c in range(Cg)]
+            fl_vs_dict = {n: v[i:i + 1] for n, i in index.items()}
+            check = self.fl_visible_by_body_zbuff(cameras, d_cond_list, [poses, trans], ratio, fl_vs_dict, def_fl_vs,
+                                                  curve.query_canosmpl_verts(fl), fl, g, name, proj_img_size, N)
+            body.append(check[..., 1].reshape(-1))
+            spans.append((len(table), len(table) + Cg))
+            for c, n in enumerate(fl):
+                table.append((bases[g] + c * S, Cg * S, index[n]))
+                thresholds.append(module.ZBUF_THRESHOLD[n])
+                weights.append(self.dataset.fl_weights[n])
+        cams = _raster.camera_rows(cameras, N, device).detach()
+        screen, visible, counts, clouds = _ops.CurveProjectFunction.apply(
+            D.float().contiguous(), cams, W, H, table, thresholds, S, fl_masks.float().contiguous(),
+            torch.cat(body).float().contiguous())
+        gt = torch.stack([gt_curves[index[n]] for fl in groups for n in fl]).reshape(len(table) * N, -1, 2)
+        proj = _fl_proj_loss_compacted(clouds, counts, gt.float().contiguous(), spans, weights)
+
+        fl_weight = conf.get_float('fl_weight.weight') if 'fl_weight.weight' in conf else 1.
+        center_weight = conf.get_float('alpha_weight.center_weight') if 'alpha_weight' in conf else 1.
+        diff_weight = conf.get_float('alpha_weight.diff_weight') if 'alpha_weight' in conf else 1.
+        sdf_weight = conf.get_float('fl_weight.sdf_weight') if 'fl_weight' in conf else 60.
+        diff_all, centre_all = reg[:, 0].sum(), reg[:, 1].sum()
+        project_loss, fl_garment_sdf_loss = 0., 0.
+        for g, (name, fl) in enumerate(zip(names, groups)):
+            fl_loss = proj[g] * fl_weight
+            used = (torch.stack([fl_masks[:, index[n]] for n in fl], -1).sum() > 0).float()
+            center_loss = 0 * (used * centre_all) * center_weight
+            diff_a_loss = diff_all * diff_weight
+            self.info['fl_loss']['{}_project loss'.format(name)] = fl_loss.detach()
+            self.info['fl_loss']['{}_center loss'.format(name)] = center_loss.detach()
+            self.info['fl_loss']['{}_diff a loss'.format(name)] = diff_a_loss.detach()
+            project_loss += fl_loss + center_loss + diff_a_loss
+            cano_fl_sdf = self.garment_nets[g](canos[g], ratio).view(-1)
+            cano_fl_sdf_loss = (cano_fl_sdf + self.sdfShrinkRadius).abs().mean()
+            self.info['fl_loss']['pc_{}_loss_sdf'.format(name)] = cano_fl_sdf_loss.detach()
+            fl_garment_sdf_loss += cano_fl_sdf_loss * sdf_weight
+        self.fl_optimizer.zero_grad()
+        loss = sdf_scale * fl_garment_sdf_loss + proj_scale * project_loss
+        loss.backward()
+        self.fl_optimizer.step()
+
+        garment_fl_vs_list, visible_mask_list, label_mask_list, gt_fl_pts_list = [], [], [], []
+        for g, fl in enumerate(groups):
+            Cg = len(fl)
+            garment_fl_vs_list.append(torch.split(screen[bases[g]:bases[g + 1]].view(N, Cg * S, 3), S, dim=1))
+            vis = visible[bases[g]:bases[g + 1]].view(N, Cg, S, 1)
+            visible_mask_list.append([vis[:, c].expand(N, S, 3) for c in range(Cg)])
+            label_mask_list.append([fl_masks[:, None, index[n]:index[n] + 1].expand(N, S, 3) for n in fl])
+            gt_fl_pts_list.append(torch.cat([gt_curves[index[n]] for n in fl], dim=1))
+        return garment_fl_vs_list, visible_mask_list, label_mask_list, gt_fl_pts_list
+
+    return project_2d_loss
 
 
 def _repeat_rows(t, G):
