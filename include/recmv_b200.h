@@ -445,6 +445,18 @@ RECMV_API int recmv_shade_phong(const int64_t* pix_to_face, const float* bary, i
                           const float* normals, const float* colors, int V, const int64_t* faces, int64_t F,
                           const float* params /*device[N][28]*/, float* out_rgba, recmv_stream_t stream);
 
+/* ---- vertex-face incidence: the TmpFid / TmpVid lists of `marching_cube_update` (DESIGN section 1o) ----------------
+ * replaces openmesh's `TriMesh(...).vertex_face_indices()` and the host round trip (OptimGarmentNetwork.py:715-735).
+ * faces [F,3] int64 -> fid [3F], vid [3F] int64: one (face, vertex) pair per face corner, grouped by vertex in
+ * ascending order, within a vertex in ascending face index (openmesh lists a vertex's faces in circulator order
+ * instead; the pairs and the grouping are the same).  Every face is kept, so a face that names a vertex twice gives
+ * it two pairs.  A face with an index outside [0, V) gives (-1, -1) for its three corners, at the end of the lists,
+ * and sets flags[0] (device int32, cleared by the call) to 1.  Deterministic; no host synchronisation.
+ * workspace: recmv_vertex_faces_workspace_bytes(F, V).                                                              */
+RECMV_API int recmv_vertex_faces_workspace_bytes(int64_t F, int V, size_t* bytes);
+RECMV_API int recmv_vertex_faces(const int64_t* faces, int64_t F, int V, void* workspace, int64_t* fid, int64_t* vid,
+                          int32_t* flags /*device*/, recmv_stream_t stream);
+
 /* ---- area-weighted surface sampling: the fans of `curve_aware_loss` (DESIGN section 1h) ---------------------------
  * replaces trimesh's `sample_surface` (OptimGarmentNetwork.py:808-809,832-833) with a pinned stream.  verts [M,V,3]
  * f32, faces [F,3] int64 shared by the M meshes -> out [M,S,3] f32.  Sample s of mesh m depends only on (seed, offset,

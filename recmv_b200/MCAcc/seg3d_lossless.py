@@ -66,11 +66,15 @@ class Seg3dLossless(nn.Module):
     # ---- query --------------------------------------------------------------------------------------
     def batch_eval(self, coords, **kwargs):
         """coords [1,M,3] integer lattice coordinates of the FINAL resolution -> [1,1,M]."""
+        return self._eval(self.query_func, coords, **kwargs)
+
+    def _eval(self, query_func, coords, **kwargs):
+        """batch_eval with a given query function."""
         res = self.resolutions[-1].to(coords.device)
         step = 1.0 / res.float()
         c = coords.detach().float() / res + step / 2
         c = c * (self.b_max - self.b_min) + self.b_min
-        occ = self.query_func(**kwargs, points=c)
+        occ = query_func(**kwargs, points=c)
         if type(occ) is list:
             occ = torch.stack(occ)
         assert occ.dim() == 3, "query_func should return a occupancy with shape of [bz, C, N]"
@@ -134,41 +138,14 @@ class Seg3dLossless(nn.Module):
     def _forward_device(self, net, ratio, mode):
         """Same sweep, same voxels re-queried, same arithmetic for the query points -- as a device worklist: per level
         ONE host read (statistics / overflow / "were there conflicts left"), no nonzero / unique / index scatter.
-        The grid equals the torch-op path's bit for bit (tests/test_gpu_surface.py)."""
-        from .. import ops
-        dev = self.b_min.device
-        resolutions, b_min, b_max, coords0 = self._host_consts()
-        Wf, Hf, Df = resolutions[-1]
-        packed, pe_w = net.packed_weights(), net._pe_weights(ratio)
-        calculated = torch.zeros((Df, Hf, Wf), dtype=torch.uint8, device=dev)
-        self.stats = []
-        occ, done = None, None
-        for li, (W, H, D) in enumerate(resolutions):
-            stride = [(Wf - 1) // max(W - 1, 1), (Hf - 1) // max(H - 1, 1), (Df - 1) // max(D - 1, 1)]
-            if li == 0:
-                with torch.no_grad():
-                    occ = self.batch_eval(coords0.unsqueeze(0)).view(1, 1, D, H, W).float().contiguous()
-                done = torch.ones((D, H, W), dtype=torch.uint8, device=dev)
-                calculated[::stride[2], ::stride[1], ::stride[0]] = 1
-                self.stats.append((W, H, D, D * H * W))
-                continue
-            total = D * H * W
-            Dc, Hc, Wc = occ.shape[2:]
-            lvl = ops.C2fLevel((Dc, Hc, Wc), (Wf, Hf, Df), b_min, b_max, dev, total if total <= (1 << 22) else total // 4)
-            occ, done = lvl.refine(occ, done, self.balance_value, 0 if self.use_cuda_impl else 1)
-            lvl.evaluate(packed, pe_w, mode, occ, done, calculated, self.balance_value)
-            while True:
-                for _ in range(2):      # conflict rounds, queued speculatively (an empty list costs three near-empty launches)
-                    lvl.next_from_conflicts(calculated)
-                    lvl.evaluate(packed, pe_w, mode, occ, done, calculated, self.balance_value)
-                queried, conflicts, overflow = lvl.read()                    # the level's one host synchronisation
-                if overflow:
-                    return None                                              # worklist overflow: caller falls back
-                if conflicts == 0:
-                    break
-            self.stats.append((W, H, D, queried))
+        The grid equals the torch-op path's bit for bit (tests/test_gpu_surface.py).  None on a worklist overflow."""
+        sweep = _DeviceSweep(self, self.query_func, net, ratio, mode)
+        self.stats = sweep.stats
+        _run_sweeps([sweep])
+        if sweep.failed:
+            return None                                                      # worklist overflow: caller falls back
         self.last_sweep_path = "device-worklist"
-        return occ
+        return sweep.occ
 
     def forward(self, **kwargs):
         devnet = self._device_net() if not kwargs else None
@@ -177,6 +154,31 @@ class Seg3dLossless(nn.Module):
             if out is not None:
                 return out
         return self._forward_torch(**kwargs)
+
+    def forward_many(self, query_funcs):
+        """forward() for several query functions on this pyramid: one grid per function, each bit-identical to forward()
+        with that function.  The device-worklist sweeps of all of them advance level by level together, so a level
+        costs one host read for every network, not one per network (plus one per extra trip round the conflict loop
+        that any of them needs).  A function that cannot use the worklist (no `recmv_sdf` tag, SIMT mode, not fusable,
+        grad enabled) or whose worklist overflows takes forward()'s one-network fallback, _forward_torch.  Afterwards
+        `query_func`, `stats` and `last_sweep_path` are the last function's, as after forward() on each in turn."""
+        sweeps = [None] * len(query_funcs)
+        if not torch.is_grad_enabled():
+            for i, q in enumerate(query_funcs):
+                self.query_func = q
+                devnet = self._device_net()
+                if devnet is not None:
+                    sweeps[i] = _DeviceSweep(self, q, *devnet)
+        _run_sweeps([s for s in sweeps if s is not None])
+        out = []
+        for q, s in zip(query_funcs, sweeps):
+            self.query_func = q
+            if s is not None and not s.failed:
+                self.stats, self.last_sweep_path = s.stats, "device-worklist"
+                out.append(s.occ)
+            else:
+                out.append(self._forward_torch())
+        return out
 
     def _forward_torch(self, **kwargs):
         dev = self.b_min.device
@@ -247,3 +249,79 @@ class Seg3dLossless(nn.Module):
                 idx, interp, vals = self._query_mask(cmask, stride, occ[0, 0], True, **kwargs)
             self.stats.append((W, H, D, queried))
         return occ
+
+
+class _DeviceSweep:
+    """One network's device-worklist sweep, advanced one pyramid level at a time by _run_sweeps.  The constructor
+    evaluates the coarse level; per finer level, begin() queues the refine pass and the first evaluation, rounds() queues
+    two conflict rounds, and after_read() takes the level's counters once the driver has read them."""
+    MORE, DONE, OVERFLOW = range(3)
+
+    def __init__(self, engine, query_func, net, ratio, mode):
+        self.dev = engine.b_min.device
+        self.res, self.b_min, self.b_max, coords0 = engine._host_consts()
+        self.balance, self.order = engine.balance_value, 0 if engine.use_cuda_impl else 1
+        self.packed, self.pe_w, self.mode = net.packed_weights(), net._pe_weights(ratio), mode
+        Wf, Hf, Df = self.res[-1]
+        W, H, D = self.res[0]
+        self.calculated = torch.zeros((Df, Hf, Wf), dtype=torch.uint8, device=self.dev)
+        with torch.no_grad():
+            self.occ = engine._eval(query_func, coords0.unsqueeze(0)).view(1, 1, D, H, W).float().contiguous()
+        self.done = torch.ones((D, H, W), dtype=torch.uint8, device=self.dev)
+        sx, sy, sz = self._stride(0)
+        self.calculated[::sz, ::sy, ::sx] = 1
+        self.stats = [(W, H, D, D * H * W)]
+        self.lvl, self.li, self.failed = None, 0, False
+
+    def _stride(self, li):
+        (Wf, Hf, Df), (W, H, D) = self.res[-1], self.res[li]
+        return (Wf - 1) // max(W - 1, 1), (Hf - 1) // max(H - 1, 1), (Df - 1) // max(D - 1, 1)
+
+    def begin(self, li):
+        from .. import ops
+        W, H, D = self.res[li]
+        total = D * H * W
+        Dc, Hc, Wc = self.occ.shape[2:]
+        self.li = li
+        self.lvl = ops.C2fLevel((Dc, Hc, Wc), self.res[-1], self.b_min, self.b_max, self.dev,
+                                total if total <= (1 << 22) else total // 4)
+        self.occ, self.done = self.lvl.refine(self.occ, self.done, self.balance, self.order)
+        self._evaluate()
+
+    def _evaluate(self):
+        self.lvl.evaluate(self.packed, self.pe_w, self.mode, self.occ, self.done, self.calculated, self.balance)
+
+    def rounds(self):
+        for _ in range(2):      # conflict rounds, queued speculatively (an empty list costs three near-empty launches)
+            self.lvl.next_from_conflicts(self.calculated)
+            self._evaluate()
+
+    def after_read(self, counts):
+        queried, conflicts, overflow = counts
+        if overflow:
+            self.failed = True
+            return self.OVERFLOW
+        if conflicts:
+            return self.MORE
+        self.stats.append(tuple(self.res[self.li]) + (queried,))
+        self.lvl = None
+        return self.DONE
+
+
+def _run_sweeps(sweeps):
+    """Advance every sweep (all on one pyramid) through the finer levels together: per level, each sweep's refine pass
+    and two conflict rounds are queued, then ONE host read (ops.read_c2f_levels) serves every sweep still on that level;
+    the ones with conflicts left get two more rounds and another shared read.  A sweep whose worklist overflows stops
+    with `failed` set."""
+    from .. import ops
+    live = list(sweeps)
+    for li in range(1, len(live[0].res) if live else 0):
+        for s in live:
+            s.begin(li)
+        pending = live
+        while pending:
+            for s in pending:
+                s.rounds()
+            counts = ops.read_c2f_levels([s.lvl for s in pending])   # the level's one host synchronisation
+            pending = [s for s, c in zip(pending, counts) if s.after_read(c) == s.MORE]
+        live = [s for s in live if not s.failed]

@@ -136,6 +136,8 @@ SIGNATURES = {
     "recmv_vertex_normals": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int64, c_void_p, c_void_p, c_void_p]),
     "recmv_shade_phong": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_void_p,
                                   c_int64, c_void_p, c_void_p, c_void_p]),
+    "recmv_vertex_faces_workspace_bytes": (c_int, [c_int64, c_int, POINTER(c_size_t)]),
+    "recmv_vertex_faces": (c_int, [c_void_p, c_int64, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "recmv_surface_sample_workspace_bytes": (c_int, [c_int, c_int64, POINTER(c_size_t)]),
     "recmv_surface_sample": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int64, c_int64, c_uint64, c_uint64, c_void_p,
                                      c_void_p, c_void_p]),

@@ -2,7 +2,8 @@
 // sort groups each slot's items in increasing item order, and segment_bounds_kernel finds every slot's [begin, end)
 // range in the sorted list.  One thread per slot then sums its range in order, so the result is bit-identical from
 // run to run and independent of the SM count.  Used by the vertex normals (shade.cu) and the KNN backward (knn.cu).
-// The mesh adjacency (nricp.cu) uses the 64-bit key sort alone.
+// The vertex-face incidence (vertex_faces.cu) uses the corner keys and the pair sort without the sums; the mesh
+// adjacency (nricp.cu) uses the 64-bit key sort alone.
 #pragma once
 #include <cub/device/device_radix_sort.cuh>
 
@@ -86,6 +87,22 @@ inline SegmentWs segment_layout(Carve& c, long long M, long long S) {
   w.ranges_bytes = c.used - ranges;
   w.temp = c.take<char>(0, 1);
   return w;
+}
+
+// One thread per (face, corner) e = 3 f + k of faces [F,3], M = 3 F: key = the corner's vertex, or V for every corner
+// of a face with an index outside [0, V) (so such faces sort last), value e.  bad (or nullptr) is set to 1 when any
+// face has such an index.
+__global__ void __launch_bounds__(kSegThreads) corner_keys_kernel(const long long* __restrict__ faces, long long M,
+                                                                   int V, unsigned* __restrict__ keys,
+                                                                   unsigned* __restrict__ vals, int* __restrict__ bad) {
+  const long long e = blockIdx.x * (long long)kSegThreads + threadIdx.x;
+  if (e >= M) return;
+  const long long f = e / 3;
+  const long long a = faces[3 * f], b = faces[3 * f + 1], c = faces[3 * f + 2];
+  const bool ok = a >= 0 && a < V && b >= 0 && b < V && c >= 0 && c < V;
+  keys[e] = ok ? (unsigned)faces[e] : (unsigned)V;
+  vals[e] = (unsigned)e;
+  if (!ok && bad) *bad = 1;
 }
 
 // The [beg, end) range of every slot k < S in the sorted keys; keys >= S (invalid items) are skipped.  beg and end

@@ -7,7 +7,8 @@
 //   n / max(|n|, 1e-6).  The sum runs in increasing (face, corner) order -- no float atomics, so the result is
 //   bit-identical from run to run and independent of the SM count.  A face with an index outside [0, V) contributes
 //   nothing; a vertex no face references gets 0.
-//   1. normals_keys_kernel   one thread per (face, corner) e = 3 f + k: key = its vertex (V for an invalid face), value e;
+//   1. corner_keys_kernel    one thread per (face, corner) e = 3 f + k: key = its vertex (V for an invalid face), value e
+//                            (segments.cuh);
 //   2. CUB radix sort        stable, so each vertex's values stay in increasing e order;
 //   3. segment_bounds_kernel the [begin, end) range of every vertex in the sorted list (segments.cuh);
 //   4. normals_sum_kernel    one thread per (frame, vertex): sum its range in order and normalise.
@@ -26,18 +27,6 @@ namespace {
 constexpr int kNormThreads = 256;
 constexpr int kShadeThreads = 256;
 constexpr int kShadeParams = 28;   // per-frame constants, layout in include/recmv_b200.h
-
-__global__ void __launch_bounds__(kNormThreads) normals_keys_kernel(const long long* __restrict__ faces, long long M,
-                                                                     int V, unsigned* __restrict__ keys,
-                                                                     unsigned* __restrict__ vals) {
-  const long long e = blockIdx.x * (long long)kNormThreads + threadIdx.x;
-  if (e >= M) return;
-  const long long f = e / 3;
-  const long long a = faces[3 * f], b = faces[3 * f + 1], c = faces[3 * f + 2];
-  const bool ok = a >= 0 && a < V && b >= 0 && b < V && c >= 0 && c < V;
-  keys[e] = ok ? (unsigned)faces[e] : (unsigned)V;
-  vals[e] = (unsigned)e;
-}
 
 // |(x, y, z)|^2 in the order the sm_90a compiler contracts the plain x * x + y * y + z * z to, written out so that the
 // float32 restatement in tests/shade_f32.py is exact: y * y rounded, then x and z fused.
@@ -184,8 +173,8 @@ extern "C" int recmv_vertex_normals(const float* verts, int N, int V, const int6
   cudaError_t e = cudaMemsetAsync(w.beg, 0, w.ranges_bytes, st);   // beg and end: empty ranges
   if (e != cudaSuccess) return (int)e;
   if (M > 0) {
-    const int nb = (int)((M + kNormThreads - 1) / kNormThreads);
-    normals_keys_kernel<<<nb, kNormThreads, 0, st>>>((const long long*)faces, M, V, w.keys_in, w.vals_in);
+    const int nb = (int)((M + kSegThreads - 1) / kSegThreads);
+    corner_keys_kernel<<<nb, kSegThreads, 0, st>>>((const long long*)faces, M, V, w.keys_in, w.vals_in, nullptr);
     s = launch_status();
     if (s) return s;
     s = sort_pairs(w.temp, w.keys_in, w.keys_out, w.vals_in, w.vals_out, M, (unsigned)V, st);

@@ -351,34 +351,87 @@ def mc_gpu(sdfs, xstep=1.0, ystep=1.0, zstep=1.0, xmin=0.0, ymin=0.0, zmin=0.0, 
 
     One C call queues every pass (sign mask, count, scan, vertices, faces) into grow-only capacity buffers; the single
     host synchronisation is the read of (V, F) AFTER everything is queued (the reference blocks between its kernels,
-    CudaKernels.cu:628).  The results are fresh tensors, as the reference returns (MCGpu.cpp:49-54)."""
+    CudaKernels.cu:628).  The results are fresh tensors, as the reference returns (MCGpu.cpp:49-54).  The one-grid case
+    of mc_gpu_many."""
     _check_input(sdfs, "sdfs")
     if sdfs.dtype != torch.float32:
         return []
     if sdfs.dim() != 3 or min(sdfs.shape) <= 0:
         return []
-    NX, NY, NZ = sdfs.shape
-    dev = sdfs.device
-    nbytes = _size("recmv_mc_scratch_bytes", NX, NY, NZ)
-    cap_v, cap_f = 4096, 8192     # at least; the output buffers kept from earlier calls may be larger
-    step = (c_float * 3)(xstep, ystep, zstep)
-    org = (c_float * 3)(xmin, ymin, zmin)
+    return mc_gpu_many([sdfs], [(xstep, ystep, zstep)], [(xmin, ymin, zmin)], fTargetValue)[0]
+
+
+def mc_gpu_many(grids, steps, origins, iso=0.0, capacity=(4096, 8192)):
+    """mc_gpu on every grid with one host synchronisation: grids, float32 CUDA [NX,NY,NZ] on one device; steps and
+    origins, one (x, y, z) per grid; one iso value.  Returns [[verts, faces], ...], each bit-identical to mc_gpu on that
+    grid.  Every grid's run is queued before the one read of all (V, F, overflow) counters; only the grids whose output
+    buffers overflowed are re-run, once, after growing them to their counts.  capacity: the (vertex, face) rows a grid's
+    output buffers hold at least at the first run (buffers kept from earlier calls may be larger).
+
+    Grid i writes its mesh into its own cached output buffers, so no later grid overwrites it before the read.  The
+    scratch (sign mask, segment sums, packed vertex words) is one buffer of the largest grid's size: each run consumes
+    it before the next one on the stream starts, and the counts leave it with the run."""
+    if not (len(grids) == len(steps) == len(origins)):
+        raise RuntimeError("mc_gpu_many: grids, steps and origins must have the same length")
+    if not grids:
+        return []
+    dev = grids[0].device
+    dims = []
+    for i, g in enumerate(grids):
+        _check_input(g, f"grids[{i}]")
+        if g.device != dev or g.dtype != torch.float32 or g.dim() != 3 or min(g.shape) <= 0:
+            raise RuntimeError(f"mc_gpu_many: grids[{i}] must be a non-empty float32 [NX,NY,NZ] tensor on {dev}, got "
+                               f"{g.dtype} {tuple(g.shape)} on {g.device}")
+        dims.append(tuple(int(n) for n in g.shape))
+    scratch = _scratch(dev, "mc_scratch", max(_size("recmv_mc_scratch_bytes", *d) for d in dims))
+    n = len(grids)
+    ctr, host = _counters(dev, ("mc_counters", n), 4 * n)
+    caps = [tuple(capacity)] * n
+    todo, out = list(range(n)), [None] * n
     for _ in range(2):
-        scratch = _scratch(dev, "mc_scratch", nbytes)
-        verts = _scratch(dev, "mc_verts", cap_v, torch.float32, (3,))
-        faces = _scratch(dev, "mc_faces", cap_f, torch.int64, (3,))
-        ctr, host = _counters(dev, "mc_counters", 4)
-        _launch("recmv_mc_run", sdfs, _ptr(sdfs), NX, NY, NZ, float(fTargetValue), _ptr(scratch), step, org, _ptr(verts),
-                verts.shape[0], _ptr(faces), faces.shape[0], _ptr(ctr))
-        V, F, overflow = (int(v) for v in _read_counters(ctr, host)[:3])
-        if V >= (1 << 25):
-            check(_lib.RECMV_E_RANGE, "recmv_mc_run (more than 2^25 vertices)")
-        if not overflow:
-            break
-        cap_v, cap_f = int(V * 1.25) + 1024, int(F * 1.25) + 2048   # grow once, re-run (buffers are kept)
-    else:
-        raise _lib.RecmvError("recmv_mc_run: output buffers still too small after growing")
-    return [verts[:V].clone(), faces[:F].clone()]
+        bufs = {}
+        for i in todo:
+            verts = _scratch(dev, ("mc_verts", i), caps[i][0], torch.float32, (3,))
+            faces = _scratch(dev, ("mc_faces", i), caps[i][1], torch.int64, (3,))
+            _launch("recmv_mc_run", grids[i], _ptr(grids[i]), *dims[i], float(iso), _ptr(scratch),
+                    (c_float * 3)(*steps[i]), (c_float * 3)(*origins[i]), _ptr(verts), verts.shape[0], _ptr(faces),
+                    faces.shape[0], _ptr(ctr[4 * i:4 * i + 4]))
+            bufs[i] = verts, faces
+        h = _read_counters(ctr, host).view(n, 4).tolist()
+        again = []
+        for i in todo:
+            V, F, overflow = h[i][:3]
+            if V >= (1 << 25):
+                check(_lib.RECMV_E_RANGE, "recmv_mc_run (more than 2^25 vertices)")
+            if overflow:
+                caps[i] = int(V * 1.25) + 1024, int(F * 1.25) + 2048   # grow once, re-run (buffers are kept)
+                again.append(i)
+            else:
+                out[i] = [bufs[i][0][:V].clone(), bufs[i][1][:F].clone()]
+        todo = again
+        if not todo:
+            return out
+    raise _lib.RecmvError("recmv_mc_run: output buffers still too small after growing")
+
+
+def vertex_faces(faces, V, check_indices=False):
+    """The vertex-face incidence of faces [F,3] int64 CUDA over V vertices (recmv_vertex_faces, DESIGN section 1o):
+    (fid [3F], vid [3F] int64), one pair per face corner, grouped by ascending vertex and, within a vertex, ascending
+    face.  The flattened `TmpFid` / `TmpVid` that OptimGarmentNetwork.marching_cube_update builds from openmesh's
+    vertex_face_indices(), in a pinned order.  A face with an index outside [0, V) gives (-1, -1) pairs at the end and
+    sets a device flag; check_indices=True reads that flag (one host synchronisation) and raises ValueError when it is
+    set.  Otherwise nothing is read back."""
+    _check_input(faces, "faces")
+    _expect("vertex_faces", "faces", faces, torch.int64, ("F", 3))
+    dev, F, V = faces.device, int(faces.shape[0]), int(V)
+    fid = torch.empty((3 * F,), dtype=torch.int64, device=dev)
+    vid = torch.empty((3 * F,), dtype=torch.int64, device=dev)
+    flag, host = _counters(dev, "vertex_faces_flag", 1)
+    ws = _scratch(dev, "vertex_faces_ws", _size("recmv_vertex_faces_workspace_bytes", F, V, dev=dev))
+    _launch("recmv_vertex_faces", faces, _ptr(faces), F, V, _ptr(ws), _ptr(fid), _ptr(vid), _ptr(flag))
+    if check_indices and int(_read_counters(flag, host)[0]):
+        raise ValueError(f"vertex_faces: a face has an index outside [0, {V})")
+    return fid, vid
 
 
 # --------------------------------------------------------------------------------------------------
@@ -2249,8 +2302,20 @@ class C2fLevel:
 
     def read(self):
         """(queried so far, conflicts of the last round, overflow) -- the level's host synchronisation."""
-        h = self.ctr.tolist()
+        return self.counts(self.ctr.tolist())
+
+    def counts(self, h):
+        """(queried, conflicts, overflow) from a host copy h of the counters."""
         return h[4], h[2 + self.cur], h[1]
+
+
+def read_c2f_levels(levels):
+    """C2fLevel.read of every level in one host synchronisation: the counters of several levels are gathered into one
+    tensor and copied back together."""
+    if len(levels) == 1:
+        return [levels[0].read()]
+    h = torch.stack([lvl.ctr for lvl in levels]).tolist()
+    return [lvl.counts(r) for lvl, r in zip(levels, h)]
 
 
 def surface_solve(cam_pos, rays, seeds, batch_inds, sdf_packed, sdf_pe_w, tr_packed, tr_pe_w, conds, skin, dthreshold,

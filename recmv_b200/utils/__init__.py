@@ -1,9 +1,12 @@
 """Mirror of the hot-path helpers of the reference's `utils` package (utils/utils.py:8-18,40-46,133-156,
 198-264).  Same names, arguments and return values; the native calls go to librecmv_b200.so."""
+import os
 import sys
 
+import numpy as np
 import torch
 
+from .. import discretize as _discretize
 from .. import ops as _ops
 from .. import raster as _raster
 from ..knn import chamfer_distance
@@ -535,6 +538,70 @@ def make_project_2d_loss(sdf_scale=10., proj_scale=1.):
         return garment_fl_vs_list, visible_mask_list, label_mask_list, gt_fl_pts_list
 
     return project_2d_loss
+
+
+def make_discretize_sdf():
+    """`OptimGarmentNetwork.discretizeSDF(self, ratio, engine=None, balance_value=0.)` (OptimGarmentNetwork.py:581-618)
+    with the sweeps of the body and every garment network advanced together; bind it as
+    `OptimGarmentNetwork.discretizeSDF = make_discretize_sdf()` (the Large-Pose class inherits it).
+    As the reference: `self.engine` and iso 0 for every network whatever `engine` and `balance_value` are passed (the
+    reference's inner function ignores both); any `ratio` the networks take, -1 included; returns
+    ([body, *garments] verts, faces) as fresh tensors, and leaves the engine's `query_func` on the last garment and its
+    `balance_value` at 0.  Unlike the reference: one host read per pyramid level for all networks
+    (discretize.discretize_many) and one for all their marching cubes (ops.mc_gpu_many), instead of one per level and
+    one per marching cubes for each network.  Each mesh is bit-identical to the network's own sweep and mc_gpu."""
+    def discretizeSDF(self, ratio, engine=None, balance_value=0.):
+        return _discretize.mesh_many([self.sdf, *self.garment_nets], self.engine, ratio)
+
+    return discretizeSDF
+
+
+def make_marching_cube_update():
+    """`OptimGarmentNetwork.marching_cube_update(self, frame_ids, ratio, root, device)` (OptimGarmentNetwork.py:678-740)
+    without openmesh; bind it as `OptimGarmentNetwork.marching_cube_update = make_marching_cube_update()` (the
+    Large-Pose class inherits it).
+    As the reference, in its order: `<root>/fl_mesh_show` created; `self.discretizeSDF(ratio, None, -sdfShrinkRadius)`
+    (whatever is bound); `body_vs/fs`, `garment_vs/fs`; `self.update_hierarchical_config(device, max garment vertices,
+    max garment faces)`; 'tmp sdf vanished...' and AssertionError on an empty body mesh; remesh_time = 1 +
+    floor(remesh_time); requires_grad on the body and garment vertices; `TmpOptimizer` = SGD(lr 0.05, momentum 0.9) over
+    [body, *garments], `garment_optimizer` = SGD(lr 0.05, momentum 0.9) over the garments, `fl_optimizer` = AdamW(lr
+    1e-4) over `inter_free_curve`; `TmpFid/TmpVid` and `garment_tmpfid/tmpvid`, the (face, vertex) pairs of every
+    vertex; `self.root`; `visualize_curve_mesh` when a visualizer is set.
+    Unlike the reference: the incidence lists come from ops.vertex_faces (csrc/vertex_faces.cu) on the device, with
+    no host copy of the meshes and no read back, and list each vertex's faces in ascending index where openmesh lists
+    them in circulator order (the same pairs, grouped by the same ascending vertices)."""
+    def marching_cube_update(self, frame_ids, ratio, root, device):
+        save_fl_mesh_path = os.path.join(root, 'fl_mesh_show')
+        os.makedirs(save_fl_mesh_path, exist_ok=True)
+        print('tmp sdf generate')
+        vs_list, fs_list = self.discretizeSDF(ratio, None, -self.sdfShrinkRadius)
+        self.body_vs, self.body_fs = vs_list[0], fs_list[0]
+        self.garment_vs, self.garment_fs = vs_list[1:], fs_list[1:]
+        max_garment_vs = max([garment_vs.shape[0] for garment_vs in self.garment_vs])
+        max_garment_fs = max([garment_fs.shape[0] for garment_fs in self.garment_fs])
+        self.update_hierarchical_config(device, max_garment_vs, max_garment_fs)
+        if self.body_vs.shape[0] == 0:
+            print('tmp sdf vanished...')
+            raise AssertionError
+        self.remesh_time = 1. + np.floor(self.remesh_time)
+        self.body_vs.requires_grad = True
+        for garment_vs in self.garment_vs:
+            garment_vs.requires_grad = True
+        self.TmpOptimizer = torch.optim.SGD([self.body_vs, *self.garment_vs], lr=0.05, momentum=0.9)
+        self.garment_optimizer = torch.optim.SGD(self.garment_vs, lr=0.05, momentum=0.9)
+        self.fl_optimizer = torch.optim.AdamW(self.inter_free_curve.parameters(), lr=1e-4)
+        fid, vid = _ops.vertex_faces(self.body_fs, self.body_vs.shape[0])
+        self.TmpFid, self.TmpVid = fid.to(device), vid.to(device)
+        self.garment_tmpfid, self.garment_tmpvid = [], []
+        for garment_vs, garment_fs in zip(self.garment_vs, self.garment_fs):
+            fid, vid = _ops.vertex_faces(garment_fs, garment_vs.shape[0])
+            self.garment_tmpfid.append(fid.to(device))
+            self.garment_tmpvid.append(vid.to(device))
+        self.root = root
+        if self.visualizer is not None:
+            self.visualize_curve_mesh(save_fl_mesh_path, int(self.opt_times), device)
+
+    return marching_cube_update
 
 
 def _repeat_rows(t, G):
