@@ -4,6 +4,7 @@ autograd graph); all arithmetic happens in librecmv_b200.so.
 """
 import contextlib
 import ctypes
+import functools
 from ctypes import byref, c_float, c_size_t
 
 import torch
@@ -73,20 +74,86 @@ def _read_counters(ctr, host):
     return host
 
 
-def _check_input(t, name):
-    # reference: CHECK_INPUT (FastMinv/M3x3Inv.cpp:4-6, MCGpu/MCGpu.cpp:3-5)
-    if not t.is_cuda:
-        raise RuntimeError(f"{name} must be a CUDA tensor")
-    if not t.is_contiguous():
-        raise RuntimeError(f"{name} must be contiguous")
+def _ptr_array(ts):
+    """Device pointers of a list of tensors (None for a missing one) as a host void*[len(ts)]."""
+    return (ctypes.c_void_p * len(ts))(*[t.data_ptr() if t is not None else None for t in ts])
 
 
-def _dtype_code(t, name):
-    if t.dtype == torch.float32:
-        return F32
-    if t.dtype == torch.float64:
-        return F64
-    raise RuntimeError(f"{name} must be a float/double tensor")
+FLOATS = (torch.float32, torch.float64)    # an operand dtype of the ops that run in either precision
+
+
+def _dtype_code(dtype):
+    return {torch.float32: F32, torch.float64: F64}[dtype]
+
+
+def _operands(fn, *specs):
+    """Refuse (RuntimeError) any operand a kernel of `fn` would misread; return the bound shape symbols.
+
+    A spec is (t, name, dtype, shape).  t: a tensor; None, an absent optional operand, passes; a list of tensors is
+    checked element by element as name[i] with the same symbols.  dtype: a torch dtype, or a tuple of accepted dtypes
+    that binds like a symbol (key "dtype").  shape entries: an int fixes an extent; a str is a symbol, bound at its first
+    use and equal at every later one; None accepts any extent; a callable of the bindings so far gives an extent derived
+    from them (row_ptr's V + 1).  A leading ... stands for any number of leading extents whose product binds like a
+    symbol (key ...): the point count P of a [..., 3] point tensor that a kernel reads as numel / 3 rows.
+    The dtype, extents and contiguity of every operand are checked in argument order, then that all of them sit on one
+    CUDA device, so that nothing is allocated, sized or launched for a call that is refused."""
+    ops = []
+    for t, name, dtype, shape in specs:
+        if isinstance(t, (list, tuple)):
+            ops += [(x, f"{name}[{i}]", dtype, shape) for i, x in enumerate(t)]
+        elif t is not None:
+            ops.append((t, name, dtype, shape))
+    bound, source = {}, {}
+    if not ops:
+        return bound
+    dev = ops[0][0].get_device()     # -1 for a CPU tensor
+
+    def refuse(t, name, dtype, shape, why="", keys=()):
+        label = {Ellipsis: "the product of the leading extents"}
+        why += "".join(f" ({label.get(k, k)} is {bound[k]} from {source[k]})" for k in keys)
+        want = "|".join(map(str, dtype)) if isinstance(dtype, tuple) else dtype
+        dims = ",".join("..." if s is Ellipsis else "*" if s is None else str(s(bound)) if callable(s) else str(s)
+                        for s in shape)
+        where = f"CUDA device cuda:{dev}" if dev >= 0 else "a CUDA device"
+        raise RuntimeError(f"{fn}: {name} must be {want} [{dims}] on {where}, got {t.dtype} {tuple(t.shape)} on "
+                           f"{t.device}{why}")
+
+    for t, name, dtype, shape in ops:
+        if isinstance(dtype, tuple):
+            if t.dtype not in dtype or t.dtype is not bound.setdefault("dtype", t.dtype):
+                refuse(t, name, dtype, shape, keys=["dtype"] if "dtype" in source else [])
+            source.setdefault("dtype", name)
+        elif t.dtype is not dtype:
+            refuse(t, name, dtype, shape)
+        sizes = t.shape
+        if shape and shape[0] is Ellipsis:
+            k = len(sizes) - len(shape) + 1
+            if k < 0:
+                refuse(t, name, dtype, shape)
+            sizes = (sizes[:k].numel(),) + tuple(sizes[k:])
+        elif len(sizes) != len(shape):
+            refuse(t, name, dtype, shape)
+        for s, n in zip(shape, sizes):
+            if s is None:
+                continue
+            if isinstance(s, int):
+                if n != s:
+                    refuse(t, name, dtype, shape)
+            elif callable(s):
+                if n != s(bound):
+                    refuse(t, name, dtype, shape, keys=[b for b in bound if b != "dtype"])
+            elif n != bound.setdefault(s, n):
+                refuse(t, name, dtype, shape, keys=[s])
+            else:
+                source.setdefault(s, name)
+        if not t.is_contiguous():
+            refuse(t, name, dtype, shape, " (not contiguous)")
+    for t, name, dtype, shape in ops:
+        if not t.is_cuda:
+            refuse(t, name, dtype, shape, " (not a CUDA tensor)")
+        if t.get_device() != dev:
+            refuse(t, name, dtype, shape, f" (not on cuda:{dev}, where {ops[0][1]} is)")
+    return bound
 
 
 # --------------------------------------------------------------------------------------------------
@@ -94,25 +161,20 @@ def _dtype_code(t, name):
 # --------------------------------------------------------------------------------------------------
 def minv3x3(ms):
     """FastMinv.Fast3x3Minv(ms) -> [invs, checks]  (FastMinv/M3x3Inv.cpp:12-37)."""
-    _check_input(ms, "ms")
-    code = _dtype_code(ms, "ms")
-    n = ms.size(0)
+    d = _operands("minv3x3", (ms, "ms", FLOATS, ("n", 3, 3)))
+    n = d["n"]
     invs = torch.empty((n, 3, 3), dtype=ms.dtype, device=ms.device)
     ok = torch.empty((n,), dtype=torch.uint8, device=ms.device)
-    _launch("recmv_minv3x3_fwd", ms, _ptr(ms), _ptr(invs), _ptr(ok), n, code)
+    _launch("recmv_minv3x3_fwd", ms, _ptr(ms), _ptr(invs), _ptr(ok), n, _dtype_code(d["dtype"]))
     return [invs, ok.view(torch.bool)]
 
 
 def minv3x3_backward(grads, invs):
     """FastMinv.Fast3x3Minv_backward(grads, invs) -> outs  (FastMinv/M3x3Inv.cpp:39-59)."""
-    _check_input(grads, "grads")
-    _check_input(invs, "invs")
-    if grads.dtype != invs.dtype:
-        raise RuntimeError("invs must have same type with grads")
-    code = _dtype_code(invs, "invs")
-    n = invs.size(0)
+    d = _operands("minv3x3_backward", (grads, "grads", FLOATS, ("n", 3, 3)), (invs, "invs", FLOATS, ("n", 3, 3)))
+    n = d["n"]
     outs = torch.empty((n, 3, 3), dtype=invs.dtype, device=invs.device)
-    _launch("recmv_minv3x3_bwd", invs, _ptr(grads), _ptr(invs), _ptr(outs), n, code)
+    _launch("recmv_minv3x3_bwd", invs, _ptr(grads), _ptr(invs), _ptr(outs), n, _dtype_code(d["dtype"]))
     return outs
 
 
@@ -135,88 +197,51 @@ class FastDiff3x3MinvFunction(torch.autograd.Function):
 # --------------------------------------------------------------------------------------------------
 # GridSamplerMine
 # --------------------------------------------------------------------------------------------------
-def _gs_dims(inp, grid, layout):
-    if inp.dim() != 5 or grid.dim() != 5:
-        raise RuntimeError("grid_sampler(): expected 5D input and grid")
-    if inp.size(0) != grid.size(0) or grid.size(-1) != 3:
-        raise RuntimeError("grid_sampler(): inconsistent input / grid sizes")
-    if inp.dtype != grid.dtype:
-        raise RuntimeError("grid_sampler(): expected input and grid to have same dtype")
-    if layout == LAYOUT_NCDHW:
-        N, C, D, H, W = inp.shape
-    else:
-        N, D, H, W, C = inp.shape
-    P = grid.size(1) * grid.size(2) * grid.size(3)
-    return N, C, D, H, W, P
+# the grid sampler's operands: input [N,C,D,H,W] (NCDHW) or [N,D,H,W,C] (NDHWC), grid [N,a,b,c,3] read as [N,P,3]
+# with P = a b c, the output cotangent [N,C,a,b,c]
+_GS_INPUT = {LAYOUT_NCDHW: ("N", "C", "D", "H", "W"), LAYOUT_NDHWC: ("N", "D", "H", "W", "C")}
+_GS_GRID = ("N", "a", "b", "c", 3)
+_GS_OUT = ("N", "C", "a", "b", "c")
 
 
-def _check_operand(t, like, shape, name):
-    """t must sit on like's device with like's dtype and the given shape: the kernels read it with like's element type
-    and extent, so anything else would be read as garbage."""
-    if t.device != like.device:
-        raise RuntimeError(f"{name} must be on {like.device}, got {t.device}")
-    if t.dtype != like.dtype:
-        raise RuntimeError(f"{name} must be {like.dtype}, got {t.dtype}")
-    if tuple(t.shape) != tuple(shape):
-        raise RuntimeError(f"{name} must have shape {tuple(shape)}, got {tuple(t.shape)}")
-
-
-def _expect(fn, name, t, dtype, shape, dev=None):
-    """Raise RuntimeError unless t is `dtype` with `shape` (ints fix an extent, letters leave it free) and, when dev is
-    given, sits on dev."""
-    if (t.dtype != dtype or t.dim() != len(shape) or (dev is not None and t.device != dev)
-            or any(isinstance(s, int) and t.shape[d] != s for d, s in enumerate(shape))):
-        on = f" on {dev}" if dev is not None else ""
-        raise RuntimeError(f"{fn}: {name} must be {dtype} [{','.join(map(str, shape))}]{on}, got {t.dtype} "
-                           f"{tuple(t.shape)} on {t.device}")
+def _gs_args(d):
+    return d["N"], d["C"], d["D"], d["H"], d["W"], d["a"] * d["b"] * d["c"], _dtype_code(d["dtype"])
 
 
 def grid_sample3d_forward(inp, grid, layout=LAYOUT_NCDHW):
     """GridSamplerMine.forward(input, grid, 0, 1)  (MCAcc/cuda/GridSamplerMine.cpp:75-81)."""
-    _check_input(inp, "input")
-    _check_input(grid, "grid")
-    code = _dtype_code(inp, "input")
-    N, C, D, H, W, P = _gs_dims(inp, grid, layout)
-    out = torch.empty((N, C, grid.size(1), grid.size(2), grid.size(3)), dtype=inp.dtype,
-                      device=inp.device)
-    _launch("recmv_gridsample3d_fwd", inp, _ptr(inp), _ptr(grid), _ptr(out), N, C, D, H, W, P, code, layout)
+    d = _operands("grid_sample3d_forward", (inp, "input", FLOATS, _GS_INPUT[layout]), (grid, "grid", FLOATS, _GS_GRID))
+    out = torch.empty((d["N"], d["C"], d["a"], d["b"], d["c"]), dtype=inp.dtype, device=inp.device)
+    _launch("recmv_gridsample3d_fwd", inp, _ptr(inp), _ptr(grid), _ptr(out), *_gs_args(d), layout)
     return out
 
 
 def grid_sample3d_backward(inp, grid, grad_out, layout=LAYOUT_NCDHW, need_grad_input=True):
     """GridSamplerMine.backward(input, grid, grad_output, 0, 1) -> (grad_input, grad_grid)."""
-    _check_input(inp, "input")
-    _check_input(grid, "grid")
-    code = _dtype_code(inp, "input")
-    N, C, D, H, W, P = _gs_dims(inp, grid, layout)
-    _check_operand(grad_out, inp, (N, C) + tuple(grid.shape[1:4]), "grad_output")
     grad_out = grad_out.contiguous()
+    d = _operands("grid_sample3d_backward", (inp, "input", FLOATS, _GS_INPUT[layout]), (grid, "grid", FLOATS, _GS_GRID),
+                  (grad_out, "grad_output", FLOATS, _GS_OUT))
     gi = torch.zeros_like(inp) if need_grad_input else None
     gg = torch.empty_like(grid)
-    _launch("recmv_gridsample3d_bwd", inp, _ptr(inp), _ptr(grid), _ptr(grad_out), _ptr(gi), _ptr(gg), N, C, D, H, W, P,
-            code, layout)
+    _launch("recmv_gridsample3d_bwd", inp, _ptr(inp), _ptr(grid), _ptr(grad_out), _ptr(gi), _ptr(gg), *_gs_args(d),
+            layout)
     return gi, gg
 
 
 def grid_sample3d_dbackward(gg_input, gg_grid, inp, grid, grad_out, layout=LAYOUT_NCDHW,
                             need_grad_input=True):
     """GridSamplerMine.dbackward(ggI, ggG, input, grid, grad_output, 0, 1) -> (gI, gG, ggO)."""
-    _check_input(inp, "input")
-    _check_input(grid, "grid")
-    code = _dtype_code(inp, "input")
-    N, C, D, H, W, P = _gs_dims(inp, grid, layout)
-    _check_operand(grad_out, inp, (N, C) + tuple(grid.shape[1:4]), "grad_output")
-    _check_operand(gg_grid, grid, grid.shape, "gg_grid")
     grad_out = grad_out.contiguous()
     gg_grid = gg_grid.contiguous()
-    if gg_input is not None:
-        _check_operand(gg_input, inp, inp.shape, "gg_input")
-        gg_input = gg_input.contiguous()
-    gi =torch.zeros_like(inp) if need_grad_input else None
+    gg_input = gg_input.contiguous() if gg_input is not None else None
+    d = _operands("grid_sample3d_dbackward", (gg_input, "gg_input", FLOATS, _GS_INPUT[layout]),
+                  (gg_grid, "gg_grid", FLOATS, _GS_GRID), (inp, "input", FLOATS, _GS_INPUT[layout]),
+                  (grid, "grid", FLOATS, _GS_GRID), (grad_out, "grad_output", FLOATS, _GS_OUT))
+    gi = torch.zeros_like(inp) if need_grad_input else None
     gg = torch.empty_like(grid)
     ggo = torch.empty_like(grad_out)
-    _launch("recmv_gridsample3d_bwd2", inp, _ptr(gg_input), _ptr(gg_grid), _ptr(inp), _ptr(grid), _ptr(grad_out), _ptr(gi),
-            _ptr(gg), _ptr(ggo), N, C, D, H, W, P, code, layout)
+    _launch("recmv_gridsample3d_bwd2", inp, _ptr(gg_input), _ptr(gg_grid), _ptr(inp), _ptr(grid), _ptr(grad_out),
+            _ptr(gi), _ptr(gg), _ptr(ggo), *_gs_args(d), layout)
     return gi, gg, ggo
 
 
@@ -297,12 +322,9 @@ class _FrozenVoxelSampleBackward(torch.autograd.Function):
 
 def voxel_to_channels_last(ws):
     """[1,C,D,H,W] fp32 -> [D,H,W,C] (private, coalesced copy of LBSkinner.ws)."""
-    _check_input(ws, "ws")
-    if ws.dtype != torch.float32 or ws.dim() != 5 or ws.size(0) != 1:
-        raise RuntimeError(f"voxel_to_channels_last expects a float32 [1,C,D,H,W] voxel, got {ws.dtype} "
-                           f"{tuple(ws.shape)}")
-    _, C, D, H, W = ws.shape
-    out =torch.empty((D, H, W, C), dtype=torch.float32, device=ws.device)
+    d = _operands("voxel_to_channels_last", (ws, "ws", torch.float32, (1, "C", "D", "H", "W")))
+    C, D, H, W = d["C"], d["D"], d["H"], d["W"]
+    out = torch.empty((D, H, W, C), dtype=torch.float32, device=ws.device)
     _launch("recmv_voxel_to_channels_last", ws, _ptr(ws), _ptr(out), C, D, H, W)
     return out
 
@@ -314,10 +336,10 @@ def lbsw_knn_blend(verts, vert_ws, bmin, bmax, resolution, k, align_corners=Fals
     """k-nearest-vertex blend of the skinning weights at every voxel centre (recmv_lbsw_knn_blend).
     verts [V,3], vert_ws [V,24] fp32 CUDA; bmin / bmax: 3 host floats; resolution (W,H,D).
     Returns ws_cl [D,H,W,24] (and idx [D*H*W,k] int32, nearest first, when want_idx)."""
-    _check_input(verts, "verts")
-    _check_input(vert_ws, "vert_ws")
+    d = _operands("lbsw_knn_blend", (verts, "verts", torch.float32, ("V", 3)),
+                  (vert_ws, "vert_ws", torch.float32, ("V", "C")))
     W, H, D = (int(r) for r in resolution)
-    V, C = vert_ws.shape
+    V, C = d["V"], d["C"]
     out = torch.empty((D, H, W, C), dtype=torch.float32, device=verts.device)
     idx = torch.empty((D * H * W, k), dtype=torch.int32, device=verts.device) if want_idx else None
     lo, hi = (c_float * 3)(*[float(v) for v in bmin]), (c_float * 3)(*[float(v) for v in bmax])
@@ -330,10 +352,8 @@ def lbsw_smooth(ws_cl, times, zero_below=0.0):
     """`times` passes of the reference's smooth_weights on a channels-last [D,H,W,24] voxel (recmv_lbsw_smooth), then
     values below zero_below (if > 0) set to 0.  `ws_cl` is consumed (used as the first ping-pong buffer).
     Returns (ws [1,24,D,H,W], ws_cl [D,H,W,24]) -- the second is what LBSkinner samples."""
-    _check_input(ws_cl, "ws_cl")
-    D, H, W, C = ws_cl.shape
-    if C != 24 or ws_cl.dtype != torch.float32:
-        raise RuntimeError("lbsw_smooth expects a float32 [D,H,W,24] voxel")
+    d = _operands("lbsw_smooth", (ws_cl, "ws_cl", torch.float32, ("D", "H", "W", 24)))
+    D, H, W, C = d["D"], d["H"], d["W"], 24
     spare = torch.empty_like(ws_cl) if times >= 2 else None
     out = torch.empty((1, C, D, H, W), dtype=torch.float32, device=ws_cl.device)
     out_cl = torch.empty_like(ws_cl)
@@ -353,10 +373,9 @@ def mc_gpu(sdfs, xstep=1.0, ystep=1.0, zstep=1.0, xmin=0.0, ymin=0.0, zmin=0.0, 
     host synchronisation is the read of (V, F) AFTER everything is queued (the reference blocks between its kernels,
     CudaKernels.cu:628).  The results are fresh tensors, as the reference returns (MCGpu.cpp:49-54).  The one-grid case
     of mc_gpu_many."""
-    _check_input(sdfs, "sdfs")
-    if sdfs.dtype != torch.float32:
-        return []
-    if sdfs.dim() != 3 or min(sdfs.shape) <= 0:
+    if not (sdfs.is_cuda and sdfs.is_contiguous()):   # CHECK_INPUT (MCGpu/MCGpu.cpp:3-5), before the dtype test
+        raise RuntimeError(f"mc_gpu: sdfs must be a contiguous CUDA tensor, got {tuple(sdfs.shape)} on {sdfs.device}")
+    if sdfs.dtype != torch.float32 or sdfs.dim() != 3 or min(sdfs.shape) <= 0:
         return []
     return mc_gpu_many([sdfs], [(xstep, ystep, zstep)], [(xmin, ymin, zmin)], fTargetValue)[0]
 
@@ -375,14 +394,11 @@ def mc_gpu_many(grids, steps, origins, iso=0.0, capacity=(4096, 8192)):
         raise RuntimeError("mc_gpu_many: grids, steps and origins must have the same length")
     if not grids:
         return []
+    _operands("mc_gpu_many", (grids, "grids", torch.float32, (None, None, None)))
+    if any(min(g.shape) <= 0 for g in grids):
+        raise RuntimeError("mc_gpu_many: every grid must be non-empty")
     dev = grids[0].device
-    dims = []
-    for i, g in enumerate(grids):
-        _check_input(g, f"grids[{i}]")
-        if g.device != dev or g.dtype != torch.float32 or g.dim() != 3 or min(g.shape) <= 0:
-            raise RuntimeError(f"mc_gpu_many: grids[{i}] must be a non-empty float32 [NX,NY,NZ] tensor on {dev}, got "
-                               f"{g.dtype} {tuple(g.shape)} on {g.device}")
-        dims.append(tuple(int(n) for n in g.shape))
+    dims = [tuple(int(n) for n in g.shape) for g in grids]
     scratch = _scratch(dev, "mc_scratch", max(_size("recmv_mc_scratch_bytes", *d) for d in dims))
     n = len(grids)
     ctr, host = _counters(dev, ("mc_counters", n), 4 * n)
@@ -421,9 +437,8 @@ def vertex_faces(faces, V, check_indices=False):
     vertex_face_indices(), in a pinned order.  A face with an index outside [0, V) gives (-1, -1) pairs at the end and
     sets a device flag; check_indices=True reads that flag (one host synchronisation) and raises ValueError when it is
     set.  Otherwise nothing is read back."""
-    _check_input(faces, "faces")
-    _expect("vertex_faces", "faces", faces, torch.int64, ("F", 3))
-    dev, F, V = faces.device, int(faces.shape[0]), int(V)
+    F = _operands("vertex_faces", (faces, "faces", torch.int64, ("F", 3)))["F"]
+    dev, V = faces.device, int(V)
     fid = torch.empty((3 * F,), dtype=torch.int64, device=dev)
     vid = torch.empty((3 * F,), dtype=torch.int64, device=dev)
     flag, host = _counters(dev, "vertex_faces_flag", 1)
@@ -437,14 +452,25 @@ def vertex_faces(faces, V, check_indices=False):
 # --------------------------------------------------------------------------------------------------
 # LBS
 # --------------------------------------------------------------------------------------------------
-def make_voxel(ws_cl, center, extend):
+# operand shapes shared by the skinning, deformer, render and surface-solve wrappers
+_POINTS = (..., 3)              # points the kernels read as P = numel / 3 rows of 3
+_BONES = ("F", 24, 4, 4)        # A of F frames; trans is [F,3]
+_VOXEL = ("D", "H", "W", 24)    # the channels-last skinning voxel ws_cl
+
+
+def _voxel(ws_cl, center, extend):
     v = Voxel()
     v.ws_cl = ws_cl.data_ptr()
     v.D, v.H, v.W = int(ws_cl.shape[0]), int(ws_cl.shape[1]), int(ws_cl.shape[2])
-    c = [float(x) for x in center]
-    v.center = (c_float * 3)(*c)
+    v.center = (c_float * 3)(*[float(x) for x in center])
     v.extend = float(extend)
     return v
+
+
+def make_voxel(ws_cl, center, extend):
+    """The recmv_voxel_t of the channels-last voxel ws_cl [D,H,W,24] f32 (CUDA, contiguous) and its box."""
+    _operands("make_voxel", (ws_cl, "ws_cl", torch.float32, _VOXEL))
+    return _voxel(ws_cl, center, extend)
 
 
 def lbs_forward(ps, A, trans, ws_cl, center, extend, batch_inds=None, points_per_frame=0, tps=None,
@@ -452,16 +478,18 @@ def lbs_forward(ps, A, trans, ws_cl, center, extend, batch_inds=None, points_per
     ps = ps.contiguous().float()
     A = A.contiguous().float()
     trans = trans.contiguous().float()
-    P = ps.numel() // 3
-    out = torch.empty_like(ps)
-    wout = torch.empty((P, 24), dtype=torch.float32, device=ps.device) if want_weights else None
     if tps is not None:
         tps = tps.contiguous().float()
     if batch_inds is not None:
         batch_inds = batch_inds.contiguous().long()
-    vox = make_voxel(ws_cl, center, extend)
+    d = _operands("lbs_forward", (ps, "ps", torch.float32, _POINTS), (A, "A", torch.float32, _BONES),
+                  (trans, "trans", torch.float32, ("F", 3)), (ws_cl, "ws_cl", torch.float32, _VOXEL),
+                  (batch_inds, "batch_inds", torch.int64, (...,)), (tps, "tps", torch.float32, _POINTS))
+    P = d[...]
+    out = torch.empty_like(ps)
+    wout = torch.empty((P, 24), dtype=torch.float32, device=ps.device) if want_weights else None
     _launch("recmv_lbs_fwd", ps, _ptr(ps), _ptr(tps), _ptr(A), _ptr(trans), _ptr(batch_inds), int(points_per_frame),
-            int(A.shape[0]), byref(vox), _ptr(out), _ptr(wout), P)
+            d["F"], byref(_voxel(ws_cl, center, extend)), _ptr(out), _ptr(wout), P)
     return (out, wout) if want_weights else out
 
 
@@ -469,43 +497,48 @@ def lbs_inverse(x_obs, A, trans, ws_cl, center, extend, batch_inds=None, points_
     x_obs = x_obs.contiguous().float()
     A = A.contiguous().float()
     trans = trans.contiguous().float()
-    P = x_obs.numel() // 3
-    xc = torch.empty_like(x_obs)
-    valid = torch.empty((P,), dtype=torch.uint8, device=x_obs.device)
     if batch_inds is not None:
         batch_inds = batch_inds.contiguous().long()
-    vox = make_voxel(ws_cl, center, extend)
+    d = _operands("lbs_inverse", (x_obs, "x_obs", torch.float32, _POINTS), (A, "A", torch.float32, _BONES),
+                  (trans, "trans", torch.float32, ("F", 3)), (ws_cl, "ws_cl", torch.float32, _VOXEL),
+                  (batch_inds, "batch_inds", torch.int64, (...,)))
+    P = d[...]
+    xc = torch.empty_like(x_obs)
+    valid = torch.empty((P,), dtype=torch.uint8, device=x_obs.device)
     _launch("recmv_lbs_inverse", x_obs, _ptr(x_obs), _ptr(A), _ptr(trans), _ptr(batch_inds), int(points_per_frame),
-            int(A.shape[0]), byref(vox), _ptr(xc), _ptr(valid), P)
+            d["F"], byref(_voxel(ws_cl, center, extend)), _ptr(xc), _ptr(valid), P)
     return xc, valid.view(torch.bool)
 
 
 def bone_matrices(poses, Js, parents_i32, init_pose=None, want_A=True):
     """(G [F,24,4,4], A [F,24,4,4] or None): the kinematic chain of LBSkinner in one launch (no autograd)."""
     poses = poses.detach().contiguous().float()
-    _check_input(poses, "poses")
-    F_ = poses.shape[0]
+    Js = Js.contiguous().float()
+    ip = init_pose.contiguous().float() if init_pose is not None else None
+    F_ = _operands("bone_matrices", (poses, "poses", torch.float32, ("F", 24, 3)), (Js, "Js", torch.float32, (24, 3)),
+                   (parents_i32, "parents_i32", torch.int32, (24,)), (ip, "init_pose", torch.float32, (24, 4, 4)))["F"]
     dev = poses.device
     G = torch.empty((F_, 24, 4, 4), dtype=torch.float32, device=dev)
     A = torch.empty((F_, 24, 4, 4), dtype=torch.float32, device=dev) if want_A else None
-    ip = init_pose.contiguous().float() if init_pose is not None else None
-    _launch("recmv_bone_matrices", poses, _ptr(poses), _ptr(Js.contiguous().float()), _ptr(parents_i32), _ptr(ip), _ptr(G),
-            _ptr(A), F_)
+    _launch("recmv_bone_matrices", poses, _ptr(poses), _ptr(Js), _ptr(parents_i32), _ptr(ip), _ptr(G), _ptr(A), F_)
     return G, A
 
 
 def bone_matrices_backward(poses, Js, parents_i32, init_pose, G, dG=None, dA=None):
     """dposes [F,24,3] = VJP of bone_matrices at `poses` (G: its output); dG / dA: cotangents of G / A or None."""
     poses = poses.detach().contiguous().float()
-    _check_input(poses, "poses")
-    F_ = poses.shape[0]
-    dev = poses.device
-    dposes = torch.empty((F_, 24, 3), dtype=torch.float32, device=dev)
+    Js = Js.contiguous().float()
+    ip = init_pose.contiguous().float() if init_pose is not None else None
+    G = G.contiguous()
     dG = dG.contiguous().float() if dG is not None else None
     dA = dA.contiguous().float() if dA is not None else None
-    ip = init_pose.contiguous().float() if init_pose is not None else None
-    _launch("recmv_bone_matrices_backward", poses, _ptr(poses), _ptr(Js.contiguous().float()), _ptr(parents_i32), _ptr(ip),
-            _ptr(G.contiguous()), _ptr(dG), _ptr(dA), _ptr(dposes), F_)
+    F_ = _operands("bone_matrices_backward", (poses, "poses", torch.float32, ("F", 24, 3)),
+                   (Js, "Js", torch.float32, (24, 3)), (parents_i32, "parents_i32", torch.int32, (24,)),
+                   (ip, "init_pose", torch.float32, (24, 4, 4)), (G, "G", torch.float32, _BONES),
+                   (dG, "dG", torch.float32, _BONES), (dA, "dA", torch.float32, _BONES))["F"]
+    dposes = torch.empty((F_, 24, 3), dtype=torch.float32, device=poses.device)
+    _launch("recmv_bone_matrices_backward", poses, _ptr(poses), _ptr(Js), _ptr(parents_i32), _ptr(ip), _ptr(G), _ptr(dG),
+            _ptr(dA), _ptr(dposes), F_)
     return dposes
 
 
@@ -537,22 +570,22 @@ def lbs_backward(ps, A, grad_out, ws_cl, center, extend, batch_inds=None, points
     ps = ps.contiguous().float()
     A = A.contiguous().float()
     g = grad_out.contiguous().float()
-    P = ps.numel() // 3
-    F_ = int(A.shape[0])
-    dev = ps.device
     if tps is not None:
         tps = tps.contiguous().float()
     if batch_inds is not None:
         batch_inds = batch_inds.contiguous().long()
+    d = _operands("lbs_backward", (ps, "ps", torch.float32, _POINTS), (A, "A", torch.float32, _BONES),
+                  (g, "grad_out", torch.float32, _POINTS), (ws_cl, "ws_cl", torch.float32, _VOXEL),
+                  (batch_inds, "batch_inds", torch.int64, (...,)), (tps, "tps", torch.float32, _POINTS))
+    P, F_, dev = d[...], d["F"], ps.device
     dps = torch.empty((P, 3), dtype=torch.float32, device=dev) if want_ps else None
     dtps = torch.empty((P, 3), dtype=torch.float32, device=dev) if want_tps and tps is not None else None
     dA = torch.empty((F_, 24, 4, 4), dtype=torch.float32, device=dev) if want_A else None
     dtrans = torch.empty((F_, 3), dtype=torch.float32, device=dev) if want_trans else None
     nbytes = _size("recmv_lbs_backward_workspace_bytes", P, F_)
     work = torch.empty((max(nbytes, 16),), dtype=torch.uint8, device=dev) if (want_A or want_trans) else None
-    vox = make_voxel(ws_cl, center, extend)
     _launch("recmv_lbs_backward", ps, _ptr(ps), _ptr(tps), _ptr(A), None, _ptr(batch_inds), int(points_per_frame), F_,
-            byref(vox), _ptr(g), _ptr(dps), _ptr(dtps), _ptr(dA), _ptr(dtrans), _ptr(work), P)
+            byref(_voxel(ws_cl, center, extend)), _ptr(g), _ptr(dps), _ptr(dtps), _ptr(dA), _ptr(dtrans), _ptr(work), P)
     return dps, dtps, dA, dtrans
 
 
@@ -564,19 +597,21 @@ def lbs_vjp_backward(ps, A, grad_out, ws_cl, center, extend, batch_inds=None, po
     ps = ps.contiguous().float()
     A = A.contiguous().float()
     g = grad_out.contiguous().float()
-    P = ps.numel() // 3
-    F_ = int(A.shape[0])
-    dev = ps.device
     if tps is not None:
         tps = tps.contiguous().float()
     else:
         cot_tps = None
     if batch_inds is not None:
         batch_inds = batch_inds.contiguous().long()
-    if cot_ps is None and cot_tps is None:
-        cot_ps = torch.zeros_like(ps)
     cot_ps = cot_ps.contiguous().float() if cot_ps is not None else None
     cot_tps = cot_tps.contiguous().float() if cot_tps is not None else None
+    d = _operands("lbs_vjp_backward", (ps, "ps", torch.float32, _POINTS), (A, "A", torch.float32, _BONES),
+                  (g, "grad_out", torch.float32, _POINTS), (ws_cl, "ws_cl", torch.float32, _VOXEL),
+                  (batch_inds, "batch_inds", torch.int64, (...,)), (tps, "tps", torch.float32, _POINTS),
+                  (cot_ps, "cot_ps", torch.float32, _POINTS), (cot_tps, "cot_tps", torch.float32, _POINTS))
+    P, F_, dev = d[...], d["F"], ps.device
+    if cot_ps is None and cot_tps is None:
+        cot_ps = torch.zeros_like(ps)
     dg = torch.empty((P, 3), dtype=torch.float32, device=dev) if want_grad_out else None
     dps = torch.empty((P, 3), dtype=torch.float32, device=dev) if want_ps else None
     dtps = torch.empty((P, 3), dtype=torch.float32, device=dev) if want_tps and tps is not None else None
@@ -584,9 +619,9 @@ def lbs_vjp_backward(ps, A, grad_out, ws_cl, center, extend, batch_inds=None, po
     work = None
     if want_A:
         work = torch.empty((max(_size("recmv_lbs_backward_workspace_bytes", P, F_), 16),), dtype=torch.uint8, device=dev)
-    vox = make_voxel(ws_cl, center, extend)
     _launch("recmv_lbs_vjp_backward", ps, _ptr(ps), _ptr(tps), _ptr(A), _ptr(batch_inds), int(points_per_frame), F_,
-            byref(vox), _ptr(g), _ptr(cot_ps), _ptr(cot_tps), _ptr(dg), _ptr(dps), _ptr(dtps), _ptr(dA), _ptr(work), P)
+            byref(_voxel(ws_cl, center, extend)), _ptr(g), _ptr(cot_ps), _ptr(cot_tps), _ptr(dg), _ptr(dps), _ptr(dtps),
+            _ptr(dA), _ptr(work), P)
     return dg, dps, dtps, dA
 
 
@@ -690,10 +725,16 @@ def _pack_weights(net, label, shapes, Ws, bs):
             raise RuntimeError(f"unexpected {label} layer shape {tuple(W.shape)} (want {(o, i)})")
     W_all = torch.cat([W.detach().reshape(-1).float() for W in Ws]).contiguous()
     b_all = torch.cat([b.detach().reshape(-1).float() for b in bs]).contiguous()
-    dev = Ws[0].device
-    packed = _aligned_blob(_size(f"recmv_{net}_packed_bytes"), dev)
+    _operands(f"{net}_pack_weights", (W_all, "Ws", torch.float32, (None,)), (b_all, "bs", torch.float32, (None,)))
+    packed = _aligned_blob(_packed_bytes(net), W_all.device)
     _launch(f"recmv_{net}_pack_weights", W_all, _ptr(W_all), _ptr(b_all), _ptr(packed))
     return packed
+
+
+@functools.cache
+def _packed_bytes(net):
+    """Length of a packed weight blob of `net` (recmv_{net}_packed_bytes): the shape its operand checks demand."""
+    return _size(f"recmv_{net}_packed_bytes")
 
 
 def sdf_pack_weights(Ws, bs):
@@ -712,8 +753,8 @@ def sdf_mlp_forward(x, packed, pe_w=None, mode=None, want_feat=True):
     """ImplicitNetwork.forward on canonical points x [P,3] -> (sdf [P,1], feat [P,256] or None)."""
     mode = DEFAULT_MLP_MODE if mode is None else mode
     x = x.contiguous().float()
-    _check_input(x, "x")
-    P = x.shape[0]
+    P = _operands("sdf_mlp_forward", (x, "x", torch.float32, ("P", 3)),
+                  (packed, "packed", torch.uint8, (_packed_bytes("sdf"),)))["P"]
     sdf = torch.empty((P, 1), dtype=torch.float32, device=x.device)
     feat = torch.empty((P, 256), dtype=torch.float32, device=x.device) if want_feat else None
     _launch("recmv_sdf_mlp_fwd", x, _ptr(x), _ptr(packed), _pe_array(pe_w), _ptr(sdf), _ptr(feat), P, mode)
@@ -726,8 +767,8 @@ def sdf_value_and_grad(x, packed, pe_w=None, mode=None, want_feat=False):
     if mode == MLP_FP32_SIMT:
         raise _lib.RecmvError("the fused value+gradient launch exists for the tensor-core modes only")
     x = x.contiguous().float()
-    _check_input(x, "x")
-    P = x.shape[0]
+    P = _operands("sdf_value_and_grad", (x, "x", torch.float32, ("P", 3)),
+                  (packed, "packed", torch.uint8, (_packed_bytes("sdf"),)))["P"]
     sdf = torch.empty((P, 1), dtype=torch.float32, device=x.device)
     grad = torch.empty((P, 3), dtype=torch.float32, device=x.device)
     feat = torch.empty((P, 256), dtype=torch.float32, device=x.device) if want_feat else None
@@ -1255,21 +1296,24 @@ def deformer_forward(ps, conds, packed, pe_w, batch_inds=None, points_per_frame=
     of the last stage w.r.t. ps (forward-mode launch) when want_jacobian."""
     mode = DEFAULT_MLP_MODE if mode is None else mode
     ps = ps.contiguous().float()
-    _check_input(ps, "ps")
     conds = conds.contiguous().float()
-    P = ps.shape[0]
-    dev = ps.device
-    tr = torch.empty((P, 3), dtype=torch.float32, device=dev) if want_translated else None
-    off = torch.empty((P, 3), dtype=torch.float32, device=dev) if want_offset else None
-    posed, A, trans, vox = None, None, None, None
+    A = trans = ws_cl = vox = posed = None
     if skin is not None:
         A, trans, ws_cl, center, extend = skin
         A, trans = A.contiguous().float(), trans.contiguous().float()
-        vox = byref(make_voxel(ws_cl, center, extend))
-        posed = torch.empty((P, 3), dtype=torch.float32, device=dev)
     if batch_inds is not None:
         batch_inds = batch_inds.contiguous().long()
-    args = (_ptr(ps), _ptr(conds), _ptr(batch_inds), int(points_per_frame), int(conds.shape[0]), _ptr(packed),
+    d = _operands("deformer_forward", (ps, "ps", torch.float32, ("P", 3)), (conds, "conds", torch.float32, ("F", 128)),
+                  (packed, "packed", torch.uint8, (_packed_bytes("translator"),)),
+                  (batch_inds, "batch_inds", torch.int64, ("P",)), (A, "A", torch.float32, _BONES),
+                  (trans, "trans", torch.float32, ("F", 3)), (ws_cl, "ws_cl", torch.float32, _VOXEL))
+    P, dev = d["P"], ps.device
+    tr = torch.empty((P, 3), dtype=torch.float32, device=dev) if want_translated else None
+    off = torch.empty((P, 3), dtype=torch.float32, device=dev) if want_offset else None
+    if skin is not None:
+        vox = byref(_voxel(ws_cl, center, extend))
+        posed = torch.empty((P, 3), dtype=torch.float32, device=dev)
+    args = (_ptr(ps), _ptr(conds), _ptr(batch_inds), int(points_per_frame), d["F"], _ptr(packed),
             _pe_array(pe_w), _ptr(A), _ptr(trans), vox, _ptr(tr), _ptr(off), _ptr(posed))
     if want_jacobian:
         jac = torch.empty((P, 3, 3), dtype=torch.float32, device=dev)
@@ -1291,11 +1335,10 @@ def rendernet_forward(points, normals, view_dirs, feats, packed, pe_w8, mode=Non
     """Fused colour MLP: [P,3] x3 + [P,256] -> rgb [P,3] (tanh)."""
     mode = DEFAULT_MLP_MODE if mode is None else mode
     args = [t.contiguous().float() for t in (points, normals, view_dirs, feats)]
-    for t, n in zip(args, ("points", "normals", "view_dirs", "feature_vectors")):
-        _check_input(t, n)
-    P = args[0].shape[0]
-    if args[3].shape != (P, 256) or any(a.shape != (P, 3) for a in args[:3]):
-        raise RuntimeError("rendernet_forward: expected [P,3] x3 and [P,256]")
+    P = _operands("rendernet_forward", *[(t, n, torch.float32, ("P", 3)) for t, n in
+                                         zip(args[:3], ("points", "normals", "view_dirs"))],
+                  (args[3], "feature_vectors", torch.float32, ("P", 256)),
+                  (packed, "packed", torch.uint8, (_packed_bytes("rendernet"),)))["P"]
     out = torch.empty((P, 3), dtype=torch.float32, device=args[0].device)
     pe = (c_float * 8)(*[float(w) for w in pe_w8])
     _launch("recmv_rendernet_fwd", out, *[_ptr(a) for a in args], _ptr(packed), pe, _ptr(out), P, mode)
@@ -1315,21 +1358,23 @@ def render_sdf(ray_dirs, cam_pos, t_near, t_far, samples, A, trans, ws_cl, cente
     """The fused render path: rays -> samples -> inverse LBS -> PE -> SDF MLP -> sdf [R,S] (+ first hit)."""
     mode = DEFAULT_MLP_MODE if mode is None else mode
     ray_dirs = ray_dirs.contiguous().float()
-    _check_input(ray_dirs, "ray_dirs")
     A = A.contiguous().float()
     trans = trans.contiguous().float()
-    R = ray_dirs.shape[0]
-    dev = ray_dirs.device
+    if frame_of_ray is not None:
+        frame_of_ray = frame_of_ray.contiguous().to(torch.int32)
+    d = _operands("render_sdf", (ray_dirs, "ray_dirs", torch.float32, ("R", 3)), (A, "A", torch.float32, _BONES),
+                  (trans, "trans", torch.float32, ("F", 3)), (ws_cl, "ws_cl", torch.float32, _VOXEL),
+                  (packed, "packed", torch.uint8, (_packed_bytes("sdf"),)),
+                  (frame_of_ray, "frame_of_ray", torch.int32, ("R",)),
+                  (out_sdf, "out_sdf", torch.float32, ("R", int(samples))))
+    R, dev = d["R"], ray_dirs.device
     sdf = out_sdf if out_sdf is not None else torch.empty((R, samples), dtype=torch.float32, device=dev)
     xc = torch.empty((R, samples, 3), dtype=torch.float32, device=dev) if want_xc else None
     hit_idx = torch.empty((R,), dtype=torch.int32, device=dev) if want_hit else None
     hit_t = torch.empty((R,), dtype=torch.float32, device=dev) if want_hit else None
-    if frame_of_ray is not None:
-        frame_of_ray = frame_of_ray.contiguous().to(torch.int32)
     rm = make_raymarch(cam_pos, t_near, t_far, samples)
-    vox = make_voxel(ws_cl, center, extend)
     _launch("recmv_render_sdf", ray_dirs, _ptr(ray_dirs), byref(rm), _ptr(A), _ptr(trans), _ptr(frame_of_ray),
-            int(rays_per_frame), int(A.shape[0]), byref(vox), _ptr(packed), _pe_array(pe_w), _ptr(sdf), _ptr(xc),
+            int(rays_per_frame), d["F"], byref(_voxel(ws_cl, center, extend)), _ptr(packed), _pe_array(pe_w), _ptr(sdf), _ptr(xc),
             _ptr(hit_idx), _ptr(hit_t), R, mode)
     return sdf, xc, hit_idx, hit_t
 
@@ -1338,10 +1383,8 @@ def interp2x_boundary3d_forward(inp, balance_value, order=0):
     """[N,C,D,H,W] f32 -> (output [N,C,2D-1,2H-1,2W-1] f32, is_boundary bool): the reference's optional
     `interp2x_boundary3d.forward` (order 0: its rounding; order 1: the rounding of F.interpolate(trilinear,
     align_corners=True), the default path of Seg3dLossless)."""
-    _check_input(inp, "input")
-    if inp.dtype != torch.float32 or inp.dim() != 5:
-        raise RuntimeError("interp2x_boundary3d: expected a float32 [N,C,D,H,W] tensor")
-    N, C, D, H, W = inp.shape
+    d = _operands("interp2x_boundary3d_forward", (inp, "input", torch.float32, ("N", "C", "D", "H", "W")))
+    N, C, D, H, W = (d[k] for k in "NCDHW")
     out = torch.empty((N, C, 2 * D - 1, 2 * H - 1, 2 * W - 1), dtype=torch.float32, device=inp.device)
     flag = torch.empty(out.shape, dtype=torch.uint8, device=inp.device)
     _launch("recmv_interp2x_boundary3d_fwd", inp, _ptr(inp), _ptr(out), _ptr(flag), N * C, D, H, W, float(balance_value),
@@ -1351,11 +1394,8 @@ def interp2x_boundary3d_forward(inp, balance_value, order=0):
 
 def interp2x_boundary3d_backward(grad_output):
     """grad_output [N,C,2D-1,2H-1,2W-1] f32 -> grad_input [N,C,D,H,W] (`interp2x_boundary3d.backward`)."""
-    _check_input(grad_output, "grad_output")
-    if grad_output.dtype != torch.float32 or grad_output.dim() != 5:
-        raise RuntimeError("interp2x_boundary3d: expected a float32 [N,C,d,h,w] tensor")
-    N, C, d, h, w = grad_output.shape
-    D, H, W = (d + 1) // 2, (h + 1) // 2, (w + 1) // 2
+    s = _operands("interp2x_boundary3d_backward", (grad_output, "grad_output", torch.float32, ("N", "C", "d", "h", "w")))
+    N, C, D, H, W = s["N"], s["C"], (s["d"] + 1) // 2, (s["h"] + 1) // 2, (s["w"] + 1) // 2
     gi = torch.empty((N, C, D, H, W), dtype=torch.float32, device=grad_output.device)
     _launch("recmv_interp2x_boundary3d_bwd", gi, _ptr(grad_output), _ptr(gi), N * C, D, H, W)
     return gi
@@ -1363,9 +1403,9 @@ def interp2x_boundary3d_backward(grad_output):
 
 def c2f_todo_mask(is_boundary, done):
     """(3x3x3 dilation of is_boundary [D,H,W] bool) & ~done [D,H,W] bool -> bool [D,H,W]."""
-    _check_input(is_boundary, "is_boundary")
-    _check_input(done, "done")
-    D, H, W = is_boundary.shape
+    d = _operands("c2f_todo_mask", (is_boundary, "is_boundary", torch.bool, ("D", "H", "W")),
+                  (done, "done", torch.bool, ("D", "H", "W")))
+    D, H, W = d["D"], d["H"], d["W"]
     todo = torch.empty((D, H, W), dtype=torch.uint8, device=done.device)
     _launch("recmv_c2f_todo_mask", todo, _ptr(is_boundary.view(torch.uint8)), _ptr(done.view(torch.uint8)), _ptr(todo),
             D, H, W)
@@ -1378,18 +1418,15 @@ def fragment_decode(pix_to_face, bary, verts, faces, mask=None, camera=None):
     One host synchronisation: the read of the row count (the reference's `nonzero` has the same one)."""
     pix_to_face = pix_to_face.contiguous().long()
     bary = bary.contiguous().float()
-    _check_input(pix_to_face, "pix_to_face")
-    N, H, W, K = pix_to_face.shape
-    dev = pix_to_face.device
     verts = verts.detach().contiguous().float()
     faces = faces.contiguous().long()
-    npix = N * H * W
-    _expect("fragment_decode", "bary", bary, torch.float32, (N, H, W, K, 3), dev)
-    for t, name in ((verts, "verts"), (faces, "faces"), (mask, "mask")):
-        if t is not None and t.device != dev:
-            raise RuntimeError(f"fragment_decode: {name} must be on {dev}, got {t.device}")
-    if mask is not None and mask.numel() != npix:
-        raise RuntimeError(f"fragment_decode: mask must have {npix} elements (N*H*W), got {mask.numel()}")
+    if mask is not None:
+        mask = mask.contiguous().float()
+    d = _operands("fragment_decode", (pix_to_face, "pix_to_face", torch.int64, ("N", "H", "W", "K")),
+                  (bary, "bary", torch.float32, ("N", "H", "W", "K", 3)), (verts, "verts", torch.float32, (..., 3)),
+                  (faces, "faces", torch.int64, ("F", 3)), (mask, "mask", torch.float32, ("N", "H", "W")))
+    N, H, W, K = d["N"], d["H"], d["W"], d["K"]
+    dev, npix = pix_to_face.device, N * H * W
     scratch = torch.empty((_size("recmv_fragment_decode_scratch_bytes", npix),), dtype=torch.uint8, device=dev)
     ob, orow, ocol, ofi = (torch.empty((npix,), dtype=torch.int64, device=dev) for _ in range(4))
     opts = torch.empty((npix, 3), dtype=torch.float32, device=dev)
@@ -1399,10 +1436,8 @@ def fragment_decode(pix_to_face, bary, verts, faces, mask=None, camera=None):
         fx, fy, px, py, R = camera
         cam = (c_float * 13)(float(fx), float(fy), float(px), float(py), *[float(v) for v in torch.as_tensor(R).reshape(-1).tolist()])
     counters = torch.zeros((1,), dtype=torch.int32, device=dev)
-    if mask is not None:
-        mask = mask.contiguous().float()
     _launch("recmv_fragment_decode", bary, _ptr(pix_to_face), _ptr(bary), N, H, W, K, _ptr(verts), _ptr(faces),
-            int(faces.shape[0]), _ptr(mask), cam, _ptr(scratch), _ptr(ob), _ptr(orow), _ptr(ocol), _ptr(opts), _ptr(ofi),
+            d["F"], _ptr(mask), cam, _ptr(scratch), _ptr(ob), _ptr(orow), _ptr(ocol), _ptr(opts), _ptr(ofi),
             _ptr(orays), _ptr(counters))
     n = int(counters.item())
     out = (ob[:n], orow[:n], ocol[:n], opts[:n], ofi[:n])
@@ -1419,14 +1454,9 @@ def rasterize_meshes(verts, faces, cameras, H, W, z_clip=1e-6, area_eps=1e-8, wa
     workspace; only when it overflowed is the call re-run, once, with a list of the reported size.  `capacity` sets the
     list size of the first attempt (the retained one when None).  host_camera=True adds cameras[0] as 16 host floats to
     the same read (what the fragment decode's view rays need)."""
-    for t, name in ((verts, "verts"), (faces, "faces"), (cameras, "cameras")):
-        _check_input(t, name)
-    dev = verts.device
-    _expect("rasterize_meshes", "verts", verts, torch.float32, ("N", "V", 3))
-    _expect("rasterize_meshes", "faces", faces, torch.int64, ("F", 3), dev)
-    N, V = int(verts.shape[0]), int(verts.shape[1])
-    F = int(faces.shape[0])
-    _expect("rasterize_meshes", "cameras", cameras, torch.float32, (N, 16), dev)
+    d = _operands("rasterize_meshes", (verts, "verts", torch.float32, ("N", "V", 3)),
+                  (faces, "faces", torch.int64, ("F", 3)), (cameras, "cameras", torch.float32, ("N", 16)))
+    N, V, F, dev = d["N"], d["V"], d["F"], verts.device
     H, W = int(H), int(W)
     ctr, host = _counters(dev, "raster_counters", 20)       # 4 counters + 16 camera floats
     kept = (dev.index, "raster_pairs")
@@ -1463,20 +1493,12 @@ def zbuf_probe(verts, faces, cameras, H, W, screen_pts, norm_size, fill, z_clip=
     x, y read), norm_size [N,2] f32 (w, h) and fill [N] f32, all CUDA and contiguous.  Returns out [N,Q] f32, and with
     return_taps also (tap_zbuf [N,Q,4] f32, tap_face [N,Q,4] int64): the rasterizer's zbuf and packed face at the taps
     nw, ne, sw, se, (-1, -1) on background and outside the image.  Five launches, no host synchronisation."""
-    for t, name in ((verts, "verts"), (faces, "faces"), (cameras, "cameras"), (screen_pts, "screen_pts"),
-                    (norm_size, "norm_size"), (fill, "fill")):
-        _check_input(t, name)
-    dev = verts.device
-    _expect("zbuf_probe", "verts", verts, torch.float32, ("N", "V", 3))
-    _expect("zbuf_probe", "faces", faces, torch.int64, ("F", 3), dev)
-    N, V, F = int(verts.shape[0]), int(verts.shape[1]), int(faces.shape[0])
-    _expect("zbuf_probe", "cameras", cameras, torch.float32, (N, 16), dev)
-    _expect("zbuf_probe", "screen_pts", screen_pts, torch.float32, (N, "Q", "D"), dev)
-    Q, D = int(screen_pts.shape[1]), int(screen_pts.shape[2])
+    d = _operands("zbuf_probe", (verts, "verts", torch.float32, ("N", "V", 3)), (faces, "faces", torch.int64, ("F", 3)),
+                  (cameras, "cameras", torch.float32, ("N", 16)), (screen_pts, "screen_pts", torch.float32, ("N", "Q", "D")),
+                  (norm_size, "norm_size", torch.float32, ("N", 2)), (fill, "fill", torch.float32, ("N",)))
+    N, V, F, Q, D, dev = d["N"], d["V"], d["F"], d["Q"], d["D"], verts.device
     if D < 2:
         raise RuntimeError(f"zbuf_probe: screen_pts must have at least 2 coordinates, got {D}")
-    _expect("zbuf_probe", "norm_size", norm_size, torch.float32, (N, 2), dev)
-    _expect("zbuf_probe", "fill", fill, torch.float32, (N,), dev)
     H, W = int(H), int(W)
     out = torch.empty((N, Q), dtype=torch.float32, device=dev)
     tz = torch.empty((N, Q, 4), dtype=torch.float32, device=dev) if return_taps else None
@@ -1488,22 +1510,6 @@ def zbuf_probe(verts, faces, cameras, H, W, screen_pts, norm_size, fill, z_clip=
     return (out, tz, tf) if return_taps else out
 
 
-def _points_dims(points, features, K, split_size):
-    """(N, P, split) of a rasterize_points call; split_size None = P (every point in the first image)."""
-    _check_input(points, "points")
-    _expect("rasterize_points", "points", points, torch.float32, ("N", "P", 3))
-    N, P = int(points.shape[0]), int(points.shape[1])
-    if features is not None:
-        _check_operand(features, points, (N, P), "features")
-        _check_input(features, "features")
-    if not 1 <= int(K) <= 64:
-        raise ValueError(f"rasterize_points: points_per_pixel must be in [1, 64], got {K}")
-    split = P if split_size is None else int(split_size)
-    if not 0 <= split <= P:
-        raise ValueError(f"rasterize_points: split_size must be in [0, {P}], got {split_size}")
-    return N, P, split
-
-
 def rasterize_points(points, features, H, W, radius, K, split_size=None, want_fragments=False, capacity=None):
     """K-nearest point rasterizer + alpha compositor (recmv_rasterize_points).  points [N,P,3] f32 (NDC x, NDC y, view z),
     features [N,P] f32 or None (ones), CUDA and contiguous.  split_size=None renders one image; an int s renders two,
@@ -1513,8 +1519,14 @@ def rasterize_points(points, features, H, W, radius, K, split_size=None, want_fr
     One host read per call: the counters after the launch.  Only when the (tile, point) pair list overflowed is the call
     re-run, once, with a list of the reported size.  `capacity` sets the list size of the first attempt (by default the
     largest pair count this device has seen, at least 8 pairs per point)."""
-    G = 1 if split_size is None else 2
-    N, P, split = _points_dims(points, features, K, split_size)
+    d = _operands("rasterize_points", (points, "points", torch.float32, ("N", "P", 3)),
+                  (features, "features", torch.float32, ("N", "P")))
+    N, P = d["N"], d["P"]
+    if not 1 <= int(K) <= 64:
+        raise ValueError(f"rasterize_points: points_per_pixel must be in [1, 64], got {K}")
+    G, split = (1, P) if split_size is None else (2, int(split_size))
+    if not 0 <= split <= P:
+        raise ValueError(f"rasterize_points: split_size must be in [0, {P}], got {split_size}")
     H, W, K = int(H), int(W), int(K)
     dev = points.device
     ctr, host = _counters(dev, "points_counters", 4)
@@ -1549,7 +1561,8 @@ def rasterize_points_backward(grad_images, ws, pairs, N, P, H, W, radius, K, spl
     split = P if split_size is None else int(split_size)
     dev = ws.device
     grad_images = grad_images.contiguous().float()
-    _expect("rasterize_points_backward", "grad_images", grad_images, torch.float32, (G, N, H, W), dev)
+    _operands("rasterize_points_backward", (grad_images, "grad_images", torch.float32, (G, N, H, W)),
+              (ws, "ws", torch.uint8, (None,)))
     grad = torch.empty((N, P, 3), dtype=torch.float32, device=dev)
     scratch = torch.empty((max(int(pairs), 1), 2), dtype=torch.float32, device=dev)
     _launch("recmv_rasterize_points_backward", grad_images, N, P, H, W, float(radius), int(K), split, G, _ptr(ws), int(pairs),
@@ -1587,12 +1600,8 @@ def vertex_normals(verts, faces):
     """Area-weighted vertex normals (recmv_vertex_normals): verts [N,V,3] f32, faces [F,3] int64 shared by the N frames,
     CUDA and contiguous -> [N,V,3] f32, n / max(|n|, 1e-6).  Summed in (face, corner) order without float atomics, so
     bit-identical from run to run; no host synchronisation."""
-    for t, name in ((verts, "verts"), (faces, "faces")):
-        _check_input(t, name)
-    dev = verts.device
-    _expect("vertex_normals", "verts", verts, torch.float32, ("N", "V", 3))
-    _expect("vertex_normals", "faces", faces, torch.int64, ("F", 3), dev)
-    N, V, F = int(verts.shape[0]), int(verts.shape[1]), int(faces.shape[0])
+    d = _operands("vertex_normals", (verts, "verts", torch.float32, ("N", "V", 3)), (faces, "faces", torch.int64, ("F", 3)))
+    N, V, F, dev = d["N"], d["V"], d["F"], verts.device
     out = torch.empty((N, V, 3), dtype=torch.float32, device=dev)
     ws = _scratch(dev, "normals_ws", max(_size("recmv_vertex_normals_workspace_bytes", V, F, dev=dev), 1))
     _launch("recmv_vertex_normals", verts, _ptr(verts), N, V, _ptr(faces), F, _ptr(ws), _ptr(out))
@@ -1604,12 +1613,8 @@ def surface_sample(verts, faces, count, seed, offset=0):
     shared by the M meshes, CUDA and contiguous -> [M,count,3] f32.  Sample s of mesh m is a pure function of (seed,
     offset, m, s) (Philox4x32-10 counter offset + m*count + s), so one call over M meshes equals M calls at offsets
     offset, offset + count, ...  Three launches, bit-identical from run to run, no host synchronisation."""
-    for t, name in ((verts, "verts"), (faces, "faces")):
-        _check_input(t, name)
-    dev = verts.device
-    _expect("surface_sample", "verts", verts, torch.float32, ("M", "V", 3))
-    _expect("surface_sample", "faces", faces, torch.int64, ("F", 3), dev)
-    M, V, F, S = int(verts.shape[0]), int(verts.shape[1]), int(faces.shape[0]), int(count)
+    d = _operands("surface_sample", (verts, "verts", torch.float32, ("M", "V", 3)), (faces, "faces", torch.int64, ("F", 3)))
+    M, V, F, S, dev = d["M"], d["V"], d["F"], int(count), verts.device
     if S < 0:
         raise RuntimeError(f"surface_sample: count must be >= 0, got {S}")
     if F == 0 and M * S > 0:
@@ -1634,34 +1639,23 @@ def train_rays_sample(batch, row, col, init_pts, masks, camera, target, seed, of
         raise RuntimeError("train_rays_sample: batch, row, col, init_pts and masks must have one entry per garment")
     if G == 0:
         return []
-    _check_input(masks[0], "masks")
-    dev = masks[0].device
-    shape = tuple(masks[0].shape)
-    if len(shape) != 3:
-        raise RuntimeError(f"train_rays_sample: masks must be [N,H,W], got {shape}")
-    lists = []
-    for g in range(G):
-        for t, name in ((batch[g], "batch"), (row[g], "row"), (col[g], "col"), (init_pts[g], "init_pts"),
-                        (masks[g], "masks")):
-            _check_input(t, name)
-        P = int(batch[g].shape[0])
-        _expect("train_rays_sample", "masks", masks[g], torch.float32, shape, dev)
-        for t, name in ((batch[g], "batch"), (row[g], "row"), (col[g], "col")):
-            _expect("train_rays_sample", name, t, torch.int64, (P,), dev)
-        _expect("train_rays_sample", "init_pts", init_pts[g], torch.float32, (P, 3), dev)
-        lists.append((P, tuple(torch.empty((P,), dtype=torch.int64, device=dev) for _ in range(3))
-                      + tuple(torch.empty((P, 3), dtype=torch.float32, device=dev) for _ in range(2))))
-    _check_input(camera, "camera")
-    if camera.device != dev or camera.dtype != torch.float32 or camera.numel() < 13:
-        raise RuntimeError(f"train_rays_sample: camera must be f32 with >= 13 values on {dev}")
-    lengths = (ctypes.c_int64 * G)(*[P for P, _ in lists])
-    ptrs = lambda ts: (ctypes.c_void_p * G)(*[t.data_ptr() for t in ts])  # noqa: E731
+    rows = [f"P{g}" for g in range(G)]      # garment g's row count
+    d = _operands("train_rays_sample", *[(t, f"{name}[{g}]", torch.int64, (f"P{g}",)) for name, ts in
+                                         (("batch", batch), ("row", row), ("col", col)) for g, t in enumerate(ts)],
+                  *[(t, f"init_pts[{g}]", torch.float32, (f"P{g}", 3)) for g, t in enumerate(init_pts)],
+                  (masks, "masks", torch.float32, ("N", "H", "W")), (camera, "camera", torch.float32, (...,)))
+    if camera.numel() < 13:
+        raise RuntimeError(f"train_rays_sample: camera must hold >= 13 values, got {camera.numel()}")
+    dev = camera.device
+    lists = [(d[r], tuple(torch.empty((d[r],), dtype=torch.int64, device=dev) for _ in range(3))
+              + tuple(torch.empty((d[r], 3), dtype=torch.float32, device=dev) for _ in range(2))) for r in rows]
+    lengths = (ctypes.c_int64 * G)(*[d[r] for r in rows])
     ws = _scratch(dev, "train_rays_ws", max(_size("recmv_train_rays_workspace_bytes", G, lengths), 1))
     ctr, host = _counters(dev, f"train_rays_counts_{G}", G)
-    N, H, W = shape
-    _launch("recmv_train_rays_sample", masks[0], G, ptrs(batch), ptrs(row), ptrs(col), ptrs(init_pts), lengths,
-            ptrs(masks), N, H, W, _ptr(camera), int(target), int(seed) % (1 << 64), int(offset) % (1 << 64), _ptr(ws),
-            *[ptrs([o[k] for _, o in lists]) for k in range(5)], _ptr(ctr))
+    _launch("recmv_train_rays_sample", masks[0], G, _ptr_array(batch), _ptr_array(row), _ptr_array(col),
+            _ptr_array(init_pts), lengths, _ptr_array(masks), d["N"], d["H"], d["W"], _ptr(camera), int(target),
+            int(seed) % (1 << 64), int(offset) % (1 << 64), _ptr(ws), *[_ptr_array([o[k] for _, o in lists])
+                                                                         for k in range(5)], _ptr(ctr))
     n = _read_counters(ctr, host).tolist()
     return [tuple(t[:n[g]] for t in o) for g, (_, o) in enumerate(lists)]
 
@@ -1679,30 +1673,22 @@ def loss_points_sample(init_pts, verts, check, batch, row, col, rays, S, seed, o
         raise RuntimeError("loss_points_sample: every input list must have one entry per garment")
     if G == 0:
         return []
-    _check_input(verts[0], "verts")
+    # garment g has M{g} rows and V{g} vertices
+    d = _operands("loss_points_sample", *[(t, f"init_pts[{g}]", torch.float32, (f"M{g}", 3)) for g, t in enumerate(init_pts)],
+                  *[(t, f"verts[{g}]", torch.float32, (f"V{g}", 3)) for g, t in enumerate(verts)],
+                  *[(t, f"check[{g}]", torch.bool, (f"M{g}",)) for g, t in enumerate(check)],
+                  *[(t, f"{name}[{g}]", torch.int64, (f"M{g}",)) for name, ts in
+                    (("batch", batch), ("row", row), ("col", col)) for g, t in enumerate(ts)],
+                  *[(t, f"rays[{g}]", torch.float32, (f"M{g}", 3)) for g, t in enumerate(rays)])
+    Ms, Vs = [d[f"M{g}"] for g in range(G)], [d[f"V{g}"] for g in range(G)]
+    if 0 in Vs:
+        raise RuntimeError("loss_points_sample: a garment has no vertices (the draw's rate S / V is undefined)")
     dev = verts[0].device
-    Ms, Vs = [], []
-    for g in range(G):
-        for t, name in ((init_pts[g], "init_pts"), (verts[g], "verts"), (check[g], "check"), (batch[g], "batch"),
-                        (row[g], "row"), (col[g], "col"), (rays[g], "rays")):
-            _check_input(t, name)
-        M, V = int(init_pts[g].shape[0]), int(verts[g].shape[0])
-        _expect("loss_points_sample", "init_pts", init_pts[g], torch.float32, (M, 3), dev)
-        _expect("loss_points_sample", "verts", verts[g], torch.float32, (V, 3), dev)
-        _expect("loss_points_sample", "check", check[g], torch.bool, (M,), dev)
-        _expect("loss_points_sample", "rays", rays[g], torch.float32, (M, 3), dev)
-        for t, name in ((batch[g], "batch"), (row[g], "row"), (col[g], "col")):
-            _expect("loss_points_sample", name, t, torch.int64, (M,), dev)
-        if V == 0:
-            raise RuntimeError("loss_points_sample: a garment has no vertices (the draw's rate S / V is undefined)")
-        Ms.append(M)
-        Vs.append(V)
     Mc, Vc = (ctypes.c_int64 * G)(*Ms), (ctypes.c_int64 * G)(*Vs)
-    ptrs = lambda ts: (ctypes.c_void_p * G)(*[t.data_ptr() if t is not None else None for t in ts])  # noqa: E731
     seed, offset = int(seed) % (1 << 64), int(offset) % (1 << 64)
     ws = _scratch(dev, "loss_points_ws", max(_size("recmv_loss_points_workspace_bytes", G, Mc, Vc), 1))
     ctr, host = _counters(dev, f"loss_points_counts_{G}", 3 * G)
-    _launch("recmv_loss_points_count", verts[0], G, Mc, Vc, ptrs(check), int(S), seed, offset, _ptr(ws), _ptr(ctr))
+    _launch("recmv_loss_points_count", verts[0], G, Mc, Vc, _ptr_array(check), int(S), seed, offset, _ptr(ws), _ptr(ctr))
     n = _read_counters(ctr, host).tolist()
     outs = []
     for g in range(G):
@@ -1710,9 +1696,9 @@ def loss_points_sample(init_pts, verts, check, batch, row, col, rays, S, seed, o
         f32 = lambda *s: torch.empty(s, dtype=torch.float32, device=dev)  # noqa: E731
         i64 = lambda k: torch.empty((k,), dtype=torch.int64, device=dev)  # noqa: E731
         outs.append((f32(nE + nE // 6, 3), f32(2 * nD, 3), f32(nc, 3), f32(nc, 3), i64(nc), i64(nc), i64(nc), i64(nc)))
-    _launch("recmv_loss_points_emit", verts[0], G, ptrs(init_pts), Mc, ptrs(verts), Vc, ptrs(batch), ptrs(row),
-            ptrs(col), ptrs(rays), (ctypes.c_int32 * (3 * G))(*n), int(S), seed, offset, _ptr(ws),
-            *[ptrs([o[k] for o in outs]) for k in range(8)])
+    _launch("recmv_loss_points_emit", verts[0], G, _ptr_array(init_pts), Mc, _ptr_array(verts), Vc, _ptr_array(batch),
+            _ptr_array(row), _ptr_array(col), _ptr_array(rays), (ctypes.c_int32 * (3 * G))(*n), int(S), seed, offset,
+            _ptr(ws), *[_ptr_array([o[k] for o in outs]) for k in range(8)])
     return outs
 
 
@@ -1729,15 +1715,11 @@ class ColorFrameMeanFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, colors, gtCs, batch, row, col, N):
         colors, gtCs = colors.contiguous(), gtCs.contiguous()
-        for t, name in ((colors, "colors"), (gtCs, "gtCs"), (batch, "batch"), (row, "row"), (col, "col")):
-            _check_input(t, name)
-        dev = colors.device
-        M, N = int(colors.shape[0]), int(N)
-        _expect("color_frame_mean", "gtCs", gtCs, torch.float32, (N, "H", "W", 3), dev)   # the kernel bounds b by N
-        _expect("color_frame_mean", "colors", colors, torch.float32, (M, 3), dev)
-        for t, name in ((batch, "batch"), (row, "row"), (col, "col")):
-            _expect("color_frame_mean", name, t, torch.int64, (M,), dev)
-        H, W = int(gtCs.shape[1]), int(gtCs.shape[2])
+        N = int(N)
+        d = _operands("color_frame_mean", (colors, "colors", torch.float32, ("M", 3)),
+                      (gtCs, "gtCs", torch.float32, (N, "H", "W", 3)),      # the kernel bounds b by N
+                      *[(t, name, torch.int64, ("M",)) for t, name in ((batch, "batch"), (row, "row"), (col, "col"))])
+        M, H, W, dev = d["M"], d["H"], d["W"], colors.device
         loss = torch.empty((), dtype=torch.float32, device=dev)
         counts = torch.empty((N,), dtype=torch.int32, device=dev)
         _launch("recmv_color_frame_mean", colors, _ptr(gtCs), N, H, W, _ptr(batch), _ptr(row), _ptr(col), _ptr(colors),
@@ -1770,15 +1752,10 @@ class NormalFrameMeanFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, gtn, J, nx, w, batch, N):
         gtn, J, nx, w = (t.contiguous() for t in (gtn, J, nx, w))
-        for t, name in ((gtn, "gtn"), (J, "J"), (nx, "nx"), (w, "w"), (batch, "batch")):
-            _check_input(t, name)
-        dev = gtn.device
-        M, N = int(gtn.shape[0]), int(N)
-        _expect("normal_frame_mean", "gtn", gtn, torch.float32, (M, 3), dev)
-        _expect("normal_frame_mean", "J", J, torch.float32, (M, 3, 3), dev)
-        _expect("normal_frame_mean", "nx", nx, torch.float32, (M, 3), dev)
-        _expect("normal_frame_mean", "w", w, torch.float32, (M,), dev)
-        _expect("normal_frame_mean", "batch", batch, torch.int64, (M,), dev)
+        M = _operands("normal_frame_mean", (gtn, "gtn", torch.float32, ("M", 3)), (J, "J", torch.float32, ("M", 3, 3)),
+                      (nx, "nx", torch.float32, ("M", 3)), (w, "w", torch.float32, ("M",)),
+                      (batch, "batch", torch.int64, ("M",)))["M"]
+        N, dev = int(N), gtn.device
         loss = torch.empty((), dtype=torch.float32, device=dev)
         counts = torch.empty((N,), dtype=torch.int32, device=dev)
         _launch("recmv_normal_frame_mean", gtn, _ptr(gtn), _ptr(J), _ptr(nx), _ptr(w), _ptr(batch), M, N,
@@ -1801,35 +1778,27 @@ class NormalFrameMeanFunction(torch.autograd.Function):
         return (dgtn if need[0] else None), (dJ if need[1] else None), (dnx if need[2] else None), None, None, None
 
 
-def _mask_iou_inputs(fn, a, b, names):
-    """Check two lists of G f32 [N,H,W] CUDA tensors of one shape on one device; returns (G, N, H, W)."""
-    if len(a) == 0 or len(a) != len(b):
-        raise RuntimeError(f"{fn}: expected the same number (>= 1) of {names[0]} and {names[1]}, got {len(a)} and "
-                           f"{len(b)}")
-    dev = a[0].device
-    _expect(fn, names[0], a[0], torch.float32, ("N", "H", "W"))
-    for t, name in [(t, names[0]) for t in a] + [(t, names[1]) for t in b]:
-        _check_input(t, name)
-        _expect(fn, name, t, torch.float32, tuple(a[0].shape), dev)
-    return (len(a),) + tuple(int(s) for s in a[0].shape)
-
-
 def mask_iou(masks, gt_masks, r):
     """Dilation and soft IoU of `mask_loss` for G garments (recmv_mask_iou, DESIGN section 1m): masks, gt_masks lists of
     G contiguous f32 [N,H,W] CUDA tensors of one shape, r in 1..32.  Returns (loss [G] f32 = mean_n (1 - I_gn / U_gn), loss_gn [G,N] f32,
     iu [G,N,2] f64 = (I, U), [G dilated masks f32 [N,H,W]]) with the dilation max_pool2d(gt, 2r+1, 1, r) bit for bit,
     I = sum m g', U = sum |m + g' - m g'|.  One pixel launch per 8 garments and one combine launch; deterministic;
     no host synchronisation.  Not differentiable: see MaskIouFunction."""
-    G, N, H, W = _mask_iou_inputs("mask_iou", masks, gt_masks, ("masks", "gt_masks"))
-    dev = masks[0].device
+    G = len(masks)
+    if G == 0 or len(gt_masks) != G:
+        raise RuntimeError(f"mask_iou: expected the same number (>= 1) of masks and gt_masks, got {G} and "
+                           f"{len(gt_masks)}")
+    d = _operands("mask_iou", (masks, "masks", torch.float32, ("N", "H", "W")),
+                  (gt_masks, "gt_masks", torch.float32, ("N", "H", "W")))
+    N, H, W, dev = d["N"], d["H"], d["W"], masks[0].device
     with torch.cuda.device(dev):
         ws = _scratch(dev, "mask_iou_ws", _size("recmv_mask_iou_workspace_bytes", G, N, H, W, int(r)))
     mgt = [torch.empty_like(g) for g in gt_masks]
     iu = torch.empty((G, N, 2), dtype=torch.float64, device=dev)
     loss_gn = torch.empty((G, N), dtype=torch.float32, device=dev)
     loss = torch.empty((G,), dtype=torch.float32, device=dev)
-    ptrs = lambda ts: (ctypes.c_void_p * G)(*[t.data_ptr() for t in ts])  # noqa: E731
-    _launch("recmv_mask_iou", masks[0], G, ptrs(masks), ptrs(gt_masks), N, H, W, int(r), _ptr(ws), ptrs(mgt),
+    _launch("recmv_mask_iou", masks[0], G, _ptr_array(masks), _ptr_array(gt_masks), N, H, W, int(r), _ptr(ws),
+            _ptr_array(mgt),
             _ptr(iu), _ptr(loss_gn), _ptr(loss))
     return loss, loss_gn, iu, mgt
 
@@ -1838,15 +1807,17 @@ def mask_iou_backward(masks, mgt, iu, grad_loss):
     """dL/dm of mask_iou for the upstream gradient grad_loss [G] f32 (recmv_mask_iou_backward): G f32 [N,H,W] tensors
     -(w_g / N) (g' U - I s (1 - g')) / U^2, s = sign(m + g' - m g') with sign(0) = 0, from the forward's dilated masks
     and iu.  One launch per 8 garments; no host synchronisation."""
-    G, N, H, W = _mask_iou_inputs("mask_iou_backward", masks, mgt, ("masks", "mgt"))
-    dev = masks[0].device
-    _expect("mask_iou_backward", "iu", iu, torch.float64, (G, N, 2), dev)
+    G = len(masks)
+    if G == 0 or len(mgt) != G:
+        raise RuntimeError(f"mask_iou_backward: expected the same number (>= 1) of masks and mgt, got {G} and "
+                           f"{len(mgt)}")
     grad_loss = grad_loss.contiguous().float().reshape(G)
-    _check_input(grad_loss, "grad_loss")
+    d = _operands("mask_iou_backward", (masks, "masks", torch.float32, ("N", "H", "W")),
+                  (mgt, "mgt", torch.float32, ("N", "H", "W")), (iu, "iu", torch.float64, (G, "N", 2)),
+                  (grad_loss, "grad_loss", torch.float32, (G,)))
     dm = [torch.empty_like(m) for m in masks]
-    ptrs = lambda ts: (ctypes.c_void_p * G)(*[t.data_ptr() for t in ts])  # noqa: E731
-    _launch("recmv_mask_iou_backward", masks[0], G, ptrs(masks), ptrs(mgt), N, H, W, _ptr(iu), _ptr(grad_loss),
-            ptrs(dm))
+    _launch("recmv_mask_iou_backward", masks[0], G, _ptr_array(masks), _ptr_array(mgt), d["N"], d["H"], d["W"],
+            _ptr(iu), _ptr(grad_loss), _ptr_array(dm))
     return dm
 
 
@@ -1885,28 +1856,22 @@ class MaskIouFunction(torch.autograd.Function):
         return (None, *[d if need else None for d, need in zip(dm, ctx.needs_input_grad[1:1 + G])]) + (None,) * G
 
 
-def _curve_inputs(fn, center, dirs, init_scale, nx, scale, nx_scale):
-    """Check the curve tensors (f32, contiguous, one CUDA device): center [C,1,3] or [C,3], dirs [C,S,3], init_scale,
-    scale, nx_scale [C,S,1] or [C,S], nx [C,1,3] or [C,3].  Returns (C, S)."""
-    for t, name in ((center, "center"), (dirs, "dirs"), (init_scale, "init_scale"), (nx, "nx"), (scale, "scale"),
-                    (nx_scale, "nx_scale")):
-        _check_input(t, name)
-    dev = dirs.device
-    _expect(fn, "dirs", dirs, torch.float32, ("C", "S", 3), dev)
-    C, S = int(dirs.shape[0]), int(dirs.shape[1])
-    for t, name in ((center, "center"), (nx, "nx")):
-        _expect(fn, name, t.reshape(-1, 3) if t.numel() == 3 * C else t, torch.float32, (C, 3), dev)
-    for t, name in ((init_scale, "init_scale"), (scale, "scale"), (nx_scale, "nx_scale")):
-        _expect(fn, name, t.reshape(C, S) if t.numel() == C * S else t, torch.float32, (C, S), dev)
-    return C, S
+def _curve_specs(center, dirs, init_scale, nx, scale, nx_scale):
+    """Operand specs of the curve tensors: center, nx [C,1,3] or [C,3], dirs [C,S,3], init_scale, scale, nx_scale
+    [C,S,1] or [C,S] (a unit axis is checked merged into its neighbour, as the kernels read it)."""
+    rows = lambda t: t.view(t.shape[0], -1) if t.dim() == 3 else t  # noqa: E731
+    return [(rows(center), "center", torch.float32, ("C", 3)), (dirs, "dirs", torch.float32, ("C", "S", 3)),
+            (rows(init_scale), "init_scale", torch.float32, ("C", "S")), (rows(nx), "nx", torch.float32, ("C", 3)),
+            (rows(scale), "scale", torch.float32, ("C", "S")), (rows(nx_scale), "nx_scale", torch.float32, ("C", "S"))]
 
 
 def curve_fit(center, dirs, init_scale, nx, scale, nx_scale):
     """The feature curves and their regulariser (recmv_curve_fit, DESIGN section 1n): Intersect_Free_Curve's buffers
-    and parameters (see _curve_inputs) -> (v [C,S,3] = center + dirs init_scale relu(scale) + nx_scale nx,
+    and parameters (see _curve_specs) -> (v [C,S,3] = center + dirs init_scale relu(scale) + nx_scale nx,
     reg [C,2] = (sum of 1 - cosine of consecutive normalised differences, sum |mean v - center|) per curve).
     Formed in double, rounded once; one launch; deterministic."""
-    C, S = _curve_inputs("curve_fit", center, dirs, init_scale, nx, scale, nx_scale)
+    d = _operands("curve_fit", *_curve_specs(center, dirs, init_scale, nx, scale, nx_scale))
+    C, S = d["C"], d["S"]
     v = torch.empty((C, S, 3), dtype=torch.float32, device=dirs.device)
     reg = torch.empty((C, 2), dtype=torch.float32, device=dirs.device)
     _launch("recmv_curve_fit", dirs, C, S, *map(_ptr, (center, dirs, init_scale, nx, scale, nx_scale, v, reg)))
@@ -1916,13 +1881,11 @@ def curve_fit(center, dirs, init_scale, nx, scale, nx_scale):
 def curve_fit_backward(center, dirs, init_scale, nx, scale, nx_scale, dv, dreg):
     """(dscale, dnx_scale) [C,S,1] of curve_fit for the upstream dv [C,S,3] (None = 0) and dreg [C,2], with torch's
     rules at relu(0), zero-length differences and the cosine eps clamp (recmv_curve_fit_backward)."""
-    C, S = _curve_inputs("curve_fit_backward", center, dirs, init_scale, nx, scale, nx_scale)
-    dev = dirs.device
-    if dv is not None:
-        dv = dv.float().contiguous()
-        _expect("curve_fit_backward", "dv", dv, torch.float32, (C, S, 3), dev)
+    dv = dv.float().contiguous() if dv is not None else None
     dreg = dreg.float().contiguous()
-    _expect("curve_fit_backward", "dreg", dreg, torch.float32, (C, 2), dev)
+    d = _operands("curve_fit_backward", *_curve_specs(center, dirs, init_scale, nx, scale, nx_scale),
+                  (dv, "dv", torch.float32, ("C", "S", 3)), (dreg, "dreg", torch.float32, ("C", 2)))
+    C, S, dev = d["C"], d["S"], dirs.device
     dscale = torch.empty((C, S, 1), dtype=torch.float32, device=dev)
     dnx = torch.empty((C, S, 1), dtype=torch.float32, device=dev)
     _launch("recmv_curve_fit_backward", dirs, C, S,
@@ -1962,15 +1925,9 @@ def curve_project(X, cams, W, H, curves, thresholds, S, fl_masks, body):
     of K (base, stride, column) and thresholds K floats: curve k owns in frame n the S rows base + n stride + s, reads
     fl_masks [N,M] column `column` and tests body [R] < threshold.  Returns (screen [R,3] (x, y, ndc z), visible [R]
     bool, slot [R] int32, clouds [K N, S, 2], counts [K N] int64).  One launch; no host synchronisation."""
-    for t, name in ((X, "X"), (cams, "cams"), (fl_masks, "fl_masks"), (body, "body")):
-        _check_input(t, name)
-    dev = X.device
-    _expect("curve_project", "X", X, torch.float32, ("R", 3), dev)
-    R = int(X.shape[0])
-    _expect("curve_project", "cams", cams, torch.float32, ("N", 16), dev)
-    N = int(cams.shape[0])
-    _expect("curve_project", "fl_masks", fl_masks, torch.float32, (N, "M"), dev)
-    _expect("curve_project", "body", body, torch.float32, (R,), dev)
+    d = _operands("curve_project", (X, "X", torch.float32, ("R", 3)), (cams, "cams", torch.float32, ("N", 16)),
+                  (fl_masks, "fl_masks", torch.float32, ("N", "M")), (body, "body", torch.float32, ("R",)))
+    R, N, dev = d["R"], d["N"], X.device
     K = len(curves)
     if K == 0 or len(thresholds) != K:
         raise RuntimeError(f"curve_project: expected K >= 1 curves and K thresholds, got {K} and {len(thresholds)}")
@@ -1984,7 +1941,7 @@ def curve_project(X, cams, W, H, curves, thresholds, S, fl_masks, body):
     clouds = torch.empty((K * N, int(S), 2), dtype=torch.float32, device=dev)
     counts = torch.empty((K * N,), dtype=torch.int64, device=dev)
     _launch("recmv_curve_project", X, _ptr(X), R, _ptr(cams), N, int(W), int(H), table, thr, K, int(S),
-            _ptr(fl_masks), int(fl_masks.shape[1]), _ptr(body), _ptr(ws), _ptr(screen), _ptr(visible), _ptr(slot),
+            _ptr(fl_masks), d["M"], _ptr(body), _ptr(ws), _ptr(screen), _ptr(visible), _ptr(slot),
             _ptr(clouds), _ptr(counts))
     return screen, visible, slot, clouds, counts
 
@@ -1992,11 +1949,10 @@ def curve_project(X, cams, W, H, curves, thresholds, S, fl_masks, body):
 def curve_project_backward(X, cams, K, S, slot, dclouds):
     """dX [R,3] of curve_project's clouds for dclouds [K N, S, 2]: J^T dclouds[slot] per row, 0 for rows without a
     slot (recmv_curve_project_backward); a gather, no atomics."""
-    dev = X.device
-    R, N = int(X.shape[0]), int(cams.shape[0])
     dclouds = dclouds.float().contiguous()
-    _expect("curve_project_backward", "dclouds", dclouds, torch.float32, (K * N, S, 2), dev)
-    _expect("curve_project_backward", "slot", slot, torch.int32, (R,), dev)
+    d = _operands("curve_project_backward", (X, "X", torch.float32, ("R", 3)), (cams, "cams", torch.float32, ("N", 16)),
+                  (slot, "slot", torch.int32, ("R",)), (dclouds, "dclouds", torch.float32, (lambda b: K * b["N"], S, 2)))
+    R, N, dev = d["R"], d["N"], X.device
     dX = torch.empty((R, 3), dtype=torch.float32, device=dev)
     _launch("recmv_curve_project_backward", X, _ptr(X), R, _ptr(cams), N, int(K), int(S), _ptr(slot), _ptr(dclouds),
             _ptr(dX))
@@ -2036,62 +1992,41 @@ def shade_phong(frags, verts, normals, colors, faces, params):
     light location and colours, material colours, shininess, background).  All CUDA and contiguous.
     Returns [N,H,W,4] f32 RGBA with alpha 1."""
     p2f, bary = (frags.pix_to_face, frags.bary_coords) if hasattr(frags, "pix_to_face") else (frags[0], frags[2])
-    for t, name in ((p2f, "pix_to_face"), (bary, "bary_coords"), (verts, "verts"), (normals, "normals"),
-                    (faces, "faces"), (params, "params")) + (((colors, "colors"),) if colors is not None else ()):
-        _check_input(t, name)
-    dev = verts.device
-    _expect("shade_phong", "pix_to_face", p2f, torch.int64, ("N", "H", "W", 1), dev)
-    N, H, W = (int(s) for s in p2f.shape[:3])
-    _expect("shade_phong", "bary_coords", bary, torch.float32, (N, H, W, 1, 3), dev)
-    _expect("shade_phong", "verts", verts, torch.float32, (N, "V", 3))
-    V = int(verts.shape[1])
-    for t, name in ((normals, "normals"), (colors, "colors")):
-        if t is not None:
-            _expect("shade_phong", name, t, torch.float32, (N, V, 3), dev)
-    _expect("shade_phong", "faces", faces, torch.int64, ("F", 3), dev)
-    _expect("shade_phong", "params", params, torch.float32, (N, SHADE_PARAMS), dev)
+    d = _operands("shade_phong", (p2f, "pix_to_face", torch.int64, ("N", "H", "W", 1)),
+                  (bary, "bary_coords", torch.float32, ("N", "H", "W", 1, 3)), (verts, "verts", torch.float32, ("N", "V", 3)),
+                  (normals, "normals", torch.float32, ("N", "V", 3)), (colors, "colors", torch.float32, ("N", "V", 3)),
+                  (faces, "faces", torch.int64, ("F", 3)), (params, "params", torch.float32, ("N", SHADE_PARAMS)))
+    N, H, W, V, dev = d["N"], d["H"], d["W"], d["V"], verts.device
     out = torch.empty((N, H, W, 4), dtype=torch.float32, device=dev)
     _launch("recmv_shade_phong", verts, _ptr(p2f), _ptr(bary), N, H, W, _ptr(verts), _ptr(normals), _ptr(colors), V,
-            _ptr(faces), int(faces.shape[0]), _ptr(params), _ptr(out))
+            _ptr(faces), d["F"], _ptr(params), _ptr(out))
     return out
-
-
-def _knn_lengths(lengths, N, dev, name):
-    if lengths is None:
-        return None
-    _check_input(lengths, name)
-    _expect("knn_nearest", name, lengths, torch.int64, (N,), dev)
-    return lengths
 
 
 def knn_nearest(p1, p2, lengths1=None, lengths2=None):
     """Nearest neighbour of every p1 point in p2 (recmv_knn_nearest): p1 [N,P1,D], p2 [N,P2,D] f32, D = 2 or 3, lengths
     int64 [N] on the device or None, all CUDA and contiguous.  Returns (dists [N,P1] f32 squared distance, idx [N,P1]
     int64); padded rows (i >= lengths1, or lengths2 == 0) get 0 and -1.  Deterministic; no host synchronisation."""
-    for t, name in ((p1, "p1"), (p2, "p2")):
-        _check_input(t, name)
-        if t.dtype != torch.float32 or t.dim() != 3 or t.shape[2] not in (2, 3):
-            raise RuntimeError(f"knn_nearest: {name} must be float32 [N,P,2|3], got {t.dtype} {tuple(t.shape)}")
-    dev = p1.device
-    N, P1, D = (int(s) for s in p1.shape)
-    _expect("knn_nearest", "p2", p2, torch.float32, (N, "P2", D), dev)
-    P2 = int(p2.shape[1])
-    l1, l2 = _knn_lengths(lengths1, N, dev, "lengths1"), _knn_lengths(lengths2, N, dev, "lengths2")
+    d = _operands("knn_nearest", (p1, "p1", torch.float32, ("N", "P1", "D")), (p2, "p2", torch.float32, ("N", "P2", "D")),
+                  (lengths1, "lengths1", torch.int64, ("N",)), (lengths2, "lengths2", torch.int64, ("N",)))
+    N, P1, P2, D, dev = d["N"], d["P1"], d["P2"], d["D"], p1.device
+    if D not in (2, 3):
+        raise RuntimeError(f"knn_nearest: the points must have 2 or 3 coordinates, got {D}")
     dists = torch.empty((N, P1), dtype=torch.float32, device=dev)
     idx = torch.empty((N, P1), dtype=torch.int64, device=dev)
     ws = _scratch(dev, "knn_ws", max(_size("recmv_knn_workspace_bytes", N, P1, P2, dev=dev), 1))
-    _launch("recmv_knn_nearest", p1, _ptr(p1), _ptr(p2), _ptr(l1), _ptr(l2), N, P1, P2, D, _ptr(ws), _ptr(dists), _ptr(idx))
+    _launch("recmv_knn_nearest", p1, _ptr(p1), _ptr(p2), _ptr(lengths1), _ptr(lengths2), N, P1, P2, D, _ptr(ws), _ptr(dists), _ptr(idx))
     return dists, idx
 
 
 def knn_nearest_backward(p1, p2, idx, grad_dists, need_p2=True):
     """(grad_p1 [N,P1,D], grad_p2 [N,P2,D] or None) of knn_nearest's dists (recmv_knn_nearest_backward), from its idx
     and grad_dists [N,P1].  grad_p2 sums each candidate's queries in increasing index without float atomics."""
-    N, P1, D = (int(s) for s in p1.shape)
-    P2 = int(p2.shape[1])
-    dev = p1.device
     grad_dists = grad_dists.contiguous().float()
-    _expect("knn_nearest_backward", "grad_dists", grad_dists, torch.float32, (N, P1), dev)
+    d = _operands("knn_nearest_backward", (p1, "p1", torch.float32, ("N", "P1", "D")),
+                  (p2, "p2", torch.float32, ("N", "P2", "D")), (idx, "idx", torch.int64, ("N", "P1")),
+                  (grad_dists, "grad_dists", torch.float32, ("N", "P1")))
+    N, P1, P2, D, dev = d["N"], d["P1"], d["P2"], d["D"], p1.device
     g1 = torch.empty((N, P1, D), dtype=torch.float32, device=dev)
     g2 = torch.empty((N, P2, D), dtype=torch.float32, device=dev) if need_p2 else None
     ws = _scratch(dev, "knn_ws", max(_size("recmv_knn_workspace_bytes", N, P1, P2, dev=dev), 1))
@@ -2130,10 +2065,8 @@ def mesh_adjacency(faces, V):
     CSR of the unique sorted face sides, neighbours ascending; col[row_ptr[V]:] is -1.  A vertex is on the boundary when
     one of its sides occurs once among the 3F sides; faces with an index outside [0, V) are skipped.  No host
     synchronisation."""
-    _check_input(faces, "faces")
-    dev = faces.device
-    _expect("mesh_adjacency", "faces", faces, torch.int64, ("F", 3))
-    F, V = int(faces.shape[0]), int(V)
+    F = _operands("mesh_adjacency", (faces, "faces", torch.int64, ("F", 3)))["F"]
+    dev, V = faces.device, int(V)
     row_ptr = torch.empty((V + 1,), dtype=torch.int32, device=dev)
     col = torch.empty((6 * F,), dtype=torch.int32, device=dev)
     deg = torch.empty((V,), dtype=torch.int32, device=dev)
@@ -2147,16 +2080,12 @@ def mesh_adjacency(faces, V):
 def nricp_warp(X, x, normals=None):
     """Local affine warp (recmv_nricp_warp): X [V,3,4] f32 = [A | b] per vertex, x [V,3] f32 -> v = A x + b [V,3]; with
     normals [V,3] also (n' = inv(A)^T n [V,3], ok [V] bool), n' = 0 where |det A| < 1e-4.  All CUDA and contiguous."""
-    for t, name in ((X, "X"), (x, "x")) + (((normals, "normals"),) if normals is not None else ()):
-        _check_input(t, name)
+    V = _operands("nricp_warp", (X, "X", torch.float32, ("V", 3, 4)), (x, "x", torch.float32, ("V", 3)),
+                  (normals, "normals", torch.float32, ("V", 3)))["V"]
     dev = x.device
-    _expect("nricp_warp", "x", x, torch.float32, ("V", 3))
-    V = int(x.shape[0])
-    _expect("nricp_warp", "X", X, torch.float32, (V, 3, 4), dev)
     v = torch.empty((V, 3), dtype=torch.float32, device=dev)
     n_out = ok = None
     if normals is not None:
-        _expect("nricp_warp", "normals", normals, torch.float32, (V, 3), dev)
         n_out = torch.empty((V, 3), dtype=torch.float32, device=dev)
         ok = torch.empty((V,), dtype=torch.bool, device=dev)
     _launch("recmv_nricp_warp", x, _ptr(X), _ptr(x), _ptr(normals), V, _ptr(v), _ptr(n_out), _ptr(ok))
@@ -2174,28 +2103,16 @@ def nricp_step(x, normals, target_v, target_n, corr_idx, adjacency, X, moments, 
     {data sum, stiffness term, Laplacian term, loss, gate count, S, 0, 0} before the update.  Two launches, no host
     synchronisation, bit-identical from run to run."""
     row_ptr, col, _deg, boundary = adjacency
-    for t, name in ((x, "x"), (normals, "normals"), (target_v, "target_v"), (target_n, "target_n"),
-                    (corr_idx, "corr_idx"), (row_ptr, "row_ptr"), (col, "col"), (boundary, "boundary"), (X, "X"),
-                    (moments[0], "exp_avg"), (moments[1], "exp_avg_sq"), (moments[2], "max_exp_avg_sq")):
-        _check_input(t, name)
-    dev = x.device
-    _expect("nricp_step", "x", x, torch.float32, ("V", 3))
-    V = int(x.shape[0])
-    _expect("nricp_step", "normals", normals, torch.float32, (V, 3), dev)
-    _expect("nricp_step", "target_v", target_v, torch.float32, ("T", 3), dev)
-    T = int(target_v.shape[0])
-    _expect("nricp_step", "target_n", target_n, torch.float32, (T, 3), dev)
-    _expect("nricp_step", "corr_idx", corr_idx, torch.int64, (V,), dev)
-    _expect("nricp_step", "row_ptr", row_ptr, torch.int32, (V + 1,), dev)
-    _expect("nricp_step", "col", col, torch.int32, ("E",), dev)
-    _expect("nricp_step", "boundary", boundary, torch.bool, (V,), dev)
-    for t, name in ((X, "X"), (moments[0], "exp_avg"), (moments[1], "exp_avg_sq"), (moments[2], "max_exp_avg_sq")):
-        _expect("nricp_step", name, t, torch.float32, (V, 3, 4), dev)
+    d = _operands("nricp_step", (x, "x", torch.float32, ("V", 3)), (normals, "normals", torch.float32, ("V", 3)),
+                  (target_v, "target_v", torch.float32, ("T", 3)), (target_n, "target_n", torch.float32, ("T", 3)),
+                  (corr_idx, "corr_idx", torch.int64, ("V",)), (row_ptr, "row_ptr", torch.int32, (lambda b: b["V"] + 1,)),
+                  (col, "col", torch.int32, (None,)), (boundary, "boundary", torch.bool, ("V",)),
+                  *[(t, name, torch.float32, ("V", 3, 4)) for t, name in
+                    ((X, "X"), (moments[0], "exp_avg"), (moments[1], "exp_avg_sq"), (moments[2], "max_exp_avg_sq"))],
+                  (stats, "stats", torch.float32, (NRICP_STATS,)))
+    V, T, dev = d["V"], d["T"], x.device
     if stats is None:
         stats = torch.empty((NRICP_STATS,), dtype=torch.float32, device=dev)
-    else:
-        _check_input(stats, "stats")
-        _expect("nricp_step", "stats", stats, torch.float32, (NRICP_STATS,), dev)
     prm = _lib.NricpParams(stiffness_weight, laplacian_weight, gamma, threshold, lr, betas[0], betas[1], eps,
                            weight_decay, int(step))
     ws = _scratch(dev, "nricp_ws", max(_size("recmv_nricp_workspace_bytes", V), 1))
@@ -2219,23 +2136,13 @@ def laplacian_edit(verts, adjacency, cidx, ctgt, constrain_weight=1.0, smooth=Tr
     constraints skipped}.  Three launches, no host synchronisation.  max_blocks caps the solver's grid (0: every
     co-resident block); the result does not depend on it."""
     row_ptr, col, deg, _boundary = adjacency
-    for t, name in ((verts, "verts"), (row_ptr, "row_ptr"), (col, "col"), (deg, "deg"), (cidx, "cidx"),
-                    (ctgt, "ctgt")):
-        _check_input(t, name)
-    dev = verts.device
-    _expect("laplacian_edit", "verts", verts, torch.float32, ("V", 3))
-    V = int(verts.shape[0])
-    _expect("laplacian_edit", "row_ptr", row_ptr, torch.int32, (V + 1,), dev)
-    _expect("laplacian_edit", "col", col, torch.int32, ("E",), dev)
-    _expect("laplacian_edit", "deg", deg, torch.int32, (V,), dev)
-    _expect("laplacian_edit", "cidx", cidx, torch.int64, ("M",), dev)
-    M = int(cidx.shape[0])
-    _expect("laplacian_edit", "ctgt", ctgt, torch.float32, (M, 3), dev)
+    d = _operands("laplacian_edit", (verts, "verts", torch.float32, ("V", 3)),
+                  (row_ptr, "row_ptr", torch.int32, (lambda b: b["V"] + 1,)), (col, "col", torch.int32, (None,)),
+                  (deg, "deg", torch.int32, ("V",)), (cidx, "cidx", torch.int64, ("M",)),
+                  (ctgt, "ctgt", torch.float32, ("M", 3)), (stats, "stats", torch.float32, (LAP_EDIT_STATS,)))
+    V, M, dev = d["V"], d["M"], verts.device
     if stats is None:
         stats = torch.empty((LAP_EDIT_STATS,), dtype=torch.float32, device=dev)
-    else:
-        _check_input(stats, "stats")
-        _expect("laplacian_edit", "stats", stats, torch.float32, (LAP_EDIT_STATS,), dev)
     # the kernel finds each vertex's constraints by binary search: sort them by vertex, keeping duplicates in order
     cidx, order = torch.sort(cidx, stable=True)
     ctgt = ctgt.index_select(0, order)
@@ -2325,20 +2232,23 @@ def surface_solve(cam_pos, rays, seeds, batch_inds, sdf_packed, sdf_pe_w, tr_pac
     mode = DEFAULT_MLP_MODE if mode is None else mode
     ps = seeds.detach().contiguous().float().clone()
     rays = rays.contiguous().float()
-    _check_input(ps, "seeds")
-    _check_input(rays, "rays")
-    P = ps.shape[0]
-    dev = ps.device
     A, trans, ws_cl, center, extend = skin
     A, trans, conds = A.contiguous().float(), trans.contiguous().float(), conds.contiguous().float()
     bi = batch_inds.contiguous().long() if batch_inds is not None else None
+    d = _operands("surface_solve", (rays, "rays", torch.float32, ("P", 3)), (ps, "seeds", torch.float32, ("P", 3)),
+                  (bi, "batch_inds", torch.int64, ("P",)),
+                  (sdf_packed, "sdf_packed", torch.uint8, (_packed_bytes("sdf"),)),
+                  (tr_packed, "tr_packed", torch.uint8, (_packed_bytes("translator"),)),
+                  (conds, "conds", torch.float32, ("F", 128)), (A, "A", torch.float32, _BONES),
+                  (trans, "trans", torch.float32, ("F", 3)), (ws_cl, "ws_cl", torch.float32, _VOXEL))
+    P, dev = d["P"], ps.device
     wsz = _size("recmv_surface_solve_workspace", P)
     work = torch.empty((max(wsz, 1),), dtype=torch.uint8, device=dev)
     ok = torch.empty((P,), dtype=torch.uint8, device=dev)
     cam = (c_float * 3)(*[float(v) for v in cam_pos.view(-1).tolist()])
     _launch("recmv_surface_solve", ps, cam, _ptr(rays), _ptr(ps), _ptr(bi), _ptr(sdf_packed), _pe_array(sdf_pe_w),
-            _ptr(tr_packed), _pe_array(tr_pe_w), _ptr(conds), int(conds.shape[0]), _ptr(A), _ptr(trans),
-            byref(make_voxel(ws_cl, center, extend)), float(dthreshold), float(athreshold), float(w1), float(w2), int(times),
+            _ptr(tr_packed), _pe_array(tr_pe_w), _ptr(conds), d["F"], _ptr(A), _ptr(trans),
+            byref(_voxel(ws_cl, center, extend)), float(dthreshold), float(athreshold), float(w1), float(w2), int(times),
             mode, _ptr(work), wsz, _ptr(ok), P)
     return ps, ok.view(torch.bool)
 
@@ -2347,13 +2257,11 @@ def surface_grad_coeffs(grad_l_p, grad_f_p, jac, rays, d_minus_c=None):
     """Per-ray algebra of propagateTmpPsGrad (OptimNetwork.py:788-851) in one launch.
     Returns (sdf_coef [n], def_vec [n,3], ray_grad [n,3] or None, ok [n] bool)."""
     args = [t.contiguous().float() for t in (grad_l_p, grad_f_p, jac, rays)]
-    for t, name in zip(args, ("grad_l_p", "grad_f_p", "jac", "rays")):
-        _check_input(t, name)
-    n = args[0].shape[0]
-    if args[2].shape != (n, 3, 3) or any(a.shape != (n, 3) for a in (args[0], args[1], args[3])):
-        raise RuntimeError("surface_grad_coeffs: expected [n,3], [n,3], [n,3,3], [n,3]")
-    dev = args[0].device
     dc = d_minus_c.contiguous().float() if d_minus_c is not None else None
+    n = _operands("surface_grad_coeffs", *[(t, name, torch.float32, ("n", 3, 3) if name == "jac" else ("n", 3))
+                                           for t, name in zip(args + [dc], ("grad_l_p", "grad_f_p", "jac", "rays",
+                                                                             "d_minus_c"))])["n"]
+    dev = args[0].device
     coef = torch.empty((n,), dtype=torch.float32, device=dev)
     vec = torch.empty((n, 3), dtype=torch.float32, device=dev)
     rg = torch.empty((n, 3), dtype=torch.float32, device=dev) if dc is not None else None
@@ -2379,23 +2287,15 @@ def implicit_surface_grad(grad_l_p, grad_f_p, jac, rays, d, offsets, cam_pos=Non
     G = len(offs) - 1
     if G < 0:
         raise RuntimeError("implicit_surface_grad: offsets needs G + 1 >= 1 entries")
-    names = ("grad_l_p", "grad_f_p", "jac", "rays")
-    for t, name in zip((grad_l_p, grad_f_p, jac, rays), names):
-        _check_input(t, name)
+    n = _operands("implicit_surface_grad", (grad_l_p, "grad_l_p", torch.float32, ("n", 3)),
+                  (grad_f_p, "grad_f_p", torch.float32, ("n", 3)), (jac, "jac", torch.float32, ("n", 3, 3)),
+                  (rays, "rays", torch.float32, ("n", 3)), (d, "d", torch.float32, ("n", 3)),
+                  (cam_pos, "cam_pos", torch.float32, (3,)))["n"]
     dev = grad_l_p.device
-    n = int(grad_l_p.shape[0])
-    for t, name, shape in zip((grad_l_p, grad_f_p, jac, rays), names, ((n, 3), (n, 3), (n, 3, 3), (n, 3))):
-        _expect("implicit_surface_grad", name, t, torch.float32, shape, dev)
     if offs[0] != 0 or offs[-1] != n or any(b < a for a, b in zip(offs, offs[1:])):
         raise RuntimeError(f"implicit_surface_grad: offsets must run from 0 to n = {n} without decreasing, got {offs}")
     if want_ray_grad and (d is None or cam_pos is None):
         raise RuntimeError("implicit_surface_grad: the ray gradient needs d and cam_pos")
-    if d is not None:
-        _check_input(d, "d")
-        _expect("implicit_surface_grad", "d", d, torch.float32, (n, 3), dev)
-    if cam_pos is not None:
-        _check_input(cam_pos, "cam_pos")
-        _expect("implicit_surface_grad", "cam_pos", cam_pos, torch.float32, (3,), dev)
     f32 = lambda *s: torch.empty(s, dtype=torch.float32, device=dev)  # noqa: E731
     coef, vec, ok = f32(n), f32(n, 3), torch.empty((n,), dtype=torch.uint8, device=dev)
     rg = f32(n, 3) if want_ray_grad else None
@@ -2419,10 +2319,9 @@ class Svd3x3Function(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, J):
-        _check_input(J, "J")
         if J.dtype != torch.float32 or J.dim() != 3 or tuple(J.shape[1:]) != (3, 3):
             raise TypeError("svd3x3 expects a float32 [N,3,3] tensor")
-        N = J.shape[0]
+        N = _operands("svd3x3", (J, "J", torch.float32, ("N", 3, 3)))["N"]
         U = torch.empty((N, 3, 3), dtype=torch.float32, device=J.device)
         V = torch.empty((N, 3, 3), dtype=torch.float32, device=J.device)
         S = torch.empty((N, 3), dtype=torch.float32, device=J.device)
