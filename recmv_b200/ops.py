@@ -2,9 +2,11 @@
 raise on non-zero status, wire autograd.  PyTorch is plumbing here (device memory, streams,
 autograd graph); all arithmetic happens in librecmv_b200.so.
 """
+import collections
 import contextlib
 import ctypes
 import functools
+import itertools
 from ctypes import byref, c_float, c_size_t
 
 import torch
@@ -1176,109 +1178,92 @@ def _plain_composite(X0, Ws, bs):
     return h
 
 
-class TranslatorTrainFunction(torch.autograd.Function):
-    """MLPTranslator offset MLP with gradients (model/Deformer.py:171-206): input row [PE6(p) 39 | cond[frame] 128] ->
-    512 x4 ReLU -> 3, forward / backward-data / weight gradient on the tensor cores (csrc/gemm3_tma.cu); returns the OFFSET (the caller
-    adds p).  create_graph=True falls back to a torch graph inside backward, like SdfMlpTrainFunction."""
-    last_backward = None
+# One column range of a ReLU network's input row, in column order: "copy" (apply argument `arg`'s `cols` columns as they
+# are), "pe" (its positional encoding, 3 + 6 bands columns) or "gather" (arg[apply argument `index`], `cols` columns).
+RowSegment = collections.namedtuple("RowSegment", "kind arg cols bands index", defaults=(0, 0, None))
 
-    @staticmethod
-    def forward(ctx, ps, conds, batch_inds, pe_w, *Wb):
+
+def _relu_mlp_train_function(name, layout, doc):
+    """The training Function of a ReLU MLP whose input row is `layout` (RowSegments, zero-padded to a multiple of 4
+    columns): apply(*row inputs, pe_w, *Ws, *bs).  Its backward takes SdfMlpTrainFunction's three branches;
+    `last_backward` says which ran."""
+    ends = list(itertools.accumulate(3 + 6 * s.bands if s.kind == "pe" else s.cols for s in layout))
+    spans = list(zip(layout, [0] + ends, ends))                  # (segment, first column, end column)
+    width = (ends[-1] + 3) // 4 * 4
+    by_arg = sorted(spans, key=lambda sp: sp[0].arg)             # the order of the returned gradients
+    n_in = 1 + max(max(s.arg, s.index or 0) for s in layout)     # row inputs; pe_w follows them, then the parameters
+
+    def forward(ctx, *args):
+        ins, pe_w, Wb = args[:n_in], args[n_in], args[n_in + 1:]
         n = len(Wb) // 2
-        Ws, bs = Wb[:n], Wb[n:]
-        P, dev = ps.shape[0], ps.device
-        X0 = torch.zeros((P, 168), dtype=torch.float32, device=dev)
-        pe_forward(ps, pe_w, 6, X0)
-        X0[:, 39:167] = conds.detach()[batch_inds]
-        out, acts, xplanes = _plain_mlp_forward(X0, Ws, bs)
+        X0 = torch.zeros((ins[0].shape[0], width), dtype=torch.float32, device=ins[0].device)
+        for s, a, b in spans:
+            t = ins[s.arg].detach()
+            if s.kind == "pe":
+                pe_forward(t.contiguous(), pe_w, s.bands, X0[:, a:b])
+            else:
+                X0[:, a:b] = t if s.kind == "copy" else t[ins[s.index]]
+        out, acts, xplanes = _plain_mlp_forward(X0, Wb[:n], Wb[n:])
         ctx.pe_w, ctx.n = [float(w) for w in pe_w], n
-        ctx.save_for_backward(ps, conds, batch_inds, *Wb, *acts, *xplanes)
+        ctx.save_for_backward(*ins, *Wb, *acts, *xplanes)
         return out.contiguous()
 
-    @staticmethod
-    def backward(ctx, g_off):
-        n = ctx.n
-        saved = ctx.saved_tensors
-        ps, conds, batch_inds = saved[:3]
-        Ws, bs, acts, xplanes = saved[3:3 + n], saved[3 + n:3 + 2 * n], saved[3 + 2 * n:3 + 3 * n], saved[3 + 3 * n:]
-        need = ctx.needs_input_grad
-        if torch.is_grad_enabled() and _inputs_only(any(need[4:])):
-            # utils.compute_Jacobian(..., create_graph=True) of the deformation regulariser: see second_order.py
-            from . import second_order
-            TranslatorTrainFunction.last_backward = "fused-tc (create_graph, input gradient)"
-            dX0 = second_order.PlainMlpInputGradFunction.apply(g_off.contiguous().float(), n, *acts, *Ws)
-            dps = second_order.pe_vjp_torch(ps, dX0, ctx.pe_w, 6) if need[0] else None
-            dconds = torch.zeros_like(conds).index_add(0, batch_inds, dX0[:, 39:167]) if need[1] else None
-            return (dps, dconds, None, None, *([None] * (2 * n)))
-        if torch.is_grad_enabled():
-            TranslatorTrainFunction.last_backward = "autograd-composite (create_graph)"
-            res = _composite_grads(lambda ps, conds, *Wb: _plain_composite(
-                torch.cat([_pe_torch(ps, ctx.pe_w, 6), conds[batch_inds]], 1), Wb[:n], Wb[n:]), [ps, conds, *Ws, *bs], [g_off])
-            return (res[0], res[1], None, None, *res[2:])
-        TranslatorTrainFunction.last_backward = "fused-tc"
-        dX0, dW, db = _plain_mlp_backward(g_off.contiguous().float(), Ws, acts, any(need[4:]), need[0] or need[1], xplanes)
-        dps = dconds = None
-        if need[0]:
-            dps = pe_backward(ps, dX0, None, ctx.pe_w, 6)
-        if need[1]:
-            dconds = torch.zeros_like(conds).index_add_(0, batch_inds, dX0[:, 39:167])
-        return (dps, dconds, None, None, *dW, *db)
-
-
-class RenderNetTrainFunction(torch.autograd.Function):
-    """RenderingNetwork_view_norm ('idr', model/RenderNet.py:59-96) with gradients: input row [p 3 | PE4(v) 27 | n 3 |
-    feat 256] -> 512 x4 ReLU -> 3 (pre-tanh; the caller applies tanh), all GEMMs on the tensor cores."""
-    last_backward = None
-
-    @staticmethod
-    def forward(ctx, points, normals, view_dirs, feats, pe_w, *Wb):
-        n = len(Wb) // 2
-        Ws, bs = Wb[:n], Wb[n:]
-        P, dev = points.shape[0], points.device
-        X0 = torch.zeros((P, 292), dtype=torch.float32, device=dev)
-        X0[:, 0:3] = points.detach()
-        pe_forward(view_dirs.detach().contiguous(), pe_w, 4, X0[:, 3:])
-        X0[:, 30:33] = normals.detach()
-        X0[:, 33:289] = feats.detach()
-        out, acts, xplanes = _plain_mlp_forward(X0, Ws, bs)
-        ctx.pe_w, ctx.n = [float(w) for w in pe_w], n
-        ctx.save_for_backward(points, normals, view_dirs, feats, *Wb, *acts, *xplanes)
-        return out.contiguous()
-
-    @staticmethod
     def backward(ctx, g_out):
-        n = ctx.n
-        saved = ctx.saved_tensors
-        points, normals, view_dirs, feats = saved[:4]
-        Ws, bs, acts, xplanes = saved[4:4 + n], saved[4 + n:4 + 2 * n], saved[4 + 2 * n:4 + 3 * n], saved[4 + 3 * n:]
-        need = ctx.needs_input_grad
-        if torch.is_grad_enabled() and _inputs_only(any(need[5:])):
+        n, saved, need = ctx.n, ctx.saved_tensors, ctx.needs_input_grad
+        ins, Ws, bs = saved[:n_in], saved[n_in:n_in + n], saved[n_in + n:n_in + 2 * n]
+        acts, xplanes = saved[n_in + 2 * n:n_in + 3 * n], saved[n_in + 3 * n:]
+        wanted = [sp for sp in by_arg if need[sp[0].arg]]
+        grads = [None] * n_in
+        if torch.is_grad_enabled() and _inputs_only(any(need[n_in + 1:])):
+            # create_graph=True for input gradients only (the translator's Jacobian in the deformation regulariser)
             from . import second_order
-            RenderNetTrainFunction.last_backward = "fused-tc (create_graph, input gradient)"
+            fn.last_backward = "fused-tc (create_graph, input gradient)"
             dX0 = second_order.PlainMlpInputGradFunction.apply(g_out.contiguous().float(), n, *acts, *Ws)
-            dp = dX0[:, 0:3] if need[0] else None
-            dn = dX0[:, 30:33] if need[1] else None
-            dv = second_order.pe_vjp_torch(view_dirs, dX0[:, 3:30], ctx.pe_w, 4) if need[2] else None
-            df = dX0[:, 33:289] if need[3] else None
-            return (dp, dn, dv, df, None, *([None] * (2 * n)))
+            for s, a, b in wanted:
+                t, d = ins[s.arg], dX0[:, a:b]
+                grads[s.arg] = (d if s.kind == "copy" else
+                                second_order.pe_vjp_torch(t, d, ctx.pe_w, s.bands) if s.kind == "pe" else
+                                torch.zeros_like(t).index_add(0, ins[s.index], d))      # out of place: stays in the graph
+            return (*grads, None, *([None] * (2 * n)))
         if torch.is_grad_enabled():
-            RenderNetTrainFunction.last_backward = "autograd-composite (create_graph)"
-            res = _composite_grads(lambda p, nrm, v, f, *Wb: _plain_composite(
-                torch.cat([p, _pe_torch(v, ctx.pe_w, 4), nrm, f], 1), Wb[:n], Wb[n:]),
-                [points, normals, view_dirs, feats, *Ws, *bs], [g_out])
-            return (*res[:4], None, *res[4:])
-        RenderNetTrainFunction.last_backward = "fused-tc"
-        dX0, dW, db = _plain_mlp_backward(g_out.contiguous().float(), Ws, acts, any(need[5:]), any(need[:4]), xplanes)
-        dp = dn = dv = df = None
-        if need[0]:
-            dp = dX0[:, 0:3].contiguous()
-        if need[1]:
-            dn = dX0[:, 30:33].contiguous()
-        if need[2]:
-            dv = pe_backward(view_dirs.detach().contiguous(), dX0[:, 3:], None, ctx.pe_w, 4)
-        if need[3]:
-            df = dX0[:, 33:289].contiguous()
-        return (dp, dn, dv, df, None, *dW, *db)
+            fn.last_backward = "autograd-composite (create_graph)"
+
+            def composite(*xs):
+                X0 = torch.cat([xs[s.arg] if s.kind == "copy" else _pe_torch(xs[s.arg], ctx.pe_w, s.bands)
+                                if s.kind == "pe" else xs[s.arg][xs[s.index]] for s in layout], 1)
+                return _plain_composite(X0, xs[n_in:n_in + n], xs[n_in + n:])
+            res = _composite_grads(composite, [*ins, *Ws, *bs], [g_out])
+            return (*res[:n_in], None, *res[n_in:])
+        fn.last_backward = "fused-tc"
+        dX0, dW, db = _plain_mlp_backward(g_out.contiguous().float(), Ws, acts, any(need[n_in + 1:]), bool(wanted),
+                                          xplanes)
+        for s, a, b in wanted:
+            t, d = ins[s.arg], dX0[:, a:b]
+            grads[s.arg] = (d.contiguous() if s.kind == "copy" else
+                            pe_backward(t.detach().contiguous(), d, None, ctx.pe_w, s.bands) if s.kind == "pe" else
+                            torch.zeros_like(t).index_add_(0, ins[s.index], d))
+        return (*grads, None, *dW, *db)
+
+    fn = type(name, (torch.autograd.Function,), dict(__doc__=doc, row_width=width, last_backward=None,
+                                                     forward=staticmethod(forward), backward=staticmethod(backward)))
+    return fn
+
+
+TranslatorTrainFunction = _relu_mlp_train_function("TranslatorTrainFunction", [
+    RowSegment("pe", 0, bands=6),                       # PE6(ps)
+    RowSegment("gather", 1, cols=128, index=2),         # conds[batch_inds]
+], """MLPTranslator offset MLP with gradients (model/Deformer.py:171-206): apply(ps, conds, batch_inds, pe_w, *Ws, *bs),
+    input row [PE6(p) 39 | cond[frame] 128] -> 512 x4 ReLU -> 3, forward / backward-data / weight gradient on the tensor
+    cores (csrc/gemm3_tma.cu); returns the OFFSET (the caller adds p).""")
+
+RenderNetTrainFunction = _relu_mlp_train_function("RenderNetTrainFunction", [
+    RowSegment("copy", 0, cols=3),                      # points
+    RowSegment("pe", 2, bands=4),                       # PE4(view_dirs)
+    RowSegment("copy", 1, cols=3),                      # normals
+    RowSegment("copy", 3, cols=256),                    # feats
+], """RenderingNetwork_view_norm ('idr', model/RenderNet.py:59-96) with gradients: apply(points, normals, view_dirs,
+    feats, pe_w, *Ws, *bs), input row [p 3 | PE4(v) 27 | n 3 | feat 256] -> 512 x4 ReLU -> 3 (pre-tanh; the caller
+    applies tanh), all GEMMs on the tensor cores.""")
 
 
 TRANSLATOR_LAYER_SHAPES = [(512, 167), (512, 512), (512, 512), (512, 512), (3, 512)]
