@@ -1,4 +1,4 @@
-// Shared helpers for librecmv_b200.so (sm_100a only).
+// Shared helpers for librecmv_b200.so (sm_90a only).
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -32,7 +32,7 @@ inline int num_sms() {
   return n;
 }
 
-// grid for a grid-stride kernel: a whole number of waves over the SMs (148 on B200)
+// grid for a grid-stride kernel: a whole number of waves over the SMs (132 on an H100 SXM)
 inline int stride_grid(int64_t work, int threads, int ctas_per_sm) {
   int64_t need = (work + threads - 1) / threads;
   int64_t cap = (int64_t)num_sms() * ctas_per_sm;
@@ -275,25 +275,6 @@ __device__ __forceinline__ void lbs_forward_jac(const Voxel& v, const float* __r
   }
 }
 
-// ------------------------------------------------------------------------------------------
-// SDF network geometry (model/network.py:135-141 getTmpSdf)
-// ------------------------------------------------------------------------------------------
-constexpr int kNumLayers = 9;
-constexpr int kPE = 39;     // 3 + 3*2*6
-constexpr int kHidden = 512;
-constexpr int kSkipOut = 473;  // layer 3 out = 512 - 39
-constexpr int kOutDim = 257;   // 1 + 256
-__host__ __device__ constexpr int layer_in(int l) { return l == 0 ? kPE : kHidden; }
-__host__ __device__ constexpr int layer_out(int l) { return l == 3 ? kSkipOut : (l == 8 ? kOutDim : kHidden); }
-
-// Packed weight blob layout (built by recmv_sdf_pack_weights, sdf_mlp_simt.cu).
-//  * fp32 transposed copies [K][Npad32] + padded biases: the FP32_SIMT kernel
-//  * fp16 hi/lo "panels" for tcgen05: the K dimension of every layer is cut into 64-wide blocks; a panel
-//    is [512 n][64 k] fp16 (128-byte rows = one TMA/UMMA swizzle row).  Panels of all layers are
-//    stacked, plane hi first then plane lo, so ONE 2-D tensor map [2*66*512 rows, 64 cols] serves every
-//    weight tile.  Layer 4 has 9 panels: 8 for the 473(+39 zero) hidden inputs and 1 for the
-//    positional-encoding inputs of the skip connection (its 1/sqrt2 folded into the weights).
-constexpr int kNumPanels = 66;
 // Exact power-of-two operand scaling of the tensor-core path: activations are stored as fp16(hi)+fp16(lo) of
 // 2^6 * a, weights of 2^10 * w, so the `lo` residuals (~2^-12 of the value) stay in fp16's NORMAL range
 // (unscaled they are subnormal whenever |value| < 0.125 and carry only ~2^-20 relative precision);
@@ -301,21 +282,24 @@ constexpr int kNumPanels = 66;
 constexpr float kActScale = 64.f;
 constexpr float kWgtScale = 1024.f;
 constexpr float kAccUnscale = 1.f / (64.f * 1024.f);
-__host__ __device__ constexpr int panel_base(int l) {
-  return l == 0 ? 0 : (l <= 4 ? 1 + 8 * (l - 1) : 34 + 8 * (l - 5));
-}
-__host__ __device__ constexpr int num_panels(int l) { return l == 0 ? 1 : (l == 4 ? 9 : 8); }
 // softplus(beta=100) evaluated in base 2: u = 100 log2(e) z;  softplus = ln2/100 * log2(1 + 2^u)
 constexpr float kSoftplusLog2Scale = 144.26950408889634f;   // 100 * log2(e)
-struct PackedLayout {
-  size_t w32_off[kNumLayers];   // fp32 [K, Npad32] (transposed) for the SIMT kernel
-  size_t b32_off[kNumLayers];   // fp32 [512] bias padded with zeros
-  size_t bias_all_off;          // == b32_off[0]; the 9 padded biases are contiguous, stride 512 floats;
-                                // a second [9][512] plane holds b * kSoftplusLog2Scale
-  size_t f16_off;               // fp16 panels: [2 planes][66 panels][512][64]
-  size_t total;
-};
-PackedLayout packed_layout();
+
+// Passes of a tensor-core precision mode: 3 (RECMV_MLP_TC_F16X3), 1 (RECMV_MLP_TC_F16X1); 0: not a tensor-core mode.
+inline int tc_passes(int mode) { return mode == RECMV_MLP_TC_F16X3 ? 3 : (mode == RECMV_MLP_TC_F16X1 ? 1 : 0); }
+
+// Opts kKernel in to `bytes` of dynamic shared memory, once per device (the attribute is per device).
+template <auto kKernel>
+int smem_opt_in(int bytes) {
+  static bool done[16] = {false};
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (done[dev & 15]) return 0;
+  cudaError_t e = cudaFuncSetAttribute(kKernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+  if (e != cudaSuccess) return (int)e;
+  done[dev & 15] = true;
+  return 0;
+}
 
 // positional encoding of one point: pe[0..2] = x, then per band k: w*sin(2^k x) (3), w*cos(2^k x) (3)
 // (model/Embedder.py:33-37 order), accurate sincosf (fast intrinsics lose >1e-4 at 32x).

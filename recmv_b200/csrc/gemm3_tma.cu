@@ -550,14 +550,9 @@ __global__ void __launch_bounds__(256) pe_forward_planes_kernel(const float* __r
 
 int make_plane_tmap(CUtensorMap* out, const void* base, uint64_t cols, uint64_t rows, uint64_t row_pitch_elems,
                     uint32_t box_rows = 128) {
-  static EncodeTiledFn fn = nullptr;
-  if (!fn) {
-    cudaDriverEntryPointQueryResult q;
-    void* p = nullptr;
-    cudaError_t e = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q);
-    if (e != cudaSuccess || !p) return e != cudaSuccess ? (int)e : (int)cudaErrorNotSupported;
-    fn = (EncodeTiledFn)p;
-  }
+  EncodeTiledFn fn = nullptr;
+  int s = tensor_map_encoder(&fn);
+  if (s) return s;
   if (((uintptr_t)base & 15) != 0 || (row_pitch_elems & 7) != 0) return RECMV_E_SHAPE;
   cuuint64_t dims[2] = {cols, rows};
   cuuint64_t strides[1] = {row_pitch_elems * 2};
@@ -623,8 +618,7 @@ extern "C" int recmv_pe_forward(const float* x, const float* pe_w, int bands, fl
   if (P < 0 || bands < 0 || bands > 6) return RECMV_E_SHAPE;
   if (P == 0) return RECMV_OK;
   if (!x || !pe_w || !out) return RECMV_E_NULL;
-  PeWeights pw;
-  for (int i = 0; i < 12; ++i) pw.w[i] = i < 2 * bands ? pe_w[i] : 0.f;
+  const PeWeights pw = pe_weights(pe_w, bands);
   pe_forward_kernel<<<(unsigned)((P + 255) / 256), 256, 0, (cudaStream_t)stream>>>(x, pw, bands, out, ld, out2, ld2, P);
   return launch_status();
 }
@@ -635,8 +629,7 @@ extern "C" int recmv_pe_backward(const float* x, const float* g, int64_t ldg, co
   if (P < 0 || bands < 0 || bands > 6) return RECMV_E_SHAPE;
   if (P == 0) return RECMV_OK;
   if (!x || !g || !pe_w || !dx) return RECMV_E_NULL;
-  PeWeights pw;
-  for (int i = 0; i < 12; ++i) pw.w[i] = i < 2 * bands ? pe_w[i] : 0.f;
+  const PeWeights pw = pe_weights(pe_w, bands);
   const long long n = 3 * P;
   pe_backward_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(x, g, ldg, g2, ldg2, pw, bands, dx, P,
                                                                                    accumulate);
@@ -648,8 +641,7 @@ extern "C" int recmv_pe_forward_planes(const float* x, const float* pe_w, int ba
   if (P < 0 || bands < 0 || bands > 6) return RECMV_E_SHAPE;
   if (P == 0) return RECMV_OK;
   if (!x || !pe_w || !out_hi || !out_lo) return RECMV_E_NULL;
-  PeWeights pw;
-  for (int i = 0; i < 12; ++i) pw.w[i] = i < 2 * bands ? pe_w[i] : 0.f;
+  const PeWeights pw = pe_weights(pe_w, bands);
   pe_forward_planes_kernel<<<(unsigned)((P * 40 + 255) / 256), 256, 0, (cudaStream_t)stream>>>(x, pw, bands, out, ld, (__half*)out_hi,
                                                                                           (__half*)out_lo, ldp, P);
   return launch_status();
@@ -678,15 +670,8 @@ extern "C" int recmv_mlp_layer_planes(const void* a_hi, const void* a_lo, int64_
   if (!s) s = make_plane_tmap(&ta_l, a_lo, (uint64_t)K, (uint64_t)M, (uint64_t)lda_p);
   if (!s) s = make_plane_tmap(&tb_h, b_hi, (uint64_t)K, (uint64_t)N, (uint64_t)ldb_p);
   if (!s) s = make_plane_tmap(&tb_l, b_lo, (uint64_t)K, (uint64_t)N, (uint64_t)ldb_p);
+  if (!s) s = smem_opt_in<gemm3_tma_kernel>((int)kSmemBytes);
   if (s) return s;
-  static bool done[16] = {false};
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (!done[dev & 15]) {
-    cudaError_t e = cudaFuncSetAttribute(gemm3_tma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
-    if (e != cudaSuccess) return (int)e;
-    done[dev & 15] = true;
-  }
   void* sd = nullptr;
   int s0 = device_status_record(&sd);
   if (s0) return s0;
@@ -744,15 +729,8 @@ extern "C" int recmv_mlp_wgrad_planes(const void* g_hi, const void* g_lo, int64_
   if (s) return s;
   void* sd = nullptr;
   s = device_status_record(&sd);
+  if (!s) s = smem_opt_in<gemm3_wgrad_kernel>((int)kSmemBytesWg);
   if (s) return s;
-  static bool attr_done[16] = {};
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (!attr_done[dev & 15]) {
-    cudaError_t e = cudaFuncSetAttribute(gemm3_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytesWg);
-    if (e != cudaSuccess) return (int)e;
-    attr_done[dev & 15] = true;
-  }
   WgParams prm = {};
   prm.ws = workspace;
   prm.nkb = (P + kBK - 1) / kBK;

@@ -1,5 +1,5 @@
-// Weight packing + the exact-fp32 (CUDA-core) implementation of the fused SDF path, the per-ray
-// first-hit scan, and the C-ABI entry points that dispatch between the SIMT and tensor-core kernels.
+// The exact-fp32 (CUDA-core) implementation of the fused SDF path, the per-ray first-hit scan, and the C-ABI entry
+// points that dispatch between the SIMT and tensor-core kernels.
 //
 // Fused per tile of 32 points: [ray -> x_obs -> skinning-voxel sample -> inverse LBS ->] positional
 // encoding -> 9 linears with softplus(100) -> sdf (+256 features).  Activations live in shared
@@ -12,64 +12,7 @@
 
 namespace recmv {
 
-// ---------------------------------------------------------------------------------------------
-// packed blob
-// ---------------------------------------------------------------------------------------------
-constexpr int kNpad32(int l) { return l == 8 ? 264 : 512; }
-constexpr int kKfull(int l) { return l == 0 ? kPE : 512; }
-
-PackedLayout packed_layout() {
-  PackedLayout L;
-  size_t off = 0;
-  auto take = [&](size_t bytes) { size_t o = off; off += (bytes + 1023) & ~(size_t)1023; return o; };
-  L.bias_all_off = take((size_t)2 * kNumLayers * 512 * 4);   // plane 0: b; plane 1: b * 100 log2(e) (tcgen05 epilogue)
-  for (int l = 0; l < kNumLayers; ++l) L.b32_off[l] = L.bias_all_off + (size_t)l * 512 * 4;
-  for (int l = 0; l < kNumLayers; ++l) L.w32_off[l] = take((size_t)kKfull(l) * kNpad32(l) * 4);
-  L.f16_off = take((size_t)2 * kNumPanels * 512 * 64 * 2);
-  L.total = off;
-  return L;
-}
-
-// fp32 transposed copy + padded bias + fp16 hi/lo panels of one layer
-__global__ void __launch_bounds__(256) pack_layer_kernel(const float* __restrict__ W /*[out,in]*/,
-                                                         const float* __restrict__ b, int l, int out,
-                                                         int in, float* __restrict__ w32t, int npad32,
-                                                         float* __restrict__ bpad,
-                                                         __half* __restrict__ planes, int* __restrict__ status /*DevStatus*/) {
-  const float scale = (l == 4) ? 0.70710678118654752440f : 1.f;  // cat([x, pe]) / sqrt(2) folded in
-  const int np = num_panels(l);
-  int64_t total = (int64_t)np * 512 * 64;
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total;
-       i += (int64_t)gridDim.x * blockDim.x) {
-    int pi = (int)(i / (512 * 64));
-    int n = (int)((i / 64) % 512), kk = (int)(i % 64);
-    int src_k;
-    if (l == 0) src_k = kk < kPE ? kk : -1;
-    else if (l == 4) src_k = pi < 8 ? (pi * 64 + kk < kSkipOut ? pi * 64 + kk : -1) : (kk < kPE ? kSkipOut + kk : -1);
-    else src_k = pi * 64 + kk;
-    float v = (n < out && src_k >= 0) ? W[(size_t)n * in + src_k] * scale : 0.f;
-    float vs = v * kWgtScale;
-    if (!(fabsf(vs) < 65504.f)) {   // |w| >= 63.97: outside the tensor-core operand range -> status code 2 (tc_common.cuh)
-      volatile int* st = status;
-      if (st[0] == 0) { st[1] = 1201; st[2] = blockIdx.x; __threadfence_system(); st[0] = 2; }
-      vs = fminf(fmaxf(vs, -65504.f), 65504.f);
-    }
-    __half h = __float2half_rn(vs);
-    size_t o = ((size_t)(panel_base(l) + pi) * 512 + n) * 64 + kk;
-    planes[o] = h;
-    planes[(size_t)kNumPanels * 512 * 64 + o] = __float2half_rn(vs - __half2float(h));
-  }
-  int64_t total32 = (int64_t)in * npad32;
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total32;
-       i += (int64_t)gridDim.x * blockDim.x) {
-    int k = (int)(i / npad32), n = (int)(i - (int64_t)k * npad32);
-    w32t[i] = n < out ? W[(size_t)n * in + k] * scale : 0.f;
-  }
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < 512; i += gridDim.x * blockDim.x) {
-    bpad[i] = i < out ? b[i] : 0.f;
-    bpad[kNumLayers * 512 + i] = i < out ? b[i] * kSoftplusLog2Scale : 0.f;
-  }
-}
+using Sdf = Net<0>;
 
 // ---------------------------------------------------------------------------------------------
 // SIMT fused forward
@@ -80,8 +23,8 @@ constexpr int kLd = 516;  // activation row stride in floats (516 % 32 = 4: the 
                           // float4 read hit different banks)
 
 struct SimtWeights {
-  const float* w[kNumLayers];
-  const float* b[kNumLayers];
+  const float* w[Sdf::kLayers];
+  const float* b[Sdf::kLayers];
 };
 
 // out[m][n] = sum_k in[m][k] * Wt[k][n] + b[n]   for m in [ty*8, ty*8+8), n in [tx*8, tx*8+8)
@@ -176,19 +119,19 @@ __global__ void __launch_bounds__(kSimtThreads, 1) sdf_simt_kernel(PointSource s
     // layer 0: K = 39 straight from the pe buffer (row stride 40) -> copy into bufA rows first
     for (int q = threadIdx.x; q < kTileM * 40; q += kSimtThreads) bufA[(q / 40) * kLd + (q % 40)] = pe[q];
     __syncthreads();
-    simt_layer<true>(bufA, bufB, wts.w[0], wts.b[0], kPE, 512, 512, tx, ty); __syncthreads();
+    simt_layer<true>(bufA, bufB, wts.w[0], wts.b[0], Sdf::kPE, 512, 512, tx, ty); __syncthreads();
     simt_layer<true>(bufB, bufA, wts.w[1], wts.b[1], 512, 512, 512, tx, ty); __syncthreads();
     simt_layer<true>(bufA, bufB, wts.w[2], wts.b[2], 512, 512, 512, tx, ty); __syncthreads();
-    simt_layer<true>(bufB, bufA, wts.w[3], wts.b[3], 512, 512, kSkipOut, tx, ty); __syncthreads();
+    simt_layer<true>(bufB, bufA, wts.w[3], wts.b[3], 512, 512, Sdf::kSkipOut, tx, ty); __syncthreads();
     // skip: columns 473..511 of the layer-4 input are the positional encoding (1/sqrt2 is in W4)
-    for (int q = threadIdx.x; q < kTileM * kPE; q += kSimtThreads)
-      bufA[(q / kPE) * kLd + kSkipOut + (q % kPE)] = pe[(q / kPE) * 40 + (q % kPE)];
+    for (int q = threadIdx.x; q < kTileM * Sdf::kPE; q += kSimtThreads)
+      bufA[(q / Sdf::kPE) * kLd + Sdf::kSkipOut + (q % Sdf::kPE)] = pe[(q / Sdf::kPE) * 40 + (q % Sdf::kPE)];
     __syncthreads();
     simt_layer<true>(bufA, bufB, wts.w[4], wts.b[4], 512, 512, 512, tx, ty); __syncthreads();
     simt_layer<true>(bufB, bufA, wts.w[5], wts.b[5], 512, 512, 512, tx, ty); __syncthreads();
     simt_layer<true>(bufA, bufB, wts.w[6], wts.b[6], 512, 512, 512, tx, ty); __syncthreads();
     simt_layer<true>(bufB, bufA, wts.w[7], wts.b[7], 512, 512, 512, tx, ty); __syncthreads();
-    simt_layer<false>(bufA, bufB, wts.w[8], wts.b[8], 512, 264, kOutDim, tx, ty); __syncthreads();
+    simt_layer<false>(bufA, bufB, wts.w[8], wts.b[8], 512, 264, Sdf::kOutDim, tx, ty); __syncthreads();
     if (threadIdx.x < kTileM && p0 + threadIdx.x < P)
       out_sdf[p0 + threadIdx.x] = s_valid[threadIdx.x] ? bufB[threadIdx.x * kLd] : kInvalidSdf;
     if (out_feat) {
@@ -203,21 +146,15 @@ __global__ void __launch_bounds__(kSimtThreads, 1) sdf_simt_kernel(PointSource s
 
 int simt_sdf_forward(const PointSource& src, const void* packed, const PeWeights& pw, float* out_sdf,
                      float* out_feat, int64_t P, cudaStream_t st) {
-  PackedLayout L = packed_layout();
+  const PackedBlob blob = carve(const_cast<void*>(packed), blob_layout<0>);
   SimtWeights w;
-  for (int l = 0; l < kNumLayers; ++l) {
-    w.w[l] = (const float*)((const char*)packed + L.w32_off[l]);
-    w.b[l] = (const float*)((const char*)packed + L.b32_off[l]);
+  for (int l = 0; l < Sdf::kLayers; ++l) {
+    w.w[l] = blob.w32[l];
+    w.b[l] = blob.bias + l * 512;
   }
   size_t smem = (size_t)(2 * kTileM * kLd + kTileM * 40) * sizeof(float);
-  static bool attr_done[16] = {false};   // the opt-in is per device
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (!attr_done[dev & 15]) {
-    cudaError_t e = cudaFuncSetAttribute(sdf_simt_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return (int)e;
-    attr_done[dev & 15] = true;
-  }
+  int s = smem_opt_in<sdf_simt_kernel>((int)smem);
+  if (s) return s;
   int64_t tiles = (P + kTileM - 1) / kTileM;
   int grid = (int)(tiles < num_sms() ? tiles : num_sms());
   sdf_simt_kernel<<<grid, kSimtThreads, smem, st>>>(src, w, pw, out_sdf, out_feat, P);
@@ -261,42 +198,13 @@ __global__ void __launch_bounds__(256) first_hit_kernel(const float* __restrict_
 
 using namespace recmv;
 
-extern "C" size_t recmv_sdf_packed_bytes(void) { return packed_layout().total; }
-
-extern "C" int recmv_sdf_pack_weights(const float* W_all, const float* b_all, void* packed,
-                                      recmv_stream_t stream) {
-  if (!W_all || !b_all || !packed) return RECMV_E_NULL;
-  if (((uintptr_t)packed & 1023) != 0) return RECMV_E_SHAPE;
-  PackedLayout L = packed_layout();
-  cudaStream_t st = (cudaStream_t)stream;
-  size_t woff = 0, boff = 0;
-  void* sd = nullptr;
-  int s0 = device_status_record(&sd);
-  if (s0) return s0;
-  for (int l = 0; l < kNumLayers; ++l) {
-    int in = layer_in(l), out = layer_out(l);
-    char* base = (char*)packed;
-    pack_layer_kernel<<<stride_grid((int64_t)num_panels(l) * 512 * 64, 256, 4), 256, 0, st>>>(
-        W_all + woff, b_all + boff, l, out, in, (float*)(base + L.w32_off[l]), kNpad32(l),
-        (float*)(base + L.b32_off[l]), (__half*)(base + L.f16_off), (int*)sd);
-    int s = launch_status();
-    if (s) return s;
-    woff += (size_t)in * out;
-    boff += out;
-  }
-  return RECMV_OK;
-}
-
 static int run_forward(const PointSource& src, const void* packed, const float* pe_w, float* out_sdf,
                        float* out_feat, int64_t P, int mode, cudaStream_t st) {
-  PeWeights pw;
-  for (int i = 0; i < 12; ++i) pw.w[i] = pe_w[i];
-  switch (mode) {
-    case RECMV_MLP_FP32_SIMT: return simt_sdf_forward(src, packed, pw, out_sdf, out_feat, P, st);
-    case RECMV_MLP_TC_F16X3: return tc_sdf_forward(src, packed, pw, out_sdf, out_feat, P, 3, st);
-    case RECMV_MLP_TC_F16X1: return tc_sdf_forward(src, packed, pw, out_sdf, out_feat, P, 1, st);
-    default: return RECMV_E_DTYPE;
-  }
+  const PeWeights pw = pe_weights(pe_w);
+  if (mode == RECMV_MLP_FP32_SIMT) return simt_sdf_forward(src, packed, pw, out_sdf, out_feat, P, st);
+  const int passes = tc_passes(mode);
+  if (!passes) return RECMV_E_DTYPE;
+  return tc_sdf_forward(src, packed, pw, out_sdf, out_feat, P, passes, st);
 }
 
 extern "C" int recmv_sdf_mlp_fwd(const float* x, const void* packed, const float* pe_w, float* out_sdf,
@@ -318,14 +226,13 @@ extern "C" int recmv_sdf_mlp_fwd_counted(const float* x, const void* packed, con
   if (capacity < 0) return RECMV_E_SHAPE;
   if (capacity == 0) return RECMV_OK;
   if (!x || !packed || !pe_w || !out_sdf || !count_dev) return RECMV_E_NULL;
-  if (mode != RECMV_MLP_TC_F16X3 && mode != RECMV_MLP_TC_F16X1) return RECMV_E_UNSUPPORTED;
+  const int passes = tc_passes(mode);
+  if (!passes) return RECMV_E_UNSUPPORTED;
   PointSource src = {};
   src.x = x;
   src.S = 1;
-  PeWeights pw;
-  for (int i = 0; i < 12; ++i) pw.w[i] = pe_w[i];
-  return tc_sdf_forward(src, packed, pw, out_sdf, out_feat, capacity, mode == RECMV_MLP_TC_F16X3 ? 3 : 1,
-                        (cudaStream_t)stream, count_dev);
+  return tc_sdf_forward(src, packed, pe_weights(pe_w), out_sdf, out_feat, capacity, passes, (cudaStream_t)stream,
+                        count_dev);
 }
 
 extern "C" int recmv_sdf_mlp_fwd_grad(const float* x, const void* packed, const float* pe_w, float* out_sdf,
@@ -334,11 +241,9 @@ extern "C" int recmv_sdf_mlp_fwd_grad(const float* x, const void* packed, const 
   if (P < 0) return RECMV_E_SHAPE;
   if (P == 0) return RECMV_OK;
   if (!x || !packed || !pe_w || !out_sdf || !out_grad) return RECMV_E_NULL;
-  if (mode != RECMV_MLP_TC_F16X3 && mode != RECMV_MLP_TC_F16X1) return RECMV_E_UNSUPPORTED;
-  PeWeights pw;
-  for (int i = 0; i < 12; ++i) pw.w[i] = pe_w[i];
-  return tc_sdf_forward_grad(x, packed, pw, out_sdf, out_feat, out_grad, P, mode == RECMV_MLP_TC_F16X3 ? 3 : 1,
-                             (cudaStream_t)stream);
+  const int passes = tc_passes(mode);
+  if (!passes) return RECMV_E_UNSUPPORTED;
+  return tc_sdf_forward_grad(x, packed, pe_weights(pe_w), out_sdf, out_feat, out_grad, P, passes, (cudaStream_t)stream);
 }
 
 extern "C" int recmv_ray_first_hit(const float* sdf, const recmv_raymarch_t* rm, int32_t* hit_idx,

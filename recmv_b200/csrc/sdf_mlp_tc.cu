@@ -167,36 +167,6 @@ __device__ __forceinline__ void positional_encode_tangent(float cx, float cy, fl
   }
 }
 
-// Network descriptions driving the same pipeline.  ntiles(l, last): 128-wide output tiles of layer l (warpgroup g owns
-// tiles 2 g and 2 g + 1; `last` = TcParams::last_tiles); kb_at(l, i): the i-th K block (64 inputs) of layer l's input,
-// 8 = the positional-encoding block.
-template <int kNet> struct Net;
-// SDF network (model/network.py:135-141): PE block -> 512 x3 -> 473 -> [skip: +PE block] 512 x4 -> 257
-template <> struct Net<0> {
-  static constexpr int kLayers = 9, kPanels = kNumPanels, kInFreeLayer = 4;
-  __device__ static int nkb(int l) { return num_panels(l); }
-  __device__ static int pbase(int l) { return panel_base(l); }
-  __device__ static int kb_at(int l, int i) { return l == 0 ? 8 : (l == 4 ? (i == 0 ? 8 : i - 1) : i); }
-  __device__ static int ntiles(int l, int last) { return l == 8 ? last : 4; }
-};
-// MLPTranslator (model/Deformer.py:141-206): [PE(39) | cond(128) | 0 x25] = 3 K blocks -> 512 x4 (ReLU) -> 3
-template <> struct Net<1> {
-  static constexpr int kLayers = 5, kPanels = 35, kInFreeLayer = 4;
-  __device__ static int nkb(int l) { return l == 0 ? 3 : 8; }
-  __device__ static int pbase(int l) { return l == 0 ? 0 : 3 + 8 * (l - 1); }
-  __device__ static int kb_at(int, int i) { return i; }   // the input block lives in the activation buffer
-  __device__ static int ntiles(int l, int) { return l == 4 ? 1 : 4; }
-};
-// RenderingNetwork_view_norm, mode 'idr' (model/RenderNet.py:59-96): [p 3 | PE4(v) 27 | n 3 | feat 256 | 0 x31] = 5 K
-// blocks -> 512 x4 (ReLU) -> 3 -> tanh
-template <> struct Net<2> {
-  static constexpr int kLayers = 5, kPanels = 37, kInFreeLayer = 4;
-  __device__ static int nkb(int l) { return l == 0 ? 5 : 8; }
-  __device__ static int pbase(int l) { return l == 0 ? 0 : 5 + 8 * (l - 1); }
-  __device__ static int kb_at(int, int i) { return i; }
-  __device__ static int ntiles(int l, int) { return l == 4 ? 1 : 4; }
-};
-
 // The MMAs of one weight box (one 64-wide K block x one 128-wide output tile x one weight plane) into accumulator `acc`.
 // The box arrives as two ring slots, b0 = inputs 0..31 and b1 = inputs 32..63 (K steps 0, 1 and 2, 3), and its MMAs
 // form two commit groups: the first is the last to read b0, the second reads b1 only, so b0 is released one group
@@ -242,7 +212,7 @@ template <bool kJvp, int kNet, int kPasses>
 __global__ void __launch_bounds__(kThreads, 1)
 sdf_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams prm) {
   using NetT = Net<kNet>;
-  constexpr int kNumLayers = NetT::kLayers;   // shadows the SDF constant of common.cuh
+  constexpr int kNumLayers = NetT::kLayers;
   static_assert(!kJvp || kNet == 0 || kNet == 1, "the forward-mode variant exists for the SDF network and the deformer");
   static_assert(kPasses == 1 || kPasses == 3, "precision mode");
   extern __shared__ uint8_t smem_raw[];
@@ -746,24 +716,12 @@ sdf_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams prm) {
 }
 
 namespace {
+// one mapped, pinned status record per device
 DevStatus* g_status_host[16] = {nullptr};
 // relative compensation of the accumulation bias per 64-wide K block (= 4 accumulating hi*hi MMAs x 2^-24), per
 // precision mode {3 passes, 1 pass}; calibrated against the reference's fp32 results (tools/calibrate_acc_gain.py)
 float g_acc_gain_kb[2] = {4.f * 5.9604645e-8f, 4.f * 5.9604645e-8f};
-inline void set_acc_scales(TcParams& prm) { prm.acc_gain_kb = g_acc_gain_kb[prm.passes == 3 ? 0 : 1]; }
 
-// one mapped, pinned status record per device
-int tc_status_record(int dev, DevStatus** out);
-}  // namespace
-int device_status_record(void** out) {
-  int dev = 0;
-  cudaGetDevice(&dev);
-  DevStatus* sd = nullptr;
-  int s = tc_status_record(dev, &sd);
-  *out = sd;
-  return s;
-}
-namespace {
 int tc_status_record(int dev, DevStatus** out) {
   DevStatus*& h = g_status_host[dev & 15];
   if (!h) {
@@ -774,184 +732,189 @@ int tc_status_record(int dev, DevStatus** out) {
   *out = h;
   return 0;
 }
-
-struct TmapCacheEntry {
-  const void* base = nullptr;
-  CUtensorMap m128;
-};
-using TmapCache = TmapCacheEntry;
-
-// the dynamic shared memory opt-in of both precision modes of one network variant
-template <bool kJvp, int kNet> cudaError_t tc_allow_smem() {
-  cudaError_t e = cudaFuncSetAttribute(sdf_tc_kernel<kJvp, kNet, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(sdf_tc_kernel<kJvp, kNet, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
-  return e;
-}
-
-// opt-in to the 226 KB of dynamic shared memory once per device for every instantiation
-int tc_prepare_launch(int dev) {
-  static bool done[16] = {false};
-  if (done[dev & 15]) return 0;
-  cudaError_t e = tc_allow_smem<false, 0>();
-  if (e == cudaSuccess) e = tc_allow_smem<true, 0>();
-  if (e == cudaSuccess) e = tc_allow_smem<false, 1>();
-  if (e == cudaSuccess) e = tc_allow_smem<true, 1>();
-  if (e == cudaSuccess) e = tc_allow_smem<false, 2>();
-  if (e != cudaSuccess) return (int)e;
-  done[dev & 15] = true;
-  return 0;
-}
-
-// launches the instantiation of prm.passes (1 or 3, checked by the callers)
-template <bool kJvp, int kNet>
-void tc_launch(int grid, cudaStream_t st, const CUtensorMap& tmap, const TcParams& prm) {
-  if (prm.passes == 3)
-    sdf_tc_kernel<kJvp, kNet, 3><<<grid, kThreads, kSmemBytes, st>>>(tmap, prm);
-  else
-    sdf_tc_kernel<kJvp, kNet, 1><<<grid, kThreads, kSmemBytes, st>>>(tmap, prm);
-}
-
 }  // namespace
 
-// persistent kernel: one CTA per SM (at most one per tile)
-static int tc_grid(int64_t P, int pts_per_tile) {
-  const int64_t tiles = (P + pts_per_tile - 1) / pts_per_tile;
-  return (int)(tiles < num_sms() ? tiles : num_sms());
-}
-
-static int launch_tc(const PointSource& src, const void* packed, const PeWeights& pw, float* out_sdf,
-                     float* out_feat, float* out_grad, int64_t P, int passes, int dbg_layer, float* dbg_out, int* status_host,
-                     cudaStream_t st, const int* P_dev = nullptr) {
-  if (passes != 1 && passes != 3) return RECMV_E_DTYPE;
-  PackedLayout L = packed_layout();
-  const char* pb = (const char*)packed;
-  static TmapCache cache[16];
+int device_status_record(void** out) {
   int dev = 0;
   cudaGetDevice(&dev);
-  TmapCache& tc_ = cache[dev & 15];
-  const void* panels = pb + L.f16_off;
-  if (tc_.base != panels) {
-    int s = make_panel_tmap(&tc_.m128, panels, (uint64_t)2 * kNumPanels * 512, 128);
-    if (s) return s;
-    tc_.base = panels;
-  }
-  int sp = tc_prepare_launch(dev);
-  if (sp) return sp;
-  // Device status record in MAPPED pinned host memory: a bounded wait that times out writes it there, the
-  // host sees it without a synchronisation and refuses further work (recmv_check_async_errors()).
   DevStatus* sd = nullptr;
-  int s0 = tc_status_record(dev, &sd);
-  if (s0) return s0;
-  if (sd->code != 0) return RECMV_E_DEVICE;  // a previous launch on this device aborted
-  TcParams prm = {};
-  prm.src = src; prm.pw = pw;
-  prm.bias = (const float*)(pb + L.bias_all_off);
-  prm.out_sdf = out_sdf; prm.out_feat = out_feat; prm.P = P; prm.P_dev = P_dev; prm.passes = passes; prm.status = sd;
-  set_acc_scales(prm);
-  prm.dbg_layer = dbg_layer; prm.dbg_out = dbg_out; prm.out_grad = out_grad;
-  // the last layer's output tiles 1 and 2 hold features only: computed when someone reads them
-  prm.last_tiles = (out_feat || (dbg_out && dbg_layer == kNumLayers - 1)) ? 3 : 1;
-  const int grid = tc_grid(P, out_grad ? kRowsPerCta / 4 : kRowsPerCta);
-  if (out_grad)
-    tc_launch<true, 0>(grid, st, tc_.m128, prm);
-  else
-    tc_launch<false, 0>(grid, st, tc_.m128, prm);
-  int s = launch_status();
+  int s = tc_status_record(dev, &sd);
+  *out = sd;
+  return s;
+}
+
+namespace {
+// Packs layer l of network kNet into its blob: the fp16 hi / lo panels of 1024 w (zero padding; a weight beyond fp16's
+// range is reported -- tag 1201 SDF, 1200 translator / colour -- and saturated), the zero-padded bias and, for the SDF,
+// the fp32 transposed copy and the bias plane b * kSoftplusLog2Scale.
+template <int kNet>
+__global__ void __launch_bounds__(256) pack_layer_kernel(const float* __restrict__ W /*[out,in]*/, const float* __restrict__ b,
+                                                         int l, PackedBlob blob, DevStatus* status) {
+  using N = Net<kNet>;
+  const int out = N::out(l), in = N::in(l);
+  const float scale = N::wscale(l);
+  const int64_t total = (int64_t)N::nkb(l) * 512 * 64;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int pi = (int)(i / (512 * 64)), n = (int)((i / 64) % 512), kk = (int)(i % 64);
+    const int k = N::src_col(l, pi, kk);
+    float v = (n < out && k >= 0) ? W[(size_t)n * in + k] * scale * kWgtScale : 0.f;
+    if (!(fabsf(v) < 65504.f)) {   // |w| >= 63.97: outside the tensor-core operand range
+      report_range(status, kNet == 0 ? 1201 : 1200);
+      v = fminf(fmaxf(v, -65504.f), 65504.f);
+    }
+    const __half h = __float2half_rn(v);
+    const size_t o = ((size_t)(N::pbase(l) + pi) * 512 + n) * 64 + kk;
+    blob.panels[o] = h;
+    blob.panels[(size_t)N::kPanels * 512 * 64 + o] = __float2half_rn(v - __half2float(h));
+  }
+  if constexpr (kNet == 0) {
+    const int npad = N::npad32(l);
+    const int64_t total32 = (int64_t)in * npad;
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total32; i += (int64_t)gridDim.x * blockDim.x) {
+      const int k = (int)(i / npad), n = (int)(i - (int64_t)k * npad);
+      blob.w32[l][i] = n < out ? W[(size_t)n * in + k] * scale : 0.f;
+    }
+  }
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < 512; i += gridDim.x * blockDim.x) {
+    blob.bias[l * 512 + i] = i < out ? b[i] : 0.f;
+    if (kNet == 0) blob.bias[(N::kLayers + l) * 512 + i] = i < out ? b[i] * kSoftplusLog2Scale : 0.f;
+  }
+}
+
+// W_all / b_all: every layer's [out, in] weights / [out] bias, concatenated; one launch per layer
+template <int kNet>
+int pack_weights(const float* W_all, const float* b_all, void* packed, recmv_stream_t stream) {
+  if (!W_all || !b_all || !packed) return RECMV_E_NULL;
+  if (((uintptr_t)packed & 1023) != 0) return RECMV_E_SHAPE;
+  void* sd = nullptr;
+  int s = device_status_record(&sd);
   if (s) return s;
-  if (status_host) {  // diagnostics path: wait for the launch, then report (and clear) the status record
-    cudaError_t e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) return (int)e;
-    status_host[0] = sd->code; status_host[1] = sd->detail; status_host[2] = sd->block; status_host[3] = 0;
-    sd->code = 0; sd->detail = 0; sd->block = 0;
+  using N = Net<kNet>;
+  const PackedBlob blob = carve(packed, blob_layout<kNet>);
+  for (int l = 0; l < N::kLayers; ++l) {
+    pack_layer_kernel<kNet><<<stride_grid((int64_t)N::nkb(l) * 512 * 64, 256, 4), 256, 0, (cudaStream_t)stream>>>(
+        W_all, b_all, l, blob, (DevStatus*)sd);
+    s = launch_status();
+    if (s) return s;
+    W_all += (size_t)N::in(l) * N::out(l);
+    b_all += N::out(l);
   }
   return RECMV_OK;
 }
 
+// per device and network: the tensor map of the panels it was last launched with
+struct TmapCacheEntry {
+  const void* base = nullptr;
+  CUtensorMap map;
+};
+TmapCacheEntry g_tmap[16][3];
+
+// Launches network kNet (kJvp: its forward-mode variant) on P points with the weights of blob `packed`; prm holds the
+// network's own fields.  status_host != nullptr (diagnostics): waits for the launch, then reports and clears the
+// device status record.
+template <bool kJvp, int kNet>
+int tc_launch(const void* packed, TcParams prm, int passes, int64_t P, cudaStream_t st, int* status_host = nullptr) {
+  int dev = 0;
+  cudaGetDevice(&dev);
+  const PackedBlob blob = carve(const_cast<void*>(packed), blob_layout<kNet>);
+  TmapCacheEntry& tm = g_tmap[dev & 15][kNet];
+  if (tm.base != blob.panels) {
+    int s = make_panel_tmap(&tm.map, blob.panels, (uint64_t)2 * Net<kNet>::kPanels * 512, 128);
+    if (s) return s;
+    tm.base = blob.panels;
+  }
+  int s = passes == 3 ? smem_opt_in<sdf_tc_kernel<kJvp, kNet, 3>>((int)kSmemBytes)
+                      : smem_opt_in<sdf_tc_kernel<kJvp, kNet, 1>>((int)kSmemBytes);
+  if (s) return s;
+  // Device status record in MAPPED pinned host memory: a bounded wait that times out writes it there, the
+  // host sees it without a synchronisation and refuses further work (recmv_check_async_errors()).
+  DevStatus* sd = nullptr;
+  s = tc_status_record(dev, &sd);
+  if (s) return s;
+  if (sd->code != 0) return RECMV_E_DEVICE;  // a previous launch on this device aborted
+  prm.bias = blob.bias;
+  prm.P = P;
+  prm.passes = passes;
+  prm.acc_gain_kb = g_acc_gain_kb[passes == 3 ? 0 : 1];
+  prm.status = sd;
+  // persistent kernel: one CTA per SM (at most one per tile); the forward-mode variant holds 4 rows per point
+  constexpr int kPtsPerTile = kJvp ? kRowsPerCta / 4 : kRowsPerCta;
+  const int64_t tiles = (P + kPtsPerTile - 1) / kPtsPerTile;
+  const int grid = (int)(tiles < num_sms() ? tiles : num_sms());
+  if (passes == 3)
+    sdf_tc_kernel<kJvp, kNet, 3><<<grid, kThreads, kSmemBytes, st>>>(tm.map, prm);
+  else
+    sdf_tc_kernel<kJvp, kNet, 1><<<grid, kThreads, kSmemBytes, st>>>(tm.map, prm);
+  s = launch_status();
+  if (s || !status_host) return s;
+  cudaError_t e = cudaStreamSynchronize(st);
+  if (e != cudaSuccess) return (int)e;
+  status_host[0] = sd->code; status_host[1] = sd->detail; status_host[2] = sd->block; status_host[3] = 0;
+  sd->code = 0; sd->detail = 0; sd->block = 0;
+  return RECMV_OK;
+}
+}  // namespace
+
+// SDF network.  The last layer's output tiles 1 and 2 hold features only: computed when someone reads them.
 int tc_sdf_forward(const PointSource& src, const void* packed, const PeWeights& pw, float* out_sdf,
                    float* out_feat, int64_t P, int passes, cudaStream_t st, const int* P_dev) {
-  return launch_tc(src, packed, pw, out_sdf, out_feat, nullptr, P, passes, -1, nullptr, nullptr, st, P_dev);
+  TcParams prm = {};
+  prm.src = src; prm.pw = pw; prm.out_sdf = out_sdf; prm.out_feat = out_feat; prm.P_dev = P_dev; prm.dbg_layer = -1;
+  prm.last_tiles = out_feat ? 3 : 1;
+  return tc_launch<false, 0>(packed, prm, passes, P, st);
 }
 
 int tc_sdf_forward_grad(const float* x, const void* packed, const PeWeights& pw, float* out_sdf, float* out_feat,
                         float* out_grad, int64_t P, int passes, cudaStream_t st) {
-  PointSource src = {};
-  src.x = x;
-  src.S = 1;
-  return launch_tc(src, packed, pw, out_sdf, out_feat, out_grad, P, passes, -1, nullptr, nullptr, st);
+  TcParams prm = {};
+  prm.src.x = x; prm.src.S = 1; prm.pw = pw; prm.out_sdf = out_sdf; prm.out_feat = out_feat; prm.dbg_layer = -1;
+  prm.out_grad = out_grad;
+  prm.last_tiles = out_feat ? 3 : 1;
+  return tc_launch<true, 0>(packed, prm, passes, P, st);
 }
 
 }  // namespace recmv
 
 using namespace recmv;
 
+extern "C" size_t recmv_sdf_packed_bytes(void) { return layout_bytes(blob_layout<0>); }
+extern "C" size_t recmv_translator_packed_bytes(void) { return layout_bytes(blob_layout<1>); }
+extern "C" size_t recmv_rendernet_packed_bytes(void) { return layout_bytes(blob_layout<2>); }
+
+extern "C" int recmv_sdf_pack_weights(const float* W_all, const float* b_all, void* packed, recmv_stream_t stream) {
+  return pack_weights<0>(W_all, b_all, packed, stream);
+}
+extern "C" int recmv_translator_pack_weights(const float* W_all, const float* b_all, void* packed,
+                                             recmv_stream_t stream) {
+  return pack_weights<1>(W_all, b_all, packed, stream);
+}
+extern "C" int recmv_rendernet_pack_weights(const float* W_all, const float* b_all, void* packed,
+                                            recmv_stream_t stream) {
+  return pack_weights<2>(W_all, b_all, packed, stream);
+}
+
 // ---------------------------------------------------------------------------------------------------------
 // Deformer network: MLPTranslator (model/Deformer.py:141-206) + LBSkinner.forward (Deformer.py:406-445)
 // ---------------------------------------------------------------------------------------------------------
-namespace recmv {
-namespace {
-constexpr int kDefLayers = 5, kDefPanels = 35;
-constexpr int def_in(int l) { return l == 0 ? 167 : 512; }
-constexpr int def_out(int l) { return l == 4 ? 3 : 512; }
-constexpr int def_pbase(int l) { return l == 0 ? 0 : 3 + 8 * (l - 1); }
-constexpr int def_npanels(int l) { return l == 0 ? 3 : 8; }
-struct DeformLayout { size_t bias_off, f16_off, total; };
-DeformLayout deform_layout() {
-  DeformLayout L;
-  L.bias_off = 0;
-  L.f16_off = ((size_t)kDefLayers * 512 * 4 + 1023) & ~(size_t)1023;
-  L.total = L.f16_off + (size_t)2 * kDefPanels * 512 * 64 * 2;
-  return L;
-}
-
-__global__ void __launch_bounds__(256) pack_plain_layer_kernel(const float* __restrict__ W, const float* __restrict__ b,
-                                                               int out, int in, int pbase, int npanels,
-                                                               float* __restrict__ bpad, __half* __restrict__ planes,
-                                                               int total_panels, DevStatus* status) {
-  int64_t total = (int64_t)npanels * 512 * 64;
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
-    const int pi = (int)(i / (512 * 64)), n = (int)((i / 64) % 512), kk = (int)(i % 64);
-    const int k = pi * 64 + kk;
-    float v = (n < out && k < in) ? W[(size_t)n * in + k] * kWgtScale : 0.f;
-    if (!(fabsf(v) < 65504.f)) { report_range(status, 1200); v = fminf(fmaxf(v, -65504.f), 65504.f); }
-    const __half h = __float2half_rn(v);
-    const size_t o = ((size_t)(pbase + pi) * 512 + n) * 64 + kk;
-    planes[o] = h;
-    planes[(size_t)total_panels * 512 * 64 + o] = __float2half_rn(v - __half2float(h));
-  }
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < 512; i += gridDim.x * blockDim.x) bpad[i] = i < out ? b[i] : 0.f;
-}
-TmapCacheEntry g_def_tmap[16];
-}  // namespace
-}  // namespace recmv
-
-extern "C" size_t recmv_translator_packed_bytes(void) { return deform_layout().total; }
-
-extern "C" int recmv_translator_pack_weights(const float* W_all, const float* b_all, void* packed,
-                                             recmv_stream_t stream) {
-  if (!W_all || !b_all || !packed) return RECMV_E_NULL;
-  if (((uintptr_t)packed & 1023) != 0) return RECMV_E_SHAPE;
-  DeformLayout L = deform_layout();
-  char* base = (char*)packed;
-  size_t woff = 0, boff = 0;
-  void* sd = nullptr;
-  int s0 = device_status_record(&sd);
-  if (s0) return s0;
-  for (int l = 0; l < kDefLayers; ++l) {
-    pack_plain_layer_kernel<<<stride_grid((int64_t)def_npanels(l) * 512 * 64, 256, 4), 256, 0, (cudaStream_t)stream>>>(
-        W_all + woff, b_all + boff, def_out(l), def_in(l), def_pbase(l), def_npanels(l),
-        (float*)(base + L.bias_off) + l * 512, (__half*)(base + L.f16_off), kDefPanels, (DevStatus*)sd);
-    int s = launch_status();
-    if (s) return s;
-    woff += (size_t)def_in(l) * def_out(l);
-    boff += def_out(l);
-  }
-  return RECMV_OK;
-}
-
 static int deformer_launch(const float* ps, const float* conds, const int64_t* batch_inds, int64_t points_per_frame,
                            int num_frames, const void* packed, const float* pe_w, const float* A, const float* trans,
                            const recmv_voxel_t* vox, float* out_translated, float* out_offset, float* out_posed,
-                           float* out_jac, int64_t P, int mode, recmv_stream_t stream);
+                           float* out_jac, int64_t P, int mode, recmv_stream_t stream) {
+  if (P < 0 || num_frames <= 0) return RECMV_E_SHAPE;
+  if (P == 0) return RECMV_OK;
+  if (!ps || !conds || !packed || !pe_w) return RECMV_E_NULL;
+  if (out_posed && (!A || !trans || !vox || !vox->ws_cl)) return RECMV_E_NULL;
+  const int passes = tc_passes(mode);
+  if (!passes) return RECMV_E_UNSUPPORTED;
+  TcParams prm = {};
+  prm.src.x = ps; prm.src.S = 1; prm.pw = pe_weights(pe_w); prm.dbg_layer = -1;
+  prm.conds = conds; prm.batch_inds = (const long long*)batch_inds; prm.points_per_frame = points_per_frame;
+  prm.num_frames = num_frames; prm.bones = A; prm.trans = trans;
+  if (vox) prm.vox = to_voxel(vox);
+  prm.out_translated = out_translated; prm.out_offset = out_offset; prm.out_posed = out_posed; prm.out_jac = out_jac;
+  if (out_jac) return tc_launch<true, 1>(packed, prm, passes, P, (cudaStream_t)stream);
+  return tc_launch<false, 1>(packed, prm, passes, P, (cudaStream_t)stream);
+}
 
 extern "C" int recmv_deformer_fwd_jac(const float* ps, const float* conds, const int64_t* batch_inds,
                                       int64_t points_per_frame, int num_frames, const void* packed, const float* pe_w,
@@ -971,136 +934,30 @@ extern "C" int recmv_deformer_fwd(const float* ps, const float* conds, const int
                          out_offset, out_posed, nullptr, P, mode, stream);
 }
 
-static int deformer_launch(const float* ps, const float* conds, const int64_t* batch_inds, int64_t points_per_frame,
-                           int num_frames, const void* packed, const float* pe_w, const float* A, const float* trans,
-                           const recmv_voxel_t* vox, float* out_translated, float* out_offset, float* out_posed,
-                           float* out_jac, int64_t P, int mode, recmv_stream_t stream) {
-  if (P < 0 || num_frames <= 0) return RECMV_E_SHAPE;
-  if (P == 0) return RECMV_OK;
-  if (!ps || !conds || !packed || !pe_w) return RECMV_E_NULL;
-  if (out_posed && (!A || !trans || !vox || !vox->ws_cl)) return RECMV_E_NULL;
-  if (mode != RECMV_MLP_TC_F16X3 && mode != RECMV_MLP_TC_F16X1) return RECMV_E_UNSUPPORTED;
-  cudaStream_t st = (cudaStream_t)stream;
-  int dev = 0;
-  cudaGetDevice(&dev);
-  DeformLayout L = deform_layout();
-  const char* pb = (const char*)packed;
-  TmapCacheEntry& tc_ = g_def_tmap[dev & 15];
-  if (tc_.base != pb + L.f16_off) {
-    int s = make_panel_tmap(&tc_.m128, pb + L.f16_off, (uint64_t)2 * kDefPanels * 512, 128);
-    if (s) return s;
-    tc_.base = pb + L.f16_off;
-  }
-  int s0 = tc_prepare_launch(dev);
-  if (s0) return s0;
-  DevStatus* sd = nullptr;
-  s0 = tc_status_record(dev, &sd);
-  if (s0) return s0;
-  if (sd->code != 0) return RECMV_E_DEVICE;
-  TcParams prm = {};
-  prm.src.x = ps; prm.src.S = 1;
-  for (int i = 0; i < 12; ++i) prm.pw.w[i] = pe_w[i];
-  prm.bias = (const float*)(pb + L.bias_off);
-  prm.P = P; prm.passes = mode == RECMV_MLP_TC_F16X3 ? 3 : 1; prm.status = sd; prm.dbg_layer = -1;
-  set_acc_scales(prm);
-  prm.conds = conds; prm.batch_inds = (const long long*)batch_inds; prm.points_per_frame = points_per_frame;
-  prm.num_frames = num_frames; prm.bones = A; prm.trans = trans;
-  if (vox) prm.vox = to_voxel(vox);
-  prm.out_translated = out_translated; prm.out_offset = out_offset; prm.out_posed = out_posed; prm.out_jac = out_jac;
-  const int grid = tc_grid(P, out_jac ? kRowsPerCta / 4 : kRowsPerCta);   // forward mode: 4 rows per point
-  if (out_jac)
-    tc_launch<true, 1>(grid, st, tc_.m128, prm);
-  else
-    tc_launch<false, 1>(grid, st, tc_.m128, prm);
-  return launch_status();
-}
-
 // ---------------------------------------------------------------------------------------------------------
 // Colour network: RenderingNetwork_view_norm, mode 'idr' (model/RenderNet.py:59-96)
 // ---------------------------------------------------------------------------------------------------------
-namespace recmv {
-namespace {
-constexpr int kRgbLayers = 5, kRgbPanels = 37;
-constexpr int rgb_in(int l) { return l == 0 ? 289 : 512; }
-constexpr int rgb_out(int l) { return l == 4 ? 3 : 512; }
-constexpr int rgb_pbase(int l) { return l == 0 ? 0 : 5 + 8 * (l - 1); }
-constexpr int rgb_npanels(int l) { return l == 0 ? 5 : 8; }
-DeformLayout rgb_layout() {
-  DeformLayout L;
-  L.bias_off = 0;
-  L.f16_off = ((size_t)kRgbLayers * 512 * 4 + 1023) & ~(size_t)1023;
-  L.total = L.f16_off + (size_t)2 * kRgbPanels * 512 * 64 * 2;
-  return L;
-}
-TmapCacheEntry g_rgb_tmap[16];
-}  // namespace
-}  // namespace recmv
-
-extern "C" size_t recmv_rendernet_packed_bytes(void) { return rgb_layout().total; }
-
-extern "C" int recmv_rendernet_pack_weights(const float* W_all, const float* b_all, void* packed,
-                                            recmv_stream_t stream) {
-  if (!W_all || !b_all || !packed) return RECMV_E_NULL;
-  if (((uintptr_t)packed & 1023) != 0) return RECMV_E_SHAPE;
-  DeformLayout L = rgb_layout();
-  char* base = (char*)packed;
-  size_t woff = 0, boff = 0;
-  void* sd = nullptr;
-  int s0 = device_status_record(&sd);
-  if (s0) return s0;
-  for (int l = 0; l < kRgbLayers; ++l) {
-    pack_plain_layer_kernel<<<stride_grid((int64_t)rgb_npanels(l) * 512 * 64, 256, 4), 256, 0, (cudaStream_t)stream>>>(
-        W_all + woff, b_all + boff, rgb_out(l), rgb_in(l), rgb_pbase(l), rgb_npanels(l),
-        (float*)(base + L.bias_off) + l * 512, (__half*)(base + L.f16_off), kRgbPanels, (DevStatus*)sd);
-    int s = launch_status();
-    if (s) return s;
-    woff += (size_t)rgb_in(l) * rgb_out(l);
-    boff += rgb_out(l);
-  }
-  return RECMV_OK;
-}
-
 extern "C" int recmv_rendernet_fwd(const float* points, const float* normals, const float* view_dirs,
                                    const float* feats, const void* packed, const float* pe_w, float* out_rgb,
                                    int64_t P, int mode, recmv_stream_t stream) {
   if (P < 0) return RECMV_E_SHAPE;
   if (P == 0) return RECMV_OK;
   if (!points || !normals || !view_dirs || !feats || !packed || !pe_w || !out_rgb) return RECMV_E_NULL;
-  if (mode != RECMV_MLP_TC_F16X3 && mode != RECMV_MLP_TC_F16X1) return RECMV_E_UNSUPPORTED;
-  cudaStream_t st = (cudaStream_t)stream;
-  int dev = 0;
-  cudaGetDevice(&dev);
-  DeformLayout L = rgb_layout();
-  const char* pb = (const char*)packed;
-  TmapCacheEntry& tc_ = g_rgb_tmap[dev & 15];
-  if (tc_.base != pb + L.f16_off) {
-    int s = make_panel_tmap(&tc_.m128, pb + L.f16_off, (uint64_t)2 * kRgbPanels * 512, 128);
-    if (s) return s;
-    tc_.base = pb + L.f16_off;
-  }
-  int s0 = tc_prepare_launch(dev);
-  if (s0) return s0;
-  DevStatus* sd = nullptr;
-  s0 = tc_status_record(dev, &sd);
-  if (s0) return s0;
-  if (sd->code != 0) return RECMV_E_DEVICE;
+  const int passes = tc_passes(mode);
+  if (!passes) return RECMV_E_UNSUPPORTED;
   TcParams prm = {};
-  prm.src.x = points; prm.src.S = 1;
-  for (int i = 0; i < 12; ++i) prm.pw.w[i] = i < 8 ? pe_w[i] : 0.f;
-  prm.bias = (const float*)(pb + L.bias_off);
-  prm.P = P; prm.passes = mode == RECMV_MLP_TC_F16X3 ? 3 : 1; prm.status = sd; prm.dbg_layer = -1;
-  set_acc_scales(prm);
+  prm.src.x = points; prm.src.S = 1; prm.pw = pe_weights(pe_w, 4); prm.dbg_layer = -1;
   prm.normals = normals; prm.view_dirs = view_dirs; prm.feats = feats; prm.out_rgb = out_rgb;
-  tc_launch<false, 2>(tc_grid(P, kRowsPerCta), st, tc_.m128, prm);
-  return launch_status();
+  return tc_launch<false, 2>(packed, prm, passes, P, (cudaStream_t)stream);
 }
 
 // Diagnostics / calibration: relative gain per 64-wide K block applied to the raw accumulators of a precision mode
 // (RECMV_MLP_TC_F16X3 or RECMV_MLP_TC_F16X1) to compensate the tensor core's truncating accumulation.
 extern "C" int recmv_tc_set_acc_gain(int mode, float gain_per_kblock) {
-  if (mode != RECMV_MLP_TC_F16X3 && mode != RECMV_MLP_TC_F16X1) return RECMV_E_DTYPE;
+  const int passes = tc_passes(mode);
+  if (!passes) return RECMV_E_DTYPE;
   if (!(fabsf(gain_per_kblock) < 1e-4f)) return RECMV_E_RANGE;
-  g_acc_gain_kb[mode == RECMV_MLP_TC_F16X3 ? 0 : 1] = gain_per_kblock;
+  g_acc_gain_kb[passes == 3 ? 0 : 1] = gain_per_kblock;
   return RECMV_OK;
 }
 
@@ -1126,13 +983,12 @@ extern "C" int recmv_sdf_mlp_tc_debug(const float* x, const void* packed, const 
                                       int* status_host, recmv_stream_t stream) {
   if (P <= 0) return RECMV_E_SHAPE;
   if (!x || !packed || !pe_w || !out_sdf || !status_host) return RECMV_E_NULL;
-  PointSource src = {};
-  src.x = x;
-  src.S = 1;
-  PeWeights pw;
-  for (int i = 0; i < 12; ++i) pw.w[i] = pe_w[i];
-  return launch_tc(src, packed, pw, out_sdf, out_feat, nullptr, P, passes, dbg_layer, dbg_out, status_host,
-                   (cudaStream_t)stream);
+  if (passes != 1 && passes != 3) return RECMV_E_DTYPE;
+  TcParams prm = {};
+  prm.src.x = x; prm.src.S = 1; prm.pw = pe_weights(pe_w); prm.out_sdf = out_sdf; prm.out_feat = out_feat;
+  prm.dbg_layer = dbg_layer; prm.dbg_out = dbg_out;
+  prm.last_tiles = (out_feat || (dbg_out && dbg_layer == Net<0>::kLayers - 1)) ? 3 : 1;
+  return tc_launch<false, 0>(packed, prm, passes, P, (cudaStream_t)stream, status_host);
 }
 
 #if RECMV_TC_STALL_PROF

@@ -88,7 +88,7 @@ extern "C" int recmv_surface_solve(const float* cam_pos, const float* rays, floa
       !workspace || !ok)
     return RECMV_E_NULL;
   if (workspace_bytes < recmv_surface_solve_workspace(P)) return RECMV_E_SHAPE;
-  if (mode != RECMV_MLP_TC_F16X3 && mode != RECMV_MLP_TC_F16X1) return RECMV_E_UNSUPPORTED;
+  if (!tc_passes(mode)) return RECMV_E_UNSUPPORTED;
   cudaStream_t st = (cudaStream_t)stream;
   const SolveWs w = carve(workspace, solve_layout, P);
   cudaError_t e = cudaMemsetAsync(ok, 0, (size_t)P, st);

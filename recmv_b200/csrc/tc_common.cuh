@@ -228,14 +228,13 @@ __device__ __forceinline__ void st_shared_b32(uint32_t addr, uint32_t v) {
   asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
 }
 
-// ---- host: tensor map over the fp16 weight panels -------------------------------------------------------
-// 2-D tensor [rows, 64] fp16 (128-byte rows), box [32 x box_rows] (half a row: inputs 0..31 or 32..63 of a panel),
-// 64-byte swizzle -- the layout smem_desc_sw64 describes.
+// ---- host: tensor maps ------------------------------------------------------------------------------------
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
-inline int make_panel_tmap(CUtensorMap* out, const void* base, uint64_t rows, uint32_t box_rows) {
+// the driver's cuTensorMapEncodeTiled, looked up once
+inline int tensor_map_encoder(EncodeTiledFn* out) {
   static EncodeTiledFn fn = nullptr;
   if (!fn) {
     cudaDriverEntryPointQueryResult q;
@@ -244,6 +243,16 @@ inline int make_panel_tmap(CUtensorMap* out, const void* base, uint64_t rows, ui
     if (e != cudaSuccess || !p) return e != cudaSuccess ? (int)e : (int)cudaErrorNotSupported;
     fn = (EncodeTiledFn)p;
   }
+  *out = fn;
+  return 0;
+}
+
+// The fp16 weight panels: 2-D tensor [rows, 64] fp16 (128-byte rows), box [32 x box_rows] (half a row: inputs 0..31
+// or 32..63 of a panel), 64-byte swizzle -- the layout smem_desc_sw64 describes.
+inline int make_panel_tmap(CUtensorMap* out, const void* base, uint64_t rows, uint32_t box_rows) {
+  EncodeTiledFn fn = nullptr;
+  int s = tensor_map_encoder(&fn);
+  if (s) return s;
   cuuint64_t dims[2] = {64, rows};
   cuuint64_t strides[1] = {128};
   cuuint32_t box[2] = {32, box_rows};
