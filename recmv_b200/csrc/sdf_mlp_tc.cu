@@ -19,6 +19,8 @@
 //  * the same engine runs three networks (Net<0> SDF, Net<1> translator + LBS, Net<2> colour) and a forward-mode
 //    (value + tangents, 4 rows per point) variant of the first two.
 // Every mbarrier wait is bounded: a protocol bug surfaces as a status code, not a hung GPU.
+#include <type_traits>
+
 #include "sdf_mlp.cuh"
 #include "tc_common.cuh"
 #include "../../include/recmv_b200_diag.h"   // recmv_sdf_mlp_tc_debug (diagnostics entry, not in the product header)
@@ -81,8 +83,12 @@ constexpr int kBarPeFree = 21;   //       the MMAs of layer kInFreeLayer are don
 constexpr int kNumBars = 22;
 constexpr int kBarConsumers = 1; // named barrier of the 256 MMA threads
 constexpr uint32_t kOffMisc = kOffBar + kNumBars * 8;  // abort flag, valid flags
-constexpr uint32_t kOffProf = kOffMisc + 16 + 128;     // diagnostics build: [4 roles][kStCounters] u64
+// SDF forward: warpgroup 1's share of each row's sdf sum, [64] fp32.  One buffer is enough: warpgroup 0 reads it before
+// the next tile's layer-0 named barriers, and warpgroup 1 writes it again only in the next tile's layer 7.
+constexpr uint32_t kOffSdfPart = kOffMisc + 16 + 128;
+constexpr uint32_t kOffProf = kOffSdfPart + 64 * 4;    // diagnostics build: [4 roles][kStCounters] u64
 constexpr uint32_t kSmemBytes = kOffProf + (kStallProf ? 4 * kStCounters * 8 : 0) + 1024 /*alignment slack*/;
+static_assert(kSmemBytes <= 227 * 1024, "shared memory: within the per-block opt-in");
 #if RECMV_TC_STALL_PROF
 __device__ unsigned long long g_tc_stall[kStCounters];   // read and cleared by recmv_tc_stall_profile
 #endif
@@ -120,7 +126,12 @@ struct TcParams {
   const float* view_dirs;        // [P,3]
   const float* feats;            // [P,256]
   float* out_rgb;                // [P,3]
-  int last_tiles;                // SDF network: 128-wide output tiles of the last layer (3: sdf + features, 1: sdf only)
+  // SDF network: 128-wide output tiles of the last layer, 3 with features.  Without them: 0 for the plain forward in
+  // parity mode (its sdf comes from layer 7's epilogue either way), otherwise 1 (tile 0 holds the sdf).
+  int last_tiles;
+  // SDF network: layer 8's weight row n = 0 (the sdf column) in the hi plane of the panels, [8 panels][512 n][64 k]
+  // apart; the lo plane lies kPanels * 512 * 64 halves further
+  const __half* sdf_w;
 };
 
 // softplus(beta=100, threshold=20) * kActScale straight from the raw accumulator, in base 2:
@@ -213,6 +224,9 @@ __global__ void __launch_bounds__(kThreads, 1)
 sdf_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams prm) {
   using NetT = Net<kNet>;
   constexpr int kNumLayers = NetT::kLayers;
+  constexpr bool kSdfFwd = !kJvp && kNet == 0;   // the SDF network's plain forward
+  // parity mode: the sdf column is folded into layer 7's epilogue (tc1 keeps it on the tensor cores: DESIGN.md section 5)
+  constexpr bool kFoldSdf = kSdfFwd && kPasses == 3;
   static_assert(!kJvp || kNet == 0 || kNet == 1, "the forward-mode variant exists for the SDF network and the deformer");
   static_assert(kPasses == 1 || kPasses == 3, "precision mode");
   extern __shared__ uint8_t smem_raw[];
@@ -316,6 +330,7 @@ sdf_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams prm) {
           stall_add(stall, signaller, kStPeReady, t0);
         }
         const int nkb = NetT::nkb(l), T = NetT::ntiles(l, prm.last_tiles), nt_own = own_tiles(T, g);
+        if (kFoldSdf && T == 0) continue;   // the last layer without features: the producers stream nothing for it
         const bool hidden = l < kNumLayers - 1;
         const bool two_sweeps = kTwoSweeps && kPasses == 3 && l == kNumLayers - 1;
         // the layer's first MMA overwrites the accumulators; zeroing them here tells the compiler that the previous
@@ -378,61 +393,118 @@ sdf_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams prm) {
           named_sync(kBarConsumers, 256);   // both warpgroups are done reading the layer input: overwrite it in place
           stall_add(stall, signaller, kStNamedBar, t_ep);
           t_ep = stall_now();
-          const float* bsel = (!kJvp && kNet == 0) ? bias + kNumLayers * 512 : bias;   // SDF: the b * 100 log2 e plane
+          const float* bsel = kSdfFwd ? bias + kNumLayers * 512 : bias;   // SDF: the b * 100 log2 e plane
+          // SDF forward, layer 7: the sdf column of layer 8, sum_k v_k w_k over this thread's columns per fragment row
+          float sdf_part[2] = {0.f, 0.f};
           // The loop body holds no per-element branch: an operand beyond fp16's range is reported once per layer (same tag),
           // the diagnostics dump branches once per column group, and the activation stores are plain C++ stores (no asm
           // memory clobber), so ptxas can overlap the bias loads and MUFU chains of neighbouring elements.  The epilogue
-          // runs with two warps per scheduler and is latency-bound.
-          bool out_of_range = false;
+          // runs with two warps per scheduler and is latency-bound.  A pass either writes the activation planes (the next
+          // layer's input) or, kFold, sums the sdf column into sdf_part; the choice is made once per layer.  Both in one
+          // pass would hold the weight pairs and row sums next to the stores' operands, and that spills in the SDF
+          // kernels at 200 registers.  The fold pass dumps before its loop, which then has no branch at all: ptxas can
+          // issue the weight loads of later column groups early (DESIGN.md section 9 has the measurement).
+          auto epilogue = [&](auto fold) {
+            constexpr bool kFold = decltype(fold)::value;
+            bool out_of_range = false;
+            if (kFold && prm.dbg_out && prm.dbg_layer == l && tile == 0) {
 #pragma unroll
-          for (int t = 0; t < 2; ++t) {
-            const int f_base = (2 * g + t) * 128 + 2 * c;
-            // column pair j outer, fragment row h inner: each bias pair is used as soon as it is loaded (the other order
-            // keeps a tile's 16 bias pairs live next to the 128 accumulator registers)
+              for (int t = 0; t < 2; ++t)
 #pragma unroll
-            for (int j = 0; j < 16; ++j) {
-              const int f = f_base + 8 * j;
-              if (prm.dbg_out && prm.dbg_layer == l && tile == 0) {
+                for (int i = 0; i < 64; ++i)
+                  prm.dbg_out[(16 * wq + (lane >> 2) + 8 * ((i >> 1) & 1)) * 512 + (2 * g + t) * 128 + 8 * (i >> 2) +
+                              2 * c + (i & 1)] = acc[t][i] * kAccUnscale;
+            }
 #pragma unroll
-                for (int i = 0; i < 4; ++i)
-                  prm.dbg_out[(16 * wq + (lane >> 2) + 8 * (i >> 1)) * 512 + f + (i & 1)] = acc[t][4 * j + i] * kAccUnscale;
-              }
+            for (int t = 0; t < 2; ++t) {
+              const int f_base = (2 * g + t) * 128 + 2 * c;
+              // column pair j outer, fragment row h inner: each bias pair is used as soon as it is loaded (the other order
+              // keeps a tile's 16 bias pairs live next to the 128 accumulator registers)
 #pragma unroll
-              for (int h = 0; h < 2; ++h) {
-                const int row = 16 * wq + (lane >> 2) + 8 * h;
-                const float r0 = acc[t][4 * j + 2 * h];
-                const float r1 = acc[t][4 * j + 2 * h + 1];
-                const float2 bb = __ldg(reinterpret_cast<const float2*>(bsel + f));
-                float v0, v1;
-                if (!kJvp && kNet == 0) {
-                  v0 = softplus100_scaled(r0, bb.x, acc_u1);
-                  v1 = softplus100_scaled(r1, bb.y, acc_u1);
-                } else if (!kJvp) {
-                  v0 = fmaxf(fmaf(r0, acc_unscale, bb.x), 0.f) * kActScale;   // ReLU (deformer, colour)
-                  v1 = fmaxf(fmaf(r1, acc_unscale, bb.y), 0.f) * kActScale;
-                } else {
-                  const float z0 = is_value ? fmaf(r0, acc_unscale, bb.x) : r0 * acc_unscale;   // tangents: no bias
-                  const float z1 = is_value ? fmaf(r1, acc_unscale, bb.y) : r1 * acc_unscale;
-                  const float zv0 = __shfl_sync(0xffffffffu, z0, lane & ~12);   // the point's value row
-                  const float zv1 = __shfl_sync(0xffffffffu, z1, lane & ~12);
-                  v0 = (kNet == 0 ? act_jvp(z0, zv0, is_value) : (zv0 > 0.f ? z0 : 0.f)) * kActScale;
-                  v1 = (kNet == 0 ? act_jvp(z1, zv1, is_value) : (zv1 > 0.f ? z1 : 0.f)) * kActScale;
+              for (int j = 0; j < 16; ++j) {
+                const int f = f_base + 8 * j;
+                if (!kFold && prm.dbg_out && prm.dbg_layer == l && tile == 0) {
+#pragma unroll
+                  for (int i = 0; i < 4; ++i)
+                    prm.dbg_out[(16 * wq + (lane >> 2) + 8 * (i >> 1)) * 512 + f + (i & 1)] = acc[t][4 * j + i] * kAccUnscale;
                 }
-                out_of_range |= !(fmaxf(fabsf(v0), fabsf(v1)) < 65504.f);
-                uint32_t hi, lo;
-                split2(v0, v1, hi, lo);
-                const uint32_t off = (uint32_t)(f >> 6) * 8192u + sw128_elem(row, f & 63);
-                *reinterpret_cast<uint32_t*>(gbase + kOffAHi + off) = hi;
-                if (kPasses == 3) *reinterpret_cast<uint32_t*>(gbase + kOffALo + off) = lo;
+                float2 w = make_float2(0.f, 0.f);   // layer 8's weights of columns f, f + 1 into the sdf: hi + lo
+                if (kFold) {
+                  const __half* wp = prm.sdf_w + (f >> 6) * (512 * 64) + (f & 63);
+                  const float2 w_hi = __half22float2(__ldg(reinterpret_cast<const __half2*>(wp)));
+                  const float2 w_lo = __half22float2(__ldg(reinterpret_cast<const __half2*>(wp + NetT::kPanels * 512 * 64)));
+                  w = make_float2(w_hi.x + w_lo.x, w_hi.y + w_lo.y);
+                }
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                  const int row = 16 * wq + (lane >> 2) + 8 * h;
+                  const float r0 = acc[t][4 * j + 2 * h];
+                  const float r1 = acc[t][4 * j + 2 * h + 1];
+                  const float2 bb = __ldg(reinterpret_cast<const float2*>(bsel + f));
+                  float v0, v1;
+                  if (kSdfFwd) {
+                    v0 = softplus100_scaled(r0, bb.x, acc_u1);
+                    v1 = softplus100_scaled(r1, bb.y, acc_u1);
+                  } else if (!kJvp) {
+                    v0 = fmaxf(fmaf(r0, acc_unscale, bb.x), 0.f) * kActScale;   // ReLU (deformer, colour)
+                    v1 = fmaxf(fmaf(r1, acc_unscale, bb.y), 0.f) * kActScale;
+                  } else {
+                    const float z0 = is_value ? fmaf(r0, acc_unscale, bb.x) : r0 * acc_unscale;   // tangents: no bias
+                    const float z1 = is_value ? fmaf(r1, acc_unscale, bb.y) : r1 * acc_unscale;
+                    const float zv0 = __shfl_sync(0xffffffffu, z0, lane & ~12);   // the point's value row
+                    const float zv1 = __shfl_sync(0xffffffffu, z1, lane & ~12);
+                    v0 = (kNet == 0 ? act_jvp(z0, zv0, is_value) : (zv0 > 0.f ? z0 : 0.f)) * kActScale;
+                    v1 = (kNet == 0 ? act_jvp(z1, zv1, is_value) : (zv1 > 0.f ? z1 : 0.f)) * kActScale;
+                  }
+                  if (kFold) {
+                    sdf_part[h] = fmaf(v0, w.x, sdf_part[h]);
+                    sdf_part[h] = fmaf(v1, w.y, sdf_part[h]);
+                  } else {
+                    out_of_range |= !(fmaxf(fabsf(v0), fabsf(v1)) < 65504.f);
+                    uint32_t hi, lo;
+                    split2(v0, v1, hi, lo);
+                    const uint32_t off = (uint32_t)(f >> 6) * 8192u + sw128_elem(row, f & 63);
+                    *reinterpret_cast<uint32_t*>(gbase + kOffAHi + off) = hi;
+                    if (kPasses == 3) *reinterpret_cast<uint32_t*>(gbase + kOffALo + off) = lo;
+                  }
+                }
               }
             }
+            if (out_of_range) report_range(prm.status, 1000 + l);
+          };
+          const bool fold = kFoldSdf && l == kNumLayers - 2;
+          // layer 7 of the SDF forward writes its output only for the features of layer 8
+          if (!fold || prm.last_tiles > 0) epilogue(std::false_type{});
+          if constexpr (kFoldSdf) {   // the fold pass is instantiated in these kernels only
+            if (fold) epilogue(std::true_type{});
           }
-          if (out_of_range) report_range(prm.status, 1000 + l);
+          if (kFoldSdf && fold) {
+            // the row sums over the quad's four column pairs, then warpgroup 1 hands its share to warpgroup 0
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              sdf_part[h] += __shfl_xor_sync(0xffffffffu, sdf_part[h], 1);
+              sdf_part[h] += __shfl_xor_sync(0xffffffffu, sdf_part[h], 2);
+              if (g == 1 && c == 0)
+                reinterpret_cast<float*>(gbase + kOffSdfPart)[16 * wq + (lane >> 2) + 8 * h] = sdf_part[h];
+            }
+          }
           fence_proxy_async();
           stall_add(stall, signaller, kStEpilogue, t_ep);
           t_ep = stall_now();
-          named_sync(kBarConsumers, 256);   // the next layer's input is complete
+          named_sync(kBarConsumers, 256);   // the next layer's input (SDF, layer 7: warpgroup 1's sdf sums) is complete
           stall_add(stall, signaller, kStNamedBar, t_ep);
+          if (kFoldSdf && fold && g == 0 && c == 0) {
+            // sdf = (s0 + s1) 2^-16 + b8[0]: both scales of the operands undone, the last layer's bias added
+            const float b8 = __ldg(prm.bias + (kNumLayers - 1) * 512);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int row = 16 * wq + (lane >> 2) + 8 * h;
+              const long long p = tile * kPtsPerTile + row;
+              const float s1 = reinterpret_cast<const float*>(gbase + kOffSdfPart)[row];
+              if (p < Ptot)
+                prm.out_sdf[p] = valid[(it & 1) * 64 + row] != 0 ? fmaf(sdf_part[h] + s1, kAccUnscale, b8) : kInvalidSdf;
+            }
+          }
           continue;
         }
         // ---- last layer ----
@@ -453,11 +525,11 @@ sdf_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams prm) {
                   const int f = (2 * g + t) * 128 + 8 * j + 2 * c + e;
                   const float r = acc[t][4 * j + 2 * h + e];
                   if (prm.dbg_out && prm.dbg_layer == l && tile == 0) prm.dbg_out[row * 512 + f] = r * kAccUnscale;
-                  // column 0 = sdf, columns 1..256 = features
+                  // column 0 = sdf (kFoldSdf: stored from layer 7's epilogue), columns 1..256 = features
                   if (kJvp && !is_value) {
                     if (f == 0) prm.out_grad[p * 3 + (comp - 1)] = r * acc_unscale;
                   } else if (f == 0) {
-                    prm.out_sdf[p] = ok ? fmaf(r, acc_unscale, __ldg(bias)) : kInvalidSdf;
+                    if (!kFoldSdf) prm.out_sdf[p] = ok ? fmaf(r, acc_unscale, __ldg(bias)) : kInvalidSdf;
                   } else if (f <= 256 && prm.out_feat) {
                     prm.out_feat[p * 256 + (f - 1)] = fmaf(r, acc_unscale, __ldg(bias + f));
                   }
@@ -833,6 +905,7 @@ int tc_launch(const void* packed, TcParams prm, int passes, int64_t P, cudaStrea
   if (s) return s;
   if (sd->code != 0) return RECMV_E_DEVICE;  // a previous launch on this device aborted
   prm.bias = blob.bias;
+  if (kNet == 0) prm.sdf_w = blob.panels + (size_t)Net<0>::pbase(Net<0>::kLayers - 1) * 512 * 64;
   prm.P = P;
   prm.passes = passes;
   prm.acc_gain_kb = g_acc_gain_kb[passes == 3 ? 0 : 1];
@@ -855,12 +928,13 @@ int tc_launch(const void* packed, TcParams prm, int passes, int64_t P, cudaStrea
 }
 }  // namespace
 
-// SDF network.  The last layer's output tiles 1 and 2 hold features only: computed when someone reads them.
+// SDF network.  In parity mode layer 7's epilogue computes the sdf and the last layer runs only when someone reads the
+// features; in tc1 the last layer's tile 0 computes it.
 int tc_sdf_forward(const PointSource& src, const void* packed, const PeWeights& pw, float* out_sdf,
                    float* out_feat, int64_t P, int passes, cudaStream_t st, const int* P_dev) {
   TcParams prm = {};
   prm.src = src; prm.pw = pw; prm.out_sdf = out_sdf; prm.out_feat = out_feat; prm.P_dev = P_dev; prm.dbg_layer = -1;
-  prm.last_tiles = out_feat ? 3 : 1;
+  prm.last_tiles = out_feat ? 3 : (passes == 3 ? 0 : 1);
   return tc_launch<false, 0>(packed, prm, passes, P, st);
 }
 
@@ -987,7 +1061,7 @@ extern "C" int recmv_sdf_mlp_tc_debug(const float* x, const void* packed, const 
   TcParams prm = {};
   prm.src.x = x; prm.src.S = 1; prm.pw = pe_weights(pe_w); prm.out_sdf = out_sdf; prm.out_feat = out_feat;
   prm.dbg_layer = dbg_layer; prm.dbg_out = dbg_out;
-  prm.last_tiles = (out_feat || (dbg_out && dbg_layer == Net<0>::kLayers - 1)) ? 3 : 1;
+  prm.last_tiles = (out_feat || (dbg_out && dbg_layer == Net<0>::kLayers - 1)) ? 3 : (passes == 3 ? 0 : 1);
   return tc_launch<false, 0>(packed, prm, passes, P, (cudaStream_t)stream, status_host);
 }
 
